@@ -14,8 +14,7 @@ globally seeded batch, no data-path collective -- SURVEY 8e).  Rank 0 prints ONE
                    D2H of the images, every step
   roofline         the WHOLE attention path of the step (batched stage I + every layer call): ALGORITHMIC bytes (read X once +
                    write X' once per layer, SURVEY 8d) / CUDA-event time, vs MEASURED_PEAKS.json hbm_gbs; stage_T = the
-                   dominant kernel alone; traffic = DRAM bytes of the largest stage-T launch parsed from the tracked
-                   profiles/r02/traffic_config<N>.csv (tools/traffic_capture.sh, ncu on the current build)
+                   dominant kernel alone
   roofline_conv    row f1: the library's own 3x3 convolution kernel against the tensor roofline (TFLOP/s, measured bf16 peak / 2)
   roofline_duplex  BASELINE's second named metric: the 12 duplex layer calls of configs[2] (K=32, batch 64), same formula
   train_step       BASELINE configs[3]: G+D training step, data-parallel with the NCCL gradient all-reduce, at every N
@@ -68,13 +67,13 @@ def measured_peak_gbs():
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json, burst copy)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md)"
+        return 3350.0, "fallback (H100 SXM data sheet, HBM3)"
 
 
 def conv_roofline_probe(device, iters: int = 5):
     """Row f1 kernel against the tensor roofline: the five stride-1 3x3 convolutions of the 256x256 generator (batch 32) on the library's
-    own tcgen05 implicit-GEMM kernel, each layer timed on its own with CUDA events after warm-up (inputs 67 MB ... 1.07 GB, alternating
-    between two buffers).  FLOPs = 2 * 9 * B * H * W * Cin * Cout.  Peak = measured cuBLAS bf16 throughput / 2 (kind::tf32 runs at half
+    own wgmma implicit-GEMM kernel, each layer timed on its own with CUDA events after warm-up (inputs 67 MB ... 1.07 GB, alternating
+    between two buffers).  FLOPs = 2 * 9 * B * H * W * Cin * Cout.  Peak = measured cuBLAS bf16 throughput / 2 (tf32 runs at half
     the bf16 rate)."""
     from importlib import import_module
     ops = import_module("gansformer-reproducibility-challenge_b200.ops")
@@ -83,7 +82,7 @@ def conv_roofline_probe(device, iters: int = 5):
             pk = json.load(f)
         peak, src = float(pk["bf16_tflops"]) / 2, "measured cuBLAS bf16 burst (MEASURED_PEAKS.json) / 2"
     except Exception:
-        peak, src = 1125.0, "nominal dense TF32 (2250 bf16 / 2)"
+        peak, src = 495.0, "H100 SXM data sheet, dense TF32"
     B = 32
     layers, tot_flop, tot_ms = [], 0.0, 0.0
     for res, C in [(16, 512), (32, 512), (64, 512), (128, 256), (256, 128)]:
@@ -107,12 +106,12 @@ def conv_roofline_probe(device, iters: int = 5):
     torch.cuda.empty_cache()
     ach = tot_flop / tot_ms / 1e9
     return {"bound": "tensor", "achieved": ach, "peak": peak, "unit": "TFLOP/s", "frac": ach / peak, "traffic": None, "peak_source": src,
-            "kernel": "conv3x3_tc_kernel / conv3x3_tc_kernel_v2 (gf_conv3x3_nhwc_tf32): the five stride-1 3x3 convolutions of the step, "
+            "kernel": "conv3x3_tc_kernel (gf_conv3x3_nhwc_tf32): the five stride-1 3x3 convolutions of the step, "
                       "timed layer by layer outside the step", "ms_total": tot_ms, "layers": layers}
 
 
 class ClockSampler:
-    """nvidia-smi clocks/throttle reasons DURING the timed region (recipe in B200_PROFILING.md)."""
+    """nvidia-smi clocks/throttle reasons DURING the timed region."""
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -173,7 +172,7 @@ def cpu_threads() -> int:
 
 
 def cpu_oracle_run(G_state, steps: int, warmup: int, sample_b: int, duplex: bool = None):
-    """Times the CPU oracle generator (fp32, NCHW, direct op order) on `sample_b` images per step: median of `steps` (>= 3)."""
+    """Times the CPU oracle generator (fp32, NCHW, direct op order) on `sample_b` images per step: median of `steps` timed steps."""
     from oracle import generator as og
     threads = cpu_threads()
     torch.set_num_threads(threads)
@@ -236,8 +235,7 @@ def duplex_attention_probe(device, peak_gbs: float, iters: int = 6):
             "ms": tot_ms, "alg_bytes": tot_bytes, "achieved": achieved,
             "unit": "GB/s", "frac": achieved / peak_gbs, "pass_a_path": cen_path,
             "dram_note": "three passes over X by construction (pass A reads it, stage T reads it again and writes X'): 1.5x the algorithmic "
-                         "bytes; the B200 L2 keeps ~50 MB of a streamed tensor (tools/probes/l2_reuse_probe.cu), less than one 256^2 image + the "
-                         "pipeline depth, so the second read cannot be an L2 hit (DESIGN.md 9.1)"}
+                         "bytes; one 256^2 image of a layer is larger than the 50 MB L2, so the second read cannot be an L2 hit"}
 
 
 def duplex_generator_probe(device, steps: int = 5, warmup: int = 2, B: int = 64, k: int = 32, with_cpu: bool = True):
@@ -343,7 +341,7 @@ def train_probe(device, rank, world, steps: int = 3, warmup: int = 1, B: int = 3
            "peak_mem_gb": torch.cuda.max_memory_allocated(device) / 2 ** 30,
            "cuda_graph": bool(graphed),
            "attention_dropout": 0.12,
-           "backward": "attention: CUDA forward (tcgen05 kernel with Philox attention dropout p = 0.12 on the probabilities) + hand-written stage-T backward kernel "
+           "backward": "attention: CUDA forward (wgmma kernel with Philox attention dropout p = 0.12 on the probabilities) + hand-written stage-T backward kernel "
                        "(gf_attn_simplex_bwd_ex, same mask) + batched GEMMs for the token reductions; FIR filters: native (self-adjoint) "
                        "kernel; convolutions / discriminator: cuDNN; gradients: bucketed NCCL all-reduce overlapped with backward"}
     del trainer, G, D
@@ -354,7 +352,7 @@ def train_probe(device, rank, world, steps: int = 3, warmup: int = 1, B: int = 3
 def run_reference(args):
     """The reference arm: the reference's own implementation cannot be installed or run (no source under /root/reference,
     TensorFlow 1.14 unavailable), so per the tier contract this times the CPU oracle port on the host cores: pinned thread
-    count, median of >= 3 steps of a bounded sample (2 images per step; config 1: its exact batch of 4)."""
+    count, median of --steps timed steps of a bounded sample (2 images per step; config 1: its exact batch of 4)."""
     rank = int(os.environ.get("RANK", 0))
     if rank != 0:
         return 0
@@ -363,7 +361,7 @@ def run_reference(args):
     import gansformer_b200 as gf
     G = gf.Generator(resolution=RES, components_num=K_LATENTS, latent_dim=LATENT_DIM, kmeans=DUPLEX)
     sample_b = B_PER_GPU if args.config == 1 else (1 if RES >= 512 else 2)
-    steps, warmup = max(3, min(args.steps, 5)), 1
+    steps, warmup = args.steps, args.warmup
     ips, t, cores = cpu_oracle_run(G.state_dict(), steps, warmup, sample_b)
     line = {"impl": "reference", "metric": METRIC, "value": ips, "unit": UNIT, "n_gpus": args.gpus, "steps": steps, "warmup": warmup,
             "ms_per_step": t * 1e3, "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "f32", "data": "synthetic",
@@ -377,32 +375,13 @@ def run_reference(args):
     return 0
 
 
-def parse_traffic(config_n: int):
-    """roofline.traffic: dram__bytes_read.sum + dram__bytes_write.sum of the dominant launch, read from the TRACKED csv that
-    tools/traffic_capture.sh produced with ncu on the current build (profiles/r02/traffic_config<N>.csv); None if absent."""
-    import csv
-    path = os.path.join(ROOT, "profiles", "r02", f"traffic_config{config_n}.csv")
-    if not os.path.exists(path):
-        return None, None
-    best = None
-    try:
-        with open(path) as f:
-            rows = list(csv.DictReader(l for l in f if not l.startswith("==")))
-        per = {}
-        for r in rows:
-            if not r["Metric Name"].startswith("dram__bytes"):
-                continue
-            v = float(r["Metric Value"].replace(",", "")) * {"byte": 1, "Kbyte": 1e3, "Mbyte": 1e6, "Gbyte": 1e9}[r["Metric Unit"]]
-            e = per.setdefault(r["ID"], {"name": r["Kernel Name"], "bytes": 0.0})
-            e["bytes"] += v
-        for e in per.values():
-            if ("token_tc_kernel" in e["name"] or "token_simt" in e["name"]) and (best is None or e["bytes"] > best["bytes"]):
-                best = e
-    except Exception:
-        return None, None
-    if best is None:
-        return None, None
-    return best["bytes"], f"profiles/r02/traffic_config{config_n}.csv ({best['name'][:60]}: largest stage-T launch of one eager step)"
+def dump_outputs(out_dir: str, arrays: dict):
+    """Writes what the timed step returned to its caller as <out_dir>/<name>.npy (float32), so that two builds can be compared
+    output for output: the inputs (weights seed 0, latents seed 1) are the same in every run with the same arguments."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    for name, t in arrays.items():
+        np.save(os.path.join(out_dir, f"{name}.npy"), t.detach().float().cpu().numpy())
 
 
 def run_ours(args):
@@ -483,14 +462,17 @@ def run_ours(args):
     ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     torch.cuda.profiler.start()              # ncu --profile-from-start off captures exactly the timed steps
     ev0.record()
+    out = None
     for _ in range(args.steps):
-        step_resident()
+        out = step_resident()
     ev1.record()
     torch.cuda.synchronize()
     torch.cuda.profiler.stop()
     dist_mod.barrier()
     clocks = sampler.stop() if rank == 0 else None
     t_total = dist_mod.max_over_ranks(ev0.elapsed_time(ev1) * 1e-3, device)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, {"images": out})
     stage_t_s = sum(r[0].elapsed_time(r[1]) for r in timer.records) * 1e-3
     call_s = sum(r[3].elapsed_time(r[1]) for r in timer.records) * 1e-3 + sum(a.elapsed_time(b) for a, b in timer.batch_records) * 1e-3
     attn_bytes = sum(r[2] for r in timer.records)
@@ -580,15 +562,14 @@ def run_ours(args):
         peak, peak_src = measured_peak_gbs()
         achieved = attn_bytes / call_s / 1e9 if call_s > 0 else 0.0
         achieved_t = attn_bytes / stage_t_s / 1e9 if stage_t_s > 0 else 0.0
-        traffic, traffic_src = parse_traffic(args.config)
         line = {
             "metric": METRIC, "value": world * B * args.steps / t_total, "unit": UNIT, "n_gpus": world, "steps": args.steps,
             "warmup": args.warmup, "ms_per_step": t_total / args.steps * 1e3, "higher_is_better": True, "scaling": "weak",
-            "vs_baseline": None, "dtype": "tf32 (fp32 storage; tcgen05 kind::tf32 attention and stride-1 3x3 convolutions (own kernels), TF32 cuDNN up-convolutions; value_fp32_convs = the same with fp32 cuDNN convolutions)" if path == "tcgen05_tf32" else "f32 (CUDA-core attention; TF32 cuDNN convs)",
+            "vs_baseline": None, "dtype": "tf32 (fp32 storage; wgmma tf32 attention and stride-1 3x3 convolutions (own kernels), TF32 cuDNN up-convolutions; value_fp32_convs = the same with fp32 cuDNN convolutions)" if path == "wgmma_tf32" else "f32 (CUDA-core attention; TF32 cuDNN convs)",
             "data": "synthetic",
             "config": {"workload": cfg["label"] + ", integration=mul, norm=layer, random-init weights (seed 0), latents seed 1",
                        "global_batch": world * B, "parallelism": f"dp{world} (images sharded, no data-path collective)",
-                       "l2_policy": "activations per layer (up to 1.07 GB) exceed the 126 MB L2; no flush needed",
+                       "l2_policy": "activations per layer (up to 1.07 GB) exceed the 50 MB L2; no flush needed",
                        "attention_path": path, "cuda_graph": bool(use_graph)},
             "gpu_launches": int(launches) * args.steps,
             "e2e": {"value": world * B * args.steps / t_e2e, "unit": UNIT, "h2d_bytes_per_step": int(z_host.numel() * 4 * world),
@@ -596,7 +577,6 @@ def run_ours(args):
                     "call": "Generator.run(latents[m*B], minibatch_size=B, cuda_graph=True, out=pinned) over the K steps in calls of m <= 10 minibatches; per minibatch: H2D latents, "
                             "graph replay, D2H images on a copy stream overlapping the next minibatch"},
             "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                         "traffic": traffic, "traffic_source": traffic_src,
                          "peak_source": peak_src,
                          "kernel": f"whole attention path of the step: stage I (one batched launch) + {'pass A + key products + ' if DUPLEX else ''}stage T ({path})",
                          "calls_timed": n_attn_calls, "alg_bytes_per_step": attn_bytes // max(args.steps, 1),
@@ -615,7 +595,7 @@ def run_ours(args):
         if t_cudnn is not None:
             line["value_cudnn_convs"] = {"value": world * B / t_cudnn, "unit": UNIT, "ms_per_step": t_cudnn * 1e3,
                                          "note": "same step with GF_CUDNN_CONV=1: cuDNN TF32 for the five stride-1 3x3 convolutions that otherwise run on "
-                                                 "the library's own tcgen05 implicit-GEMM kernel (gf_conv3x3_nhwc_tf32, SURVEY row f1)"}
+                                                 "the library's own wgmma implicit-GEMM kernel (gf_conv3x3_nhwc_tf32, SURVEY row f1)"}
         state["line"] = line
     if world == 1 and not args.no_duplex_probe and args.config == 2:
         peak, _ = measured_peak_gbs()
@@ -673,7 +653,14 @@ def main():
     ap.add_argument("--no-train-probe", action="store_true", help="skip the BASELINE configs[3] probe (G+D training step, train_step object)")
     ap.add_argument("--train-probe", action="store_true", help="(kept for compatibility: the probe now runs at every N by default)")
     ap.add_argument("--train-timeout", type=float, default=240.0, help="watchdog of the training probe in seconds")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the images of the last timed step as DIR/images.npy (float32); with several "
+                         "GPUs, rank 0's shard of the batch (the first batch / N latents)")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
+    if args.dump_outputs and args.impl == "reference":
+        ap.error("--dump-outputs writes what the GPU implementation computed: it needs --impl ours")
     if args.impl == "ours":
         args.warmup = max(args.warmup, 3)
     rc = run_reference(args) if args.impl == "reference" else run_ours(args)

@@ -1,4 +1,4 @@
-"""B200-native GANsformer bipartite-attention hot path (sm_100a CUDA behind a C ABI) + the generator host code.
+"""GANsformer bipartite-attention hot path for the H100 (sm_90a CUDA behind a C ABI) + the generator host code.
 
 The directory name carries the reference repo's name and is not a Python identifier; import it as
 ``import gansformer_b200`` (alias package at the repo root) or via ``importlib.import_module``.

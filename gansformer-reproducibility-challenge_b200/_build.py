@@ -1,4 +1,4 @@
-"""Ahead-of-time, in-tree build of libgf_attn.so (sm_100a only) with nvcc.
+"""Ahead-of-time, in-tree build of libgf_attn.so (sm_90a only) with nvcc.
 
 The reference JIT-compiles its two custom ops at import time (dnnlib/tflib/custom_ops.py upstream, not in the
 checkout); here the library is built once, in-tree, so the .so travels with the repo snapshot to the GPU box.
@@ -15,7 +15,7 @@ CSRC = PKG_DIR / "csrc"
 LIB_PATH = PKG_DIR / "libgf_attn.so"
 SOURCES = ["gf_api.cu", "gf_fold.cu", "gf_simt.cu", "gf_tc.cu", "gf_tc_cen.cu", "gf_tc_gemm.cu", "gf_bwd.cu", "gf_ops.cu", "gf_conv.cu"]
 COMPILE_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC",
 ]
@@ -68,7 +68,7 @@ def build_extension(force: bool = False, verbose: bool = False) -> Path:
     with ThreadPoolExecutor(max_workers=min(8, max(1, len(jobs)))) as pool:
         logs = list(pool.map(lambda j: _compile_one(nvcc, j[0], j[1], verbose), jobs))
     tag.write_text(flags_now)
-    cmd = [nvcc, "-gencode", "arch=compute_100a,code=sm_100a", "-shared", "-o", str(LIB_PATH)] + [str(objdir / (n[:-3] + ".o")) for n in SOURCES]
+    cmd = [nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-shared", "-o", str(LIB_PATH)] + [str(objdir / (n[:-3] + ".o")) for n in SOURCES]
     res = subprocess.run(cmd, capture_output=True, text=True)
     if res.returncode != 0:
         raise RuntimeError("nvcc link failed:\n" + " ".join(cmd) + "\n" + res.stdout + res.stderr)

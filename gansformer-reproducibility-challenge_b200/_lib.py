@@ -20,7 +20,7 @@ FLAG_CENTROIDS_IN = 2
 FLAG_TABLES_READY = 4
 FLAG_IMG2LTNT = 8
 FLAG_CENTROIDS_INIT = 16
-PATH_NAMES = {0: "none", 1: "simt_fp32", 2: "tcgen05_tf32"}
+PATH_NAMES = {0: "none", 1: "simt_fp32", 2: "wgmma_tf32"}
 
 WEIGHT_FIELDS = ("wq", "bq", "wpq", "wk", "bk", "wpk", "wv", "bv", "wo", "bo", "pos_latent",
                  "wq2", "bq2", "wpq2", "wk2", "bk2", "wpk2", "wv2", "bv2", "wkc", "wcq", "wi2l", "bi2l")

@@ -1,4 +1,4 @@
-"""Host-side mirror of the reference's attention operator, backed by libgf_attn.so (sm_100a kernels).
+"""Host-side mirror of the reference's attention operator, backed by libgf_attn.so (sm_90a kernels).
 
 Reference interface mirrored (expected ``src/training/network.py`` upstream; the file is NOT in the reference
 checkout -- ``/root/reference/.SUBMODULES.json:2`` reports zero payload bytes -- so names/kwargs follow
@@ -302,7 +302,7 @@ def bipartite_attention_forward(x: torch.Tensor, y: torch.Tensor, params: Dict[s
 
 
 def tc_eligible(module: "BipartiteAttention", shape, k: int) -> bool:
-    """Will stage T of this layer call run on the tcgen05 kernel (gf_attn_tc_eligible)?  Decides fusions only that kernel serves."""
+    """Will stage T of this layer call run on the wgmma tensor-core kernel (gf_attn_tc_eligible)?  Decides fusions only that kernel serves."""
     B, H, W, C = shape
     desc = _lib.make_desc(B, H, W, C, k, module.latent_dim, heads=module.num_heads, norm=module.norm, integration=module.integration,
                           pos_dim=module.pos_dim if module.use_pos else 0, duplex=module.kmeans_iters if module.duplex else 0,

@@ -21,7 +21,7 @@ void set_centroid_path(int path) { g_cen_path = path; }
 static std::atomic<long long> g_launches{0};
 void note_launch() { g_launches.fetch_add(1, std::memory_order_relaxed); }
 
-// The library is sm_100a-only: refuse anything else loudly instead of failing at launch.
+// The library is built for sm_90a only: refuse anything else loudly instead of failing at launch.
 int check_device() {
   static thread_local int checked_dev = -1;
   int dev = -1;
@@ -30,8 +30,8 @@ int check_device() {
   int major = 0, minor = 0;
   GF_CUDA_OK(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev));
   GF_CUDA_OK(cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, dev));
-  if (major != 10) {
-    set_error("libgf_attn is built for sm_100a (B200) only; device %d has compute capability %d.%d", dev, major, minor);
+  if (major != 9 || minor != 0) {
+    set_error("libgf_attn is built for sm_90a (H100) only; device %d has compute capability %d.%d", dev, major, minor);
     return GF_ERR_UNSUPPORTED;
   }
   checked_dev = dev;
@@ -78,7 +78,7 @@ static int token_pass(const Layout& L, const gf_attn_desc* d, const float* X, fl
   if (post && (post->rgb_out || post->rgb_w)) {
     if (!post->rgb_out || !post->rgb_w || ((uintptr_t)post->rgb_w & 15)) { set_error("postop: fused tRGB needs rgb_w (16-byte aligned) and rgb_out"); return GF_ERR_INVALID; }
     if (!tc || (L.C > 256 && L.KP > 16)) {
-      set_error("postop: the fused tRGB is served by the tcgen05 path with C <= 256, or C = 512 and k <= 16 (see gf_attn_tc_eligible)");
+      set_error("postop: the fused tRGB is served by the tensor-core path with C <= 256, or C = 512 and k <= 16 (see gf_attn_tc_eligible)");
       return GF_ERR_UNSUPPORTED;
     }
   }
@@ -248,9 +248,9 @@ int gf_attn_duplex_fwd_ex(const gf_attn_desc* desc, const float* X, const float*
     for (int it = 0; it < L.iters; ++it) {
       if ((it > 0 || cen_init) && (rc = duplex_tables_from_centroids(L, desc, cen, Y, folded, ws, st, isc, isc_ld))) return rc;   // queries from the centroids
       if (cen_tc) {
-        if ((rc = centroid_pass_tc(L, desc, X, ws, st, isc, isc_ld))) return rc;
-        if (L.nsplit_cen > 1 && (rc = centroid_merge(L, ws, st, isc, isc_ld))) return rc;   // one split: the kernel wrote Xbar itself
-        set_centroid_path(GF_PATH_TCGEN05_TF32);
+        if ((rc = centroid_pass_tc(L, X, ws, st))) return rc;
+        if ((rc = centroid_merge(L, ws, st, isc, isc_ld))) return rc;
+        set_centroid_path(GF_PATH_WGMMA_TF32);
       } else {
         if ((rc = centroid_pass_simt(L, desc, X, ws, st, isc, isc_ld))) return rc;
         set_centroid_path(GF_PATH_SIMT_FP32);

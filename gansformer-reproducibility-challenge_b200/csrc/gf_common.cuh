@@ -1,4 +1,4 @@
-// gf_common.cuh -- shared host/device definitions for libgf_attn (sm_100a only).
+// gf_common.cuh -- shared host/device definitions for libgf_attn (sm_90a).
 //
 // Buffer layouts are the ones restated in oracle/folded.py (stage W / I / T); keep the two in sync.
 #pragma once
@@ -58,13 +58,13 @@ struct Layout {
   int nsplit_norm, nsplit_cen;
 };
 
-// SM count of the current device (B200: 148), queried once per process; grids and split models are sized from it.
+// SM count of the current device (H100 SXM: 132), queried once per process; grids and split models are sized from it.
 inline int num_sms() {
   static int v = -1;
   if (v < 0) {
     int dev = 0, n = 0;
     if (cudaGetDevice(&dev) == cudaSuccess && cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess && n > 0) v = n;
-    else return 148;          // no device visible (host-only layout queries): the B200 figure, not cached
+    else return 132;          // no device visible (host-only layout queries): the H100 SXM figure, not cached
   }
   return v;
 }
@@ -104,7 +104,7 @@ inline int pad_k(int k) { return k <= 16 ? 16 : 32; }
 
 // Fills L; returns GF_OK or an error (message set).
 int make_layout(const gf_attn_desc* d, Layout* L);
-int check_device();          // GF_OK on a compute-capability-10.x device, an error otherwise (gf_api.cu)
+int check_device();          // GF_OK on a compute-capability-9.0 device, an error otherwise (gf_api.cu)
 
 // ---- stage W / I kernels (gf_fold.cu) ---------------------------------------------------------------
 int fold_weights(const Layout& L, const gf_attn_desc* d, const gf_attn_weights* w, float* folded, cudaStream_t st);
@@ -123,7 +123,8 @@ int duplex_tables(const Layout& L, const gf_attn_desc* d, const float* Y, const 
 int gemm(cudaStream_t st, int M, int N, int K, const float* A, int lda, bool ta, const float* B, int ldb, bool tb,
          float* Cm, int ldc, float alpha, const float* E = nullptr, int lde = 0, int emod = 1, const float* v = nullptr,
          bool allow_tf32 = false);
-// tcgen05 TF32 version for dense row-major operands (gf_tc_gemm.cu); gemm() routes to it when allow_tf32 and the shape fits
+
+// wgmma TF32 version for dense row-major operands (gf_tc_gemm.cu); gemm() routes to it when allow_tf32 and the shape fits
 bool gemm_tc_ok(int M, int N, int K, const float* A, const float* B, const float* Cm, int ldc);
 int gemm_tc(cudaStream_t st, int M, int N, int K, const float* A, const float* B, float* Cm, int ldc, float alpha,
             const float* E, int lde, int emod, const float* v);
@@ -137,12 +138,10 @@ int centroid_pass_simt(const Layout& L, const gf_attn_desc* d, const float* X, f
                        const float* in_scale = nullptr, int in_scale_ld = 0);
 // Xbar = merge of the split partials (times the load-side scale, when given)
 int centroid_merge(const Layout& L, float* ws, cudaStream_t st, const float* in_scale = nullptr, int in_scale_ld = 0);
-// tcgen05 duplex pass A (gf_tc_cen.cu): partials into ws (same format as the CUDA-core kernel), then centroid_merge
+// wgmma duplex pass A (gf_tc_cen.cu): partials into ws (same format as the CUDA-core kernel), merged by centroid_merge
 bool tc_centroid_supported(const Layout& L, const gf_attn_desc* d);
-// in_scale: only used when the split count is 1 and the kernel writes the normalised Xbar itself (no merge kernel)
-int centroid_pass_tc(const Layout& L, const gf_attn_desc* d, const float* X, float* ws, cudaStream_t st,
-                     const float* in_scale = nullptr, int in_scale_ld = 0);
-// tcgen05 / TMA path (gf_tc.cu).  tc_supported() says whether the shape is served by it.
+int centroid_pass_tc(const Layout& L, const float* X, float* ws, cudaStream_t st);
+// wgmma / TMA path (gf_tc.cu).  tc_supported() says whether the shape is served by it.
 bool tc_supported(const Layout& L, const gf_attn_desc* d);
 int token_pass_tc(const Layout& L, const gf_attn_desc* d, const float* X, float* Xout, float* att, float* ws, const gf_attn_postop* post, cudaStream_t st);
 

@@ -85,7 +85,7 @@ int make_layout(const gf_attn_desc* d, Layout* L) {
   int want = (2 * sms + l.B - 1) / l.B;
   l.nsplit_norm = want; if (l.nsplit_norm > (l.n + 63) / 64) l.nsplit_norm = (l.n + 63) / 64; if (l.nsplit_norm < 1) l.nsplit_norm = 1;
   {
-    // centroid splits: one CTA per SM.  Cost model in tile units: every CTA pays a fixed cost (TMEM allocation, loading M,
+    // centroid splits: one CTA per SM.  Cost model in tile units: every CTA pays a fixed cost (barrier set-up, loading M,
     // flushing its [KP, C] partial -- about two tiles' worth) plus its share of the image's tiles, and the grid runs in
     // ceil(CTAs / SMs) rounds.  Small images therefore get ONE split (a 32x32 grid used to be cut into 8 one-tile CTAs, each
     // moving as many bytes of M and partials as of X).
@@ -536,7 +536,7 @@ struct StageIJob {
   float *Kp, *Vt, *Rt, *Ct, *CBout;
   int H, W, C, k, D, p, KP, Cout, LDK, in_ld;
   int heads, seg;                // multi-head: table column J = head * seg + j; A / Cst / AV / CV hold one copy per head
-  int tf32_k, tf32_v;            // round K' (and take the logits in log2 units) / round V^T for the tcgen05 kernels
+  int tf32_k, tf32_v;            // round K' (and take the logits in log2 units) / round V^T for the tensor-core kernels
   int nvblk, npos, nkblk;        // CTAs per image and role
   int blk_begin;                 // first blockIdx.y of this job
 };
@@ -718,7 +718,7 @@ int prologue(const Layout& L, const gf_attn_desc* d, const float* Y, const float
   int rc;
   const float* AK = f + (keys_from_xbar ? L.f_AK2 : L.f_AK);
   const float* CK = f + (keys_from_xbar ? L.f_CK2 : L.f_CK);
-  // operands of the tcgen05 TF32 contractions are pre-rounded here; the fp32-FMA kernel gets them untouched
+  // operands of the wgmma TF32 contractions are pre-rounded here; the fp32-FMA kernel gets them untouched
   const int tf32 = (!(d->flags & GF_FLAG_FP32_EXACT) && tc_supported(L, d)) ? 1 : 0;
   if (!L.duplex) {
     // simplex: keys from the latents (inner dimension D): the whole of stage I is one launch
@@ -746,7 +746,7 @@ int prologue(const Layout& L, const gf_attn_desc* d, const float* Y, const float
 // depends on the latents only (one launch for everything that does not need the centroids)
 int duplex_tables(const Layout& L, const gf_attn_desc* d, const float* Y, const float* f, float* ws, cudaStream_t st,
                   const float* in_scale, int in_scale_ld) {
-  const int tf32 = tc_centroid_supported(L, d) ? 1 : 0;      // M is an operand of the tcgen05 pass-A kernel: pre-round it
+  const int tf32 = tc_centroid_supported(L, d) ? 1 : 0;      // M is an operand of the wgmma pass-A kernel: pre-round it
   const int tf32_v = (!(d->flags & GF_FLAG_FP32_EXACT) && tc_supported(L, d)) ? 1 : 0;
   StageIBatch batch;
   batch.njobs = 1;

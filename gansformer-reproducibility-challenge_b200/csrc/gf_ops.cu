@@ -1,7 +1,7 @@
 // gf_ops.cu -- memory-bound companions of the attention hot path (include/gf_ops.h): channel scaling
 // (style modulation / demodulation), the two upfirdn_2d uses of the generator, and fused bias + noise + activation.
 //
-// B200-native equivalents of the reference's native ops dnnlib/tflib/ops/{fused_bias_act,upfirdn_2d}.cu (expected
+// sm_90a equivalents of the reference's native ops dnnlib/tflib/ops/{fused_bias_act,upfirdn_2d}.cu (expected
 // upstream; not in the checkout).  All are pure streaming kernels: float4 accesses on channels-last rows, grids
 // sized to a few waves of the device's SMs, no shared memory (the FIR reuse is served by L1/L2).
 #include "gf_common.cuh"

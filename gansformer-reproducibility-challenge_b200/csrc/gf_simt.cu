@@ -1,4 +1,4 @@
-// gf_simt.cu -- CUDA-core fp32-FMA kernels of stage T (tight-tolerance mode and shapes the tcgen05 kernel
+// gf_simt.cu -- CUDA-core fp32-FMA kernels of stage T (tight-tolerance mode and shapes the wgmma kernel
 // does not take), the instance/batch-norm statistics pass, and duplex pass A (centroids).
 //
 // Replaces, on the reference side (expected src/training/network.py, not in the checkout): the body of

@@ -1,21 +1,20 @@
-// gf_tc.cu -- stage T on the Blackwell tensor path: TMA-staged tiles, tcgen05 (kind::tf32) MMAs with TMEM
-// accumulators, per-token softmax and LayerNorm on CUDA cores, in-place modulation in shared memory, TMA stores.
+// gf_tc.cu -- stage T on the Hopper tensor path: TMA-staged tiles, wgmma (tf32) with register accumulators, per-token
+// softmax and LayerNorm on CUDA cores, in-place modulation in shared memory, TMA stores.
 //
 // Replaces, on the reference side (expected src/training/network.py, not in the checkout): the body of
 // transformer_layer (Q projection folded into K', QK^T, softmax, PV), integrate and att_norm.  Same algorithm as
 // oracle/folded.py per_token(); operands of both contractions are rounded to TF32 by the tensor cores.
 //
-// One persistent CTA per SM, 14 warps:
-//   warp 0       TMA producer: X slabs (128 tokens x 32 channels, 16 KB, SWIZZLE_128B) into a ring; K'/V^T per image
-//   warp 1       MMA issuer:   GEMM1  S[128,KP]   = X[128,C] . K'^T            (A,B from smem, D in TMEM)
-//                              GEMM2  G[128,32]   = P[128,KP] . V^T[32 ch,KP]^T per slab (A = P from TMEM, B from smem)
-//   warps 10-13  row warps (one per TMEM lane quadrant, thread = token row), run up to a tile ahead: LayerNorm statistics
-//                of the whole row from the swizzled slabs, softmax (S from TMEM -> P back to TMEM), attention-map store
-//   warps 2-9    two epilogue groups of 4 warps; group g owns the slabs with (slab & 1) == g: gain(/bias) from TMEM,
-//                y = LN(x)*g (+b) [+ noise + bias, leaky-ReLU] written in place over the slab, TMA store, slab release
-// Single-pass mode (C <= 256): the tile's slabs stay resident from load to store -> X read once, X' written once from HBM
-// (the algorithmic bytes of SURVEY 8d).  Two-pass mode (C = 512, a tile does not fit): slabs stream through the ring
-// once for GEMM1 + statistics and are fetched a second time (L2 hits) for the epilogue.
+// One persistent CTA per SM, 9 warps:
+//   warp 8       TMA producer: X slabs (128 tokens x 32 channels, 16 KB, SWIZZLE_128B) into a ring; K'/V^T per image
+//   warps 0-3,   two consumer warpgroups; warpgroup g owns token rows [64 g, 64 g + 64) of every tile and runs, for them:
+//   warps 4-7      GEMM1  S[64,KP] = X[64,C] . K'^T (wgmma, A and B from shared memory), the LayerNorm statistics of the rows
+//                  from the same slabs, softmax in registers (a row lives in the 4 lanes of a quad), then per slab
+//                  GEMM2  G[64,32] = P[64,KP] . V^T[32 ch,KP]^T (A = P from registers) and the store side
+//                  y = LN(x)*g (+b) [+ noise + bias, leaky-ReLU, tRGB, next style] written in place over its half slab, TMA store.
+// Single-pass mode (C <= 256): the tile's slabs stay resident from load to store -> X read once, X' written once from HBM.
+// Two-pass mode (C = 512, a tile does not fit): slabs stream through the ring once for GEMM1 + statistics and are fetched
+// a second time (L2 hits) for the store side.
 #include <stdlib.h>
 #include "gf_common.cuh"
 #include "gf_tc_common.cuh"
@@ -24,24 +23,20 @@ namespace gf {
 
 namespace tc {
 
-constexpr int TILE = 128;                 // tokens per tile (UMMA M)
+constexpr int TILE = 128;                 // tokens per tile
+constexpr int HALF = 64;                  // rows of one consumer warpgroup (wgmma M)
 constexpr int SLAB_CH = 32;               // channels per slab = one 128-byte swizzle span of fp32
 constexpr int SLAB_BYTES = TILE * SLAB_CH * 4;
 constexpr int MAX_STAGES = 13;
-constexpr int NACC = 4;                   // accumulator stages of GEMM2 in TMEM
-constexpr int NUM_THREADS = 448;        // warp 0 producer, 1 MMA, 2-9 epilogue (two groups), 10-13 row warps
-constexpr int TMEM_COLS = 512;
-// TMEM column map
-constexpr int COL_S = 0;                  // S[2]  : 2 x 32
-constexpr int COL_P = 64;                 // P[2]  : 2 x 32
-constexpr int COL_ACC = 128;              // ACC[4]: 4 x 64
+constexpr int NUM_THREADS = 288;          // warps 0-7 two consumer warpgroups, warp 8 producer
+constexpr int PRODUCER_WARP = 8;
 
 struct Params {
   float* att; const float* Rt; const float* Ct;
   int n, H, W, k, Cout, B;
   int norm_layer;            // 1 = LayerNorm over C, 0 = none
   int nstages;
-  int drain_each_tile;       // 1: release every slab at tile end (ring barely larger than a tile)
+  int nwg;                   // consumer warpgroups with rows: 2, or 1 when an image has at most 64 tokens
   long long total_tiles;
   int tiles_per_image;
   int rows;                  // token rows per tile: TILE, or n when an image is smaller than a tile (8x8 grid)
@@ -51,8 +46,8 @@ struct Params {
   // fused tRGB (1x1 modulated conv of the layer output to 3 planes): rgb_w [B][3][C] per-sample weights, rgb_out [B][3][n]
   const float* rgb_w; const float* rgb_bias; float* rgb_out;
   int heads, seg_shift;      // multi-head: the softmax runs per segment of (1 << seg_shift) table columns (heads * seg == KP)
-  // attention dropout (training): the row warps drop / rescale the probabilities with the Philox mask the CUDA-core kernels and the
-  // backward draw, and pass 1 - sum(q) to the store side, which re-adds the un-droppable constants cb [Cout] (bo, the 1 of 1 + gain)
+  // attention dropout (training): the probabilities are dropped / rescaled with the Philox mask the CUDA-core kernels and the
+  // backward draw; 1 - sum(q) re-adds the un-droppable constants cb [Cout] (bo, the 1 of 1 + gain) on the store side
   DropoutArgs dp; const float* cb;
 };
 
@@ -62,13 +57,7 @@ struct Params {
 struct Bars {
   uint64_t slab_full[MAX_STAGES], slab_empty[MAX_STAGES];
   uint64_t kv_full, kv_free;
-  uint64_t s_full[2], p_full[2], p_free[2];
-  uint64_t st_full[2], st_free[2];
-  uint64_t acc_full[NACC], acc_empty[NACC];
   uint64_t sc_full[2], sc_free[2];       // per-image load/store-side scale vectors (double-buffered by image parity)
-  uint64_t rgb_full[2], rgb_free[2];     // tRGB partial sums of epilogue group 1 -> group 0 (double-buffered by tile parity)
-  uint32_t tmem_base;
-  uint32_t pad;
 };
 
 template <int KP, int NS, int MODE>
@@ -78,45 +67,48 @@ struct Cfg {
   static constexpr int KP_BYTES = KP * C * 4;            // K' : NS chunks of [KP rows x 128 B]
   static constexpr int V_ROW_BYTES = KP * 4;             // V^T row (one channel): KP latents
   static constexpr int V_BYTES = COUT * V_ROW_BYTES;
-  static constexpr int STATS_BYTES = 2 * TILE * 4 * 4;   // [tile parity][row]{mean, rstd, 1 - sum q (dropout), -}
   static constexpr int PBIAS_BYTES = C * 4;              // post-op bias vector
   static constexpr int OFF_KP = 0;
   static constexpr int OFF_V = OFF_KP + KP_BYTES;
-  static constexpr int OFF_STATS = OFF_V + V_BYTES;
-  static constexpr int OFF_PBIAS = OFF_STATS + STATS_BYTES;
-  // fused tRGB: C <= 256, and C = 512 with k <= 16 (its weights + partial sums cost the two-pass ring one of 9 stages there;
-  // with k = 32 the tables already leave the ring 5 stages, so that shape keeps the separate tRGB kernel)
+  static constexpr int OFF_PBIAS = OFF_V + V_BYTES;
+  // fused tRGB: C <= 256, and C = 512 with k <= 16 (with k = 32 the tables leave the two-pass ring too few stages for the
+  // tRGB weights, so that shape keeps the separate tRGB kernel)
   static constexpr bool RGB_OK = NS <= 8 || KP <= 16;
   static constexpr int NVEC = RGB_OK ? 5 : 2;             // per-image vectors: in_scale, post_scale (+ tRGB weights r / g / b)
   static constexpr int SCALE_BYTES = 2 * NVEC * C * 4;   // [image parity][NVEC][C]
   static constexpr int OFF_SCALE = OFF_PBIAS + PBIAS_BYTES;
-  static constexpr int RGBP_BYTES = RGB_OK ? 2 * 3 * TILE * 4 : 0;    // [tile parity][plane][row]: group 1's partial sums
-  static constexpr int OFF_RGBP = OFF_SCALE + SCALE_BYTES;
-  static constexpr int OFF_BARS = OFF_RGBP + RGBP_BYTES;
+  static constexpr int OFF_BARS = OFF_SCALE + SCALE_BYTES;
   static constexpr int OFF_RING = (OFF_BARS + (int)sizeof(Bars) + 1023) / 1024 * 1024;
   static constexpr int FIXED_BYTES = OFF_RING;
 };
 
+__device__ __forceinline__ float quad_sum(float v) {
+  v += __shfl_xor_sync(0xffffffffu, v, 1);
+  return v + __shfl_xor_sync(0xffffffffu, v, 2);
+}
+__device__ __forceinline__ float quad_max(float v) {
+  v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 1));
+  return fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 2));
+}
+
 template <int KP, int NS, int MODE, bool TWO_PASS>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
-token_tc_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmO,
+token_tc_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmO0, const __grid_constant__ CUtensorMap tmO1,
                 const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV, const Params P) {
   using CF = Cfg<KP, NS, MODE>;
   constexpr int C = CF::C;
+  constexpr int NJ = KP / 8;                           // 8-column blocks of S / k-blocks of GEMM2
   constexpr int SPT = TWO_PASS ? 2 * NS : NS;          // ring slots a tile consumes
-  constexpr uint32_t EMPTY_COUNT = TWO_PASS ? 5u : 1u;  // pass-1 slab: MMA commit + 4 row warps; pass-2 / single: store leader
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);   // SWIZZLE_128B atoms need 1024 B alignment
   const uint32_t s_base = smem_u32(smem);
   const uint32_t s_kp = s_base + CF::OFF_KP, s_v = s_base + CF::OFF_V, s_ring = s_base + CF::OFF_RING;
   Bars* bars = reinterpret_cast<Bars*>(smem + CF::OFF_BARS);
-  float* stats = reinterpret_cast<float*>(smem + CF::OFF_STATS);
   float* pbias_s = reinterpret_cast<float*>(smem + CF::OFF_PBIAS);
   const float* scale_s = reinterpret_cast<const float*>(smem + CF::OFF_SCALE);
   const uint32_t s_scale = s_base + CF::OFF_SCALE;
   const bool has_rgb = CF::RGB_OK && P.rgb_out != nullptr;
   const bool has_scales = P.in_scale != nullptr || P.post_scale != nullptr || has_rgb;      // any per-image vector to stage
-  float* rgbp = reinterpret_cast<float*>(smem + CF::OFF_RGBP);
   constexpr int NV = CF::NVEC;
   if (P.has_post)
     for (int i = threadIdx.x; i < C; i += NUM_THREADS) pbias_s[i] = P.pbias ? P.pbias[i] : 0.f;
@@ -125,39 +117,22 @@ token_tc_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__
   const int nst = P.nstages;
 
   // contiguous tile range of this CTA
-  // (the 64-bit divisions are library calls: broadcast their results so the compiler knows the loop bounds are warp-uniform)
   const long long tile_beg = __shfl_sync(0xffffffffu, (long long)blockIdx.x * P.total_tiles / gridDim.x, 0);
   const long long tile_end = __shfl_sync(0xffffffffu, (long long)(blockIdx.x + 1) * P.total_tiles / gridDim.x, 0);
 
-  if (warp == 0 && lane == 0) {
-    prefetch_tmap(&tmX); prefetch_tmap(&tmO); prefetch_tmap(&tmK); prefetch_tmap(&tmV);
-    for (int i = 0; i < nst; ++i) { mbar_init(smem_u32(&bars->slab_full[i]), 1); mbar_init(smem_u32(&bars->slab_empty[i]), EMPTY_COUNT); }
-    mbar_init(smem_u32(&bars->kv_full), 1); mbar_init(smem_u32(&bars->kv_free), 1);
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(smem_u32(&bars->s_full[i]), 1);
-      mbar_init(smem_u32(&bars->p_full[i]), 4);
-      mbar_init(smem_u32(&bars->p_free[i]), 1);
-      mbar_init(smem_u32(&bars->st_full[i]), 4);
-      mbar_init(smem_u32(&bars->st_free[i]), 8);
-    }
-    for (int i = 0; i < NACC; ++i) { mbar_init(smem_u32(&bars->acc_full[i]), 1); mbar_init(smem_u32(&bars->acc_empty[i]), 4); }
-    for (int i = 0; i < 2; ++i) { mbar_init(smem_u32(&bars->sc_full[i]), 1); mbar_init(smem_u32(&bars->sc_free[i]), 12); }   // 4 row + 8 epilogue warps
-    for (int i = 0; i < 2; ++i) { mbar_init(smem_u32(&bars->rgb_full[i]), 4); mbar_init(smem_u32(&bars->rgb_free[i]), 4); }
+  if (warp == PRODUCER_WARP && lane == 0) {
+    prefetch_tmap(&tmX); prefetch_tmap(&tmO0); prefetch_tmap(&tmO1); prefetch_tmap(&tmK); prefetch_tmap(&tmV);
+    for (int i = 0; i < nst; ++i) { mbar_init(smem_u32(&bars->slab_full[i]), 1); mbar_init(smem_u32(&bars->slab_empty[i]), (uint32_t)P.nwg); }
+    mbar_init(smem_u32(&bars->kv_full), 1); mbar_init(smem_u32(&bars->kv_free), (uint32_t)P.nwg);
+    for (int i = 0; i < 2; ++i) { mbar_init(smem_u32(&bars->sc_full[i]), 1); mbar_init(smem_u32(&bars->sc_free[i]), (uint32_t)P.nwg); }
     fence_barrier_init();
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&bars->tmem_base)), "n"(TMEM_COLS) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = __shfl_sync(0xffffffffu, bars->tmem_base, 0);
 
-  if (warp == 0) {
+  if (warp == PRODUCER_WARP) {
     // =============================== TMA producer ===============================
     if (lane == 0) {
-      uint32_t ctr = 0;        // global ring-slot counter of this CTA (32-bit: 64-bit div/mod is ~100 instructions)
+      uint32_t ctr = 0;        // global ring-slot counter of this CTA
       int img_changes = 0;
       int prev_b = -1;
       for (long long tile = tile_beg; tile < tile_end; ++tile) {
@@ -172,8 +147,6 @@ token_tc_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__
 #pragma unroll
           for (int r0 = 0; r0 < CF::COUT; r0 += VROWS) tma_load_2d(s_v + r0 * CF::V_ROW_BYTES, &tmV, bar, 0, b * CF::COUT + r0);
           if (has_scales) {
-            // per-(b,c) scale vectors of this image -> shared memory (the consumers read them once per slab: from global
-            // that was 8-16 dependent L2 round trips per slab on the critical path of the fused post-op)
             const int par = img_changes & 1;
             mbar_wait(smem_u32(&bars->sc_free[par]), (uint32_t)(((img_changes >> 1) & 1) ^ 1));
             const uint32_t sb = smem_u32(&bars->sc_full[par]);
@@ -187,7 +160,7 @@ token_tc_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__
         }
         const int row0 = (int)(tile * P.rows);
         for (int ss = 0; ss < SPT; ++ss, ++ctr) {
-          const int s = ss % NS;                     // two-pass: the same slabs are fetched again for the epilogue
+          const int s = ss % NS;                     // two-pass: the same slabs are fetched again for the store side
           const int stage = (int)(ctr % (uint32_t)nst);
           const uint32_t phase = (ctr / (uint32_t)nst) & 1u;
           mbar_wait(smem_u32(&bars->slab_empty[stage]), phase ^ 1u);
@@ -197,445 +170,337 @@ token_tc_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__
         }
       }
     }
-  } else if (warp == 1) {
-    // =============================== MMA issuer ===============================
-    // Warp-converged: all 32 lanes run the loop with operands derived from kernel parameters / __shfl_sync, so the
-    // descriptors stay in uniform registers and every tcgen05.mma / commit is one elect.sync-predicated instruction
-    // (issued from an `if (lane == 0)` branch each MMA costs ~16 SASS instructions, tools/probes/mma_issue_probe.cu).
-    {
-      constexpr uint32_t IDESC1 = umma_idesc_tf32(TILE, KP);
-      constexpr uint32_t IDESC2 = umma_idesc_tf32(TILE, 32);
-      constexpr uint32_t V_LAYOUT = KP == 32 ? LAYOUT_SW128 : LAYOUT_SW64;
-      constexpr uint32_t V_SBO = 8 * CF::V_ROW_BYTES;
-      int acc = 0; uint32_t acc_ph = 0;          // accumulator ring position
-      int stage = 0; uint32_t ph = 0;            // ring walker: every fill, in slot order
-      int img_changes = 0;
-      uint32_t it = 0;
-      int b = __shfl_sync(0xffffffffu, (int)(tile_beg / P.tiles_per_image), 0);      // (division = library call: re-broadcast)
-      int t_in_img = __shfl_sync(0xffffffffu, (int)(tile_beg - (long long)b * P.tiles_per_image), 0);
-      bool new_img = true;
-      // base descriptors, advanced with one 64-bit add per MMA (start-address field = 16-byte units)
-      const uint64_t dRing = umma_desc(s_ring, 1024, LAYOUT_SW128);
-      const uint64_t dKp = umma_desc(s_kp, 1024, LAYOUT_SW128);
-      const uint64_t dV = umma_desc(s_v, V_SBO, V_LAYOUT);
-      for (long long tile = tile_beg; tile < tile_end; ++tile, ++it) {
-        const int buf = (int)(it & 1);
-        const uint32_t bphase = (it >> 1) & 1u;
-        if (new_img) {
-          mbar_wait(smem_u32(&bars->kv_full), (uint32_t)(img_changes & 1));
-          tc_fence_after();
-          ++img_changes;
-          new_img = false;
-        }
-        // ---- GEMM1: S[buf] = X . K'^T over all slabs (pass 1 of a two-pass tile)
-        const uint32_t d_s = tmem + COL_S + buf * 32;
-#pragma unroll 1
-        for (int s = 0; s < NS; ++s) {
-          mbar_wait(smem_u32(&bars->slab_full[stage]), ph);
-          tc_fence_after();
-          const uint64_t da = dRing + (uint64_t)(stage * (SLAB_BYTES >> 4));
-          const uint64_t db = dKp + (uint64_t)(s * ((KP * 128) >> 4));
+    return;
+  }
+
+  // =============================== consumer warpgroups ===============================
+  const int wg = warp >> 2;
+  if (wg >= P.nwg) return;                         // short images: the second warpgroup has no rows
+  const int gid = lane >> 2, qd = lane & 3;        // quad (row pair) and lane inside it
+  const int rA = wg * HALF + (warp & 3) * 16 + gid;  // tile rows of this thread: rA and rA + 8
+  const bool leader = (warp & 3) == 0 && lane == 0;
+  const CUtensorMap* tmO = wg ? &tmO1 : &tmO0;
+  const uint32_t half_off = (uint32_t)(wg * HALF * 128);
+  const float act_a = P.pact == 1 ? 0.6f * P.pgain : P.pgain, act_b = P.pact == 1 ? 0.4f * P.pgain : 0.f;
+  const bool has_noise = P.has_post && P.pnoise != nullptr;
+  const float pstr = (has_noise && P.pstrength) ? __ldg(P.pstrength) : 1.f;
+  const float rgb_b0 = (has_rgb && P.rgb_bias) ? __ldg(P.rgb_bias) : 0.f, rgb_b1 = (has_rgb && P.rgb_bias) ? __ldg(P.rgb_bias + 1) : 0.f,
+              rgb_b2 = (has_rgb && P.rgb_bias) ? __ldg(P.rgb_bias + 2) : 0.f;
+  const bool dp_on = P.dp.thr != 0;
+  const uint64_t dKp = gmma_desc(s_kp, 1024, LAYOUT_SW128);
+  const uint64_t dV = gmma_desc(s_v, 8 * CF::V_ROW_BYTES, KP == 32 ? LAYOUT_SW128 : LAYOUT_SW64);
+
+  int stage = 0; uint32_t ph = 0;                  // ring walker: every fill, in slot order
+  int img_changes = 0, imgc = 0;
+  int b = (int)(tile_beg / P.tiles_per_image);
+  int t_in_img = (int)(tile_beg - (long long)b * P.tiles_per_image);
+  bool new_img = true;
+  int pending_stage = -1;                          // leader: slab whose store may still be reading shared memory
+  for (long long tile = tile_beg; tile < tile_end; ++tile) {
+    const int bimg = b, t_cur = t_in_img;
+    const bool img_first = t_in_img == 0 || tile == tile_beg;
+    if (++t_in_img == P.tiles_per_image) { t_in_img = 0; ++b; }
+    const bool img_last = t_in_img == 0;
+    const int spar = imgc & 1;
+    if (new_img) { mbar_wait(smem_u32(&bars->kv_full), (uint32_t)(img_changes & 1)); ++img_changes; new_img = false; }
+    if (has_scales && img_first) mbar_wait(smem_u32(&bars->sc_full[spar]), (uint32_t)((imgc >> 1) & 1));
+    const float* isc_img = P.in_scale ? scale_s + spar * NV * C : nullptr;
+
+    // positional logits of this thread's rows and columns (issued before the slab loop: their latency hides under it)
+    int tok[2];
+    float pos[NJ][4];
 #pragma unroll
-          for (int kk = 0; kk < 4; ++kk) umma_ss_elect(d_s, da + kk * 2, db + kk * 2, IDESC1, (s | kk) ? 1u : 0u);
-          if (TWO_PASS) umma_commit_elect(smem_u32(&bars->slab_empty[stage]));    // slab may be recycled once these MMAs are done
-          if (++stage == nst) { stage = 0; ph ^= 1u; }
-        }
-        umma_commit_elect(smem_u32(&bars->s_full[buf]));
-        // ---- GEMM2: per slab, ACC = P[buf] . V^T (gain | bias)
-        mbar_wait(smem_u32(&bars->p_full[buf]), bphase);
-        tc_fence_after();
-        const uint32_t a_p = tmem + COL_P + buf * 32;
-#pragma unroll 1
-        for (int s = 0; s < NS; ++s) {
-          if (TWO_PASS) {
-            // Parity waits are only valid if a waiter never falls two phases behind a barrier: every consumer walks the
-            // fills of the ring in slot order.  Waiting the pass-2 fill here also makes acc_full(s) imply "slab s landed".
-            mbar_wait(smem_u32(&bars->slab_full[stage]), ph);
-            if (++stage == nst) { stage = 0; ph ^= 1u; }
-          }
-          mbar_wait(smem_u32(&bars->acc_empty[acc]), acc_ph ^ 1u);
-          tc_fence_after();
-          const uint32_t d_acc = tmem + COL_ACC + acc * 64;
-          const uint64_t dvg = dV + (uint64_t)((s * 32 * CF::V_ROW_BYTES) >> 4);
+    for (int i = 0; i < 2; ++i) {
+      tok[i] = min(t_cur * P.rows + rA + 8 * i, P.n - 1);
+      const int h = tok[i] / P.W, w = tok[i] - h * P.W;
+      const float* rt = P.Rt + ((size_t)bimg * P.H + h) * KP + 2 * qd;
+      const float* ct = P.Ct + ((size_t)bimg * P.W + w) * KP + 2 * qd;
 #pragma unroll
-          for (int kk = 0; kk < KP / 8; ++kk) umma_ts_elect(d_acc, a_p + kk * 8, dvg + kk * 2, IDESC2, kk ? 1u : 0u);
-          if constexpr (MODE == GF_INT_BOTH) {
-            const uint64_t dvb = dV + (uint64_t)(((C + s * 32) * CF::V_ROW_BYTES) >> 4);
-#pragma unroll
-            for (int kk = 0; kk < KP / 8; ++kk) umma_ts_elect(d_acc + 32, a_p + kk * 8, dvb + kk * 2, IDESC2, kk ? 1u : 0u);
-          }
-          umma_commit_elect(smem_u32(&bars->acc_full[acc]));
-          if (++acc == NACC) { acc = 0; acc_ph ^= 1u; }
-        }
-        umma_commit_elect(smem_u32(&bars->p_free[buf]));
-        if (++t_in_img == P.tiles_per_image) {
-          t_in_img = 0; ++b; new_img = true;
-          if (tile + 1 < tile_end) umma_commit_elect(smem_u32(&bars->kv_free));
-        }
+      for (int j = 0; j < NJ; ++j) {
+        const float2 r = __ldg(reinterpret_cast<const float2*>(rt + 8 * j)), c = __ldg(reinterpret_cast<const float2*>(ct + 8 * j));
+        pos[j][2 * i] = r.x + c.x; pos[j][2 * i + 1] = r.y + c.y;
       }
     }
-  } else if (warp >= 10) {
-    // =============================== row warps: statistics + softmax ===============================
-    const int q = warp & 3;                        // TMEM lane quadrant this warp may access
-    const int row = q * 32 + lane;                 // token row inside the tile
-    const uint32_t lane_addr = (uint32_t)(q * 32) << 16;
-    const int sw = row & 7;
-    const uint32_t row_off = (uint32_t)row * 128u;
-    uint32_t it = 0;
-    int b = (int)(tile_beg / P.tiles_per_image);
-    int t_in_img = (int)(tile_beg - (long long)b * P.tiles_per_image);
-    int stage = 0; uint32_t ph = 0;                // ring walker: every fill, in slot order
-    // Positional logits of (image bb, tile tt), row `row`.  The column part (per token) is fetched one tile ahead, the row part
-    // (the same line for the whole tile when W >= 128) at the top of its tile and consumed after the statistics sweep, so
-    // that neither L2 latency is exposed; KP = 32 has no registers for prefetching both a tile ahead.
-    float4 pr[KP / 4], pc[KP / 4];
-    auto pos_ptrs = [&](int bb, int tt, const float4*& rt, const float4*& ct) {
-      const int tok = min(tt * P.rows + row, P.n - 1);               // clamped: rows past a short tile
-      const int h = tok / P.W, w = tok - h * P.W;
-      rt = reinterpret_cast<const float4*>(P.Rt + ((size_t)bb * P.H + h) * KP);
-      ct = reinterpret_cast<const float4*>(P.Ct + ((size_t)bb * P.W + w) * KP);
-    };
-    int imgc = 0;                                  // images this CTA has started (parity selects the scale buffer)
-    const float4 *rt_cur = nullptr, *ct_nxt = nullptr;
-    if (tile_beg < tile_end) {
-      pos_ptrs(b, t_in_img, rt_cur, ct_nxt);
-#pragma unroll
-      for (int j4 = 0; j4 < KP / 4; ++j4) pc[j4] = __ldg(ct_nxt + j4);
-    }
-    for (long long tile = tile_beg; tile < tile_end; ++tile, ++it) {
-      const int buf = (int)(it & 1);
-      const uint32_t bphase = (it >> 1) & 1u;
-      const int tok = min(t_in_img * P.rows + row, P.n - 1);         // token inside the image (for the attention-map store)
-#pragma unroll
-      for (int j4 = 0; j4 < KP / 4; ++j4) pr[j4] = __ldg(rt_cur + j4);  // consumed after the statistics sweep (fence below)
-      const bool img_first = t_in_img == 0 || tile == tile_beg;
-      if (++t_in_img == P.tiles_per_image) { t_in_img = 0; ++b; }
-      const bool img_last = t_in_img == 0;
-      const int spar = imgc & 1;
-      if (has_scales && img_first) mbar_wait(smem_u32(&bars->sc_full[spar]), (uint32_t)((imgc >> 1) & 1));
-      // ---- LayerNorm statistics of the whole row (shifted sums)
-      float mean = 0.f, rstd = 1.f;
-      if (P.norm_layer || TWO_PASS) {
-        float sh = 0.f, sum = 0.f, sumsq = 0.f;
+
+    // ---- GEMM1 S = X . K'^T and the LayerNorm statistics (shifted sums; a row's channels are split over its quad)
+    const int stage0 = stage; const uint32_t ph0 = ph;
+    float sacc[KP / 2];
+    float sh[2] = {0.f, 0.f}, sum[2] = {0.f, 0.f}, sumsq[2] = {0.f, 0.f};
 #pragma unroll 1
-        for (int s = 0; s < NS; ++s) {
-          mbar_wait(smem_u32(&bars->slab_full[stage]), ph);
-          if (P.norm_layer) {
-            const uint8_t* slab = smem + CF::OFF_RING + stage * SLAB_BYTES + row_off;
-            const float4* isc = P.in_scale ? reinterpret_cast<const float4*>(scale_s + spar * NV * C + s * SLAB_CH) : nullptr;
+    for (int s = 0; s < NS; ++s) {
+      mbar_wait(smem_u32(&bars->slab_full[stage]), ph);
+      const uint32_t sa = s_ring + stage * SLAB_BYTES + half_off;
+      const uint64_t da = gmma_desc(sa, 1024, LAYOUT_SW128);
+      const uint64_t db = dKp + (uint64_t)(s * ((KP * 128) >> 4));
+      wgmma_fence();
 #pragma unroll
-            for (int c = 0; c < 8; ++c) {
-              float4 x = *reinterpret_cast<const float4*>(slab + ((c ^ sw) << 4));
-              if (isc) { const float4 d = isc[c]; x.x *= d.x; x.y *= d.y; x.z *= d.z; x.w *= d.w; }   // shared-memory broadcast
-              if (s == 0 && c == 0) sh = x.x;
-              const float d0 = x.x - sh, d1 = x.y - sh, d2 = x.z - sh, d3 = x.w - sh;
-              sum += (d0 + d1) + (d2 + d3);
-              sumsq = fmaf(d0, d0, fmaf(d1, d1, fmaf(d2, d2, fmaf(d3, d3, sumsq))));
-            }
+      for (int kk = 0; kk < 4; ++kk) {
+        if constexpr (KP == 32) wgmma_ss_n32(sacc, da + kk * 2, db + kk * 2, (s | kk) ? 1u : 0u);
+        else wgmma_ss_n16(sacc, da + kk * 2, db + kk * 2, (s | kk) ? 1u : 0u);
+      }
+      wgmma_commit();
+      if (P.norm_layer) {
+        const float4* isc = isc_img ? reinterpret_cast<const float4*>(isc_img + s * SLAB_CH) : nullptr;
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+          const int r = rA + 8 * i;
+          const uint8_t* slab = smem + CF::OFF_RING + stage * SLAB_BYTES + r * 128;
+          if (s == 0) { sh[i] = reinterpret_cast<const float*>(slab + ((0 ^ (r & 7)) << 4))[0]; if (isc) sh[i] *= isc[0].x; }
+#pragma unroll
+          for (int cc = 0; cc < 2; ++cc) {
+            const int c = 2 * qd + cc;
+            float4 x = *reinterpret_cast<const float4*>(slab + ((c ^ (r & 7)) << 4));
+            if (isc) { const float4 d = isc[c]; x.x *= d.x; x.y *= d.y; x.z *= d.z; x.w *= d.w; }
+            const float d0 = x.x - sh[i], d1 = x.y - sh[i], d2 = x.z - sh[i], d3 = x.w - sh[i];
+            sum[i] += (d0 + d1) + (d2 + d3);
+            sumsq[i] = fmaf(d0, d0, fmaf(d1, d1, fmaf(d2, d2, fmaf(d3, d3, sumsq[i]))));
           }
-          if (TWO_PASS) {                            // this warp is done with the pass-1 slab
-            __syncwarp();
-            if (lane == 0) mbar_arrive(smem_u32(&bars->slab_empty[stage]));
-          }
-          if (++stage == nst) { stage = 0; ph ^= 1u; }
         }
-        if (P.norm_layer) {
-          const float md = sum * (1.f / (float)C);
-          const float var = fmaxf(sumsq * (1.f / (float)C) - md * md, 0.f);
-          mean = sh + md;
-          rstd = rsqrtf(var + 1e-8f);
-        }
-      } else {                                       // no statistics pass: skip this tile's fills
-        stage += NS;
-        while (stage >= nst) { stage -= nst; ph ^= 1u; }
       }
-      if (has_scales && img_last) {                  // this warp is done with the image's scale vectors
-        __syncwarp();
-        if (lane == 0) mbar_arrive(smem_u32(&bars->sc_free[spar]));
+      if (TWO_PASS) {                              // the pass-1 slab may be recycled once this warpgroup's MMAs read it
+        wgmma_wait<0>();
+        named_bar_sync(1 + wg, 128);
+        if (leader) mbar_arrive(smem_u32(&bars->slab_empty[stage]));
       }
-      if (img_last) ++imgc;
-      // positional logits of this tile; then start the next tile's column-part loads (consumed one iteration later)
-      float sv[KP];
+      if (++stage == nst) { stage = 0; ph ^= 1u; }
+    }
+    wgmma_wait<0>();
+    fence_regs<KP / 2>(sacc);
+    float mean[2] = {0.f, 0.f}, rstd[2] = {1.f, 1.f};
+    if (P.norm_layer) {
 #pragma unroll
-      for (int j4 = 0; j4 < KP / 4; ++j4) {
-        asm volatile("" : "+f"(pr[j4].x), "+f"(pr[j4].y), "+f"(pr[j4].z), "+f"(pr[j4].w));   // keeps the adds below the sweep
-        sv[j4 * 4 + 0] = pr[j4].x + pc[j4].x; sv[j4 * 4 + 1] = pr[j4].y + pc[j4].y;
-        sv[j4 * 4 + 2] = pr[j4].z + pc[j4].z; sv[j4 * 4 + 3] = pr[j4].w + pc[j4].w;
+      for (int i = 0; i < 2; ++i) {
+        const float md = quad_sum(sum[i]) * (1.f / (float)C);
+        const float var = fmaxf(quad_sum(sumsq[i]) * (1.f / (float)C) - md * md, 0.f);
+        mean[i] = sh[i] + md;
+        rstd[i] = rsqrtf(var + 1e-8f);
       }
-      if (tile + 1 < tile_end) {
-        pos_ptrs(b, t_in_img, rt_cur, ct_nxt);
+    }
+
+    // ---- softmax over the latents (logits in log2 units: gf_fold.cu folds log2 e into K' / Rt / Ct).  sacc[4j + 2i + e] is
+    // row rA + 8i, column 8j + 2 qd + e.
 #pragma unroll
-        for (int j4 = 0; j4 < KP / 4; ++j4) pc[j4] = __ldg(ct_nxt + j4);
-      }
-      const bool dp_on = P.dp.thr != 0;                            // (kernel parameter: uniform)
-      if (!dp_on) {                                                // with dropout the hand-off waits for 1 - sum q, below
-        mbar_wait(smem_u32(&bars->st_free[buf]), bphase ^ 1u);     // epilogue of the tile two iterations back has read its stats
-        *reinterpret_cast<float2*>(stats + (buf * TILE + row) * 4) = make_float2(mean, rstd);
-        __syncwarp();
-        if (lane == 0) mbar_arrive(smem_u32(&bars->st_full[buf]));
-      }
-      // ---- softmax over the latents: S (TMEM) -> P (TMEM)
-      mbar_wait(smem_u32(&bars->s_full[buf]), bphase);
-      tc_fence_after();
+    for (int j = 0; j < NJ; ++j)
+#pragma unroll
+      for (int e = 0; e < 4; ++e) sacc[4 * j + e] += pos[j][e];
+    float qdef[2] = {0.f, 0.f};
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      const int r = rA + 8 * i;
+      float* a = (P.att && r < P.rows) ? P.att + ((size_t)bimg * P.n + tok[i]) * P.k : nullptr;
       if (P.heads == 1) {
         float mx = -INFINITY;
 #pragma unroll
-        for (int hh = 0; hh < KP / 16; ++hh) {                        // 16 columns at a time: keeps the register peak down
-          float acc[16];
-          tmem_ld16(tmem + lane_addr + COL_S + buf * 32 + hh * 16, acc);
-          tmem_wait_ld();
-#pragma unroll
-          for (int j = 0; j < 16; ++j) { sv[hh * 16 + j] += acc[j]; mx = fmaxf(mx, sv[hh * 16 + j]); }
-        }
+        for (int j = 0; j < NJ; ++j) mx = fmaxf(mx, fmaxf(sacc[4 * j + 2 * i], sacc[4 * j + 2 * i + 1]));
+        mx = quad_max(mx);
         float den = 0.f;
 #pragma unroll
-        for (int j = 0; j < KP; ++j) { sv[j] = exp2f(sv[j] - mx); den += sv[j]; }   // logits arrive in log2 units (gf_fold.cu folds log2 e into K' / Rt / Ct)
-        const float inv = 1.f / den;
+        for (int j = 0; j < NJ; ++j)
 #pragma unroll
-        for (int j = 0; j < KP; ++j) sv[j] *= inv;
-        if (P.att && row < P.rows) {
-          float* a = P.att + ((size_t)(img_last ? b - 1 : b) * P.n + tok) * P.k;
+          for (int e = 0; e < 2; ++e) { const float v = exp2f(sacc[4 * j + 2 * i + e] - mx); sacc[4 * j + 2 * i + e] = v; den += v; }
+        const float inv = 1.f / quad_sum(den);
 #pragma unroll
-          for (int j = 0; j < KP; ++j) if (j < P.k) a[j] = sv[j];
-        }
-      } else {
-        // multi-head: one softmax per segment of table columns (head h owns columns [h * seg, (h + 1) * seg)); the attention map is
-        // the mean over the heads
+        for (int j = 0; j < NJ; ++j)
 #pragma unroll
-        for (int hh = 0; hh < KP / 16; ++hh) {
-          float acc[16];
-          tmem_ld16(tmem + lane_addr + COL_S + buf * 32 + hh * 16, acc);
-          tmem_wait_ld();
-#pragma unroll
-          for (int j = 0; j < 16; ++j) sv[hh * 16 + j] += acc[j];
-        }
-        float mxs[4] = {-INFINITY, -INFINITY, -INFINITY, -INFINITY}, dens[4] = {0.f, 0.f, 0.f, 0.f};
-#pragma unroll
-        for (int j = 0; j < KP; ++j) { const int g_ = j >> P.seg_shift; mxs[g_] = fmaxf(mxs[g_], sv[j]); }
-#pragma unroll
-        for (int j = 0; j < KP; ++j) { const int g_ = j >> P.seg_shift; sv[j] = exp2f(sv[j] - mxs[g_]); dens[g_] += sv[j]; }
-#pragma unroll
-        for (int g_ = 0; g_ < 4; ++g_) dens[g_] = 1.f / dens[g_];
-#pragma unroll
-        for (int j = 0; j < KP; ++j) sv[j] *= dens[j >> P.seg_shift];
-        if (P.att && row < P.rows) {
-          float* a = P.att + ((size_t)(img_last ? b - 1 : b) * P.n + tok) * P.k;
-          const int seg = 1 << P.seg_shift;
-          const float ih = 1.f / (float)P.heads;
-          for (int j = 0; j < P.k; ++j) {
-            float m = 0.f;
-#pragma unroll
-            for (int c = 0; c < KP; ++c) if ((c & (seg - 1)) == j) m += sv[c];
-            a[j] = m * ih;
+          for (int e = 0; e < 2; ++e) {
+            sacc[4 * j + 2 * i + e] *= inv;
+            const int c = 8 * j + 2 * qd + e;
+            if (a && c < P.k) a[c] = sacc[4 * j + 2 * i + e];
           }
+      } else {
+        // multi-head: one softmax per segment of table columns (head h owns columns [h * seg, (h + 1) * seg)); segments are
+        // multiples of 8 columns, so a thread's column 8j + 2 qd + e lies in segment j >> (seg_shift - 3)
+        const int jsh = P.seg_shift - 3;
+        // per-block partials, then combined over the blocks of the same segment (compile-time indices: stays in registers)
+        float bm[NJ], mx[NJ], bs[NJ];
+#pragma unroll
+        for (int j = 0; j < NJ; ++j) bm[j] = quad_max(fmaxf(sacc[4 * j + 2 * i], sacc[4 * j + 2 * i + 1]));
+#pragma unroll
+        for (int j = 0; j < NJ; ++j) {
+          mx[j] = -INFINITY;
+#pragma unroll
+          for (int j2 = 0; j2 < NJ; ++j2) if ((j2 >> jsh) == (j >> jsh)) mx[j] = fmaxf(mx[j], bm[j2]);
+        }
+#pragma unroll
+        for (int j = 0; j < NJ; ++j) {
+          bs[j] = 0.f;
+#pragma unroll
+          for (int e = 0; e < 2; ++e) { const float v = exp2f(sacc[4 * j + 2 * i + e] - mx[j]); sacc[4 * j + 2 * i + e] = v; bs[j] += v; }
+          bs[j] = quad_sum(bs[j]);
+        }
+#pragma unroll
+        for (int j = 0; j < NJ; ++j) {
+          float den = 0.f;
+#pragma unroll
+          for (int j2 = 0; j2 < NJ; ++j2) if ((j2 >> jsh) == (j >> jsh)) den += bs[j2];
+          const float inv = 1.f / den;
+#pragma unroll
+          for (int e = 0; e < 2; ++e) sacc[4 * j + 2 * i + e] *= inv;
+        }
+        if (a) {                                   // attention map = mean over the heads
+          const int segj = 1 << jsh;
+          const float ih = 1.f / (float)P.heads;
+#pragma unroll
+          for (int j = 0; j < NJ; ++j)
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const int c = 8 * j + 2 * qd + e;
+              if (j < segj && c < P.k) {
+                float m = 0.f;
+#pragma unroll
+                for (int j2 = 0; j2 < NJ; ++j2) if ((j2 & (segj - 1)) == j) m += sacc[4 * j2 + 2 * i + e];
+                a[c] = m * ih;
+              }
+            }
         }
       }
       if (dp_on) {
         // attention dropout on the probabilities (the map above is pre-dropout): same Philox stream as token_simt_kernel / the backward
         const unsigned long long seed = P.dp.state[0], step = P.dp.state[1];
-        const uint32_t gtok = (uint32_t)((size_t)(img_last ? b - 1 : b) * P.n + tok);
+        const uint32_t gtok = (uint32_t)((size_t)bimg * P.n + tok[i]);
         float qs = 0.f;
 #pragma unroll
-        for (int q4 = 0; q4 < KP / 4; ++q4) {
+        for (int j = 0; j < NJ; ++j) {
           float mk[4];
-          dropout_mult4(P.dp, seed, step, gtok, q4, mk);
-          sv[q4 * 4] *= mk[0]; sv[q4 * 4 + 1] *= mk[1]; sv[q4 * 4 + 2] *= mk[2]; sv[q4 * 4 + 3] *= mk[3];
-          qs += (sv[q4 * 4] + sv[q4 * 4 + 1]) + (sv[q4 * 4 + 2] + sv[q4 * 4 + 3]);
-        }
-        mbar_wait(smem_u32(&bars->st_free[buf]), bphase ^ 1u);
-        *reinterpret_cast<float4*>(stats + (buf * TILE + row) * 4) = make_float4(mean, rstd, 1.f - qs, 0.f);
-        __syncwarp();
-        if (lane == 0) mbar_arrive(smem_u32(&bars->st_full[buf]));
-      }
-      // round P to the nearest TF32 so the tensor core's operand truncation is exact (see gf_fold.cu: round_tf32)
+          dropout_mult4(P.dp, seed, step, gtok, 2 * j + (qd >> 1), mk);
 #pragma unroll
-      for (int j = 0; j < KP; ++j) sv[j] = cvt_tf32(sv[j]);
-      mbar_wait(smem_u32(&bars->p_free[buf]), bphase ^ 1u);       // GEMM2 of the tile two iterations back is done
-      tc_fence_after();
-      tmem_st16(tmem + lane_addr + COL_P + buf * 32, sv);
-      if constexpr (KP == 32) tmem_st16(tmem + lane_addr + COL_P + buf * 32 + 16, sv + 16);
-      tmem_wait_st();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(smem_u32(&bars->p_full[buf]));
-      if (TWO_PASS) {   // observe the pass-2 fills too (see the MMA warp): keeps this thread's parity bookkeeping in step
-#pragma unroll 1
-        for (int s = 0; s < NS; ++s) {
-          mbar_wait(smem_u32(&bars->slab_full[stage]), ph);
-          if (++stage == nst) { stage = 0; ph ^= 1u; }
+          for (int e = 0; e < 2; ++e) { sacc[4 * j + 2 * i + e] *= mk[2 * (qd & 1) + e]; qs += sacc[4 * j + 2 * i + e]; }
+        }
+        qdef[i] = 1.f - quad_sum(qs);
+      }
+    }
+    // P rounded to the nearest TF32 (the tensor core's operand truncation is then exact, see gf_fold.cu: round_tf32), then
+    // rearranged from the accumulator layout (columns 2 qd, 2 qd + 1) into the A-operand layout (columns qd, qd + 4)
+    uint32_t pa[NJ][4];
+    {
+      const int srcA = (lane & ~3) | (qd >> 1), srcB = srcA + 2;
+      const bool odd = qd & 1;
+#pragma unroll
+      for (int j = 0; j < NJ; ++j) {
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+          const float v0 = cvt_tf32(sacc[4 * j + 2 * i]), v1 = cvt_tf32(sacc[4 * j + 2 * i + 1]);
+          const float a0 = __shfl_sync(0xffffffffu, v0, srcA), a1 = __shfl_sync(0xffffffffu, v1, srcA);
+          const float b0 = __shfl_sync(0xffffffffu, v0, srcB), b1 = __shfl_sync(0xffffffffu, v1, srcB);
+          pa[j][i] = __float_as_uint(odd ? a1 : a0);          // (row rA + 8i, column 8j + qd)
+          pa[j][2 + i] = __float_as_uint(odd ? b1 : b0);      // (row rA + 8i, column 8j + qd + 4)
         }
       }
     }
-  } else {
-    // =============================== epilogue warps ===============================
-    const int q = warp & 3;                        // TMEM lane quadrant this warp may access
-    const int g = (warp - 2) >> 2;                 // group: owns slabs with (slab & 1) == g
-    const int row = q * 32 + lane;                 // token row inside the tile
-    const uint32_t lane_addr = (uint32_t)(q * 32) << 16;
-    const bool leader = ((warp - 2) & 3) == 0 && lane == 0;
-    const int sw = row & 7;                        // 128B-swizzle phase of this row
-    const uint32_t row_off = (uint32_t)row * 128u;
-    int pending_stage = -1;
-    uint32_t it = 0;
-    int imgc = 0;
-    int b_next = (int)(tile_beg / P.tiles_per_image);
-    int t_in_img = (int)(tile_beg - (long long)b_next * P.tiles_per_image);
-    // post-op noise: one value per token, fetched a tile ahead (its L2 latency sat on the epilogue's critical path)
-    const bool has_noise = P.has_post && P.pnoise != nullptr;
-    const float pstr = (has_noise && P.pstrength) ? __ldg(P.pstrength) : 1.f;
-    const float act_a = P.pact == 1 ? 0.6f * P.pgain : P.pgain, act_b = P.pact == 1 ? 0.4f * P.pgain : 0.f;
-    const float rgb_b0 = (has_rgb && P.rgb_bias) ? __ldg(P.rgb_bias) : 0.f, rgb_b1 = (has_rgb && P.rgb_bias) ? __ldg(P.rgb_bias + 1) : 0.f,
-                rgb_b2 = (has_rgb && P.rgb_bias) ? __ldg(P.rgb_bias + 2) : 0.f;
-    float pnz_next = 0.f;
-    if (has_noise && tile_beg < tile_end) pnz_next = __ldg(P.pnoise + (size_t)b_next * P.pnoise_bstride + min(t_in_img * P.rows + row, P.n - 1));
-    for (long long tile = tile_beg; tile < tile_end; ++tile, ++it) {
-      const int b = b_next;
-      const int buf = (int)(it & 1);
-      const uint32_t bphase = (it >> 1) & 1u;
-      const float pnz_t = pnz_next * pstr;           // post-op: per-token noise value (0 without noise / post-op)
-      const int t_cur = t_in_img;                      // this tile's index inside its image
-      float rgb0 = 0.f, rgb1 = 0.f, rgb2 = 0.f;         // fused tRGB: this thread's share (its group's slabs) of the token's 3 sums
-      const bool img_first = t_in_img == 0 || tile == tile_beg;
-      if (++t_in_img == P.tiles_per_image) { t_in_img = 0; ++b_next; }
-      if (has_noise && tile + 1 < tile_end)
-        pnz_next = __ldg(P.pnoise + (size_t)b_next * P.pnoise_bstride + min(t_in_img * P.rows + row, P.n - 1));
-      const bool img_last = t_in_img == 0;
-      const int spar = imgc & 1;
-      if (has_scales && img_first) mbar_wait(smem_u32(&bars->sc_full[spar]), (uint32_t)((imgc >> 1) & 1));
-      // ---- row statistics from the row warps
-      mbar_wait(smem_u32(&bars->st_full[buf]), bphase);
-      const float4 st4 = *reinterpret_cast<const float4*>(stats + (buf * TILE + row) * 4);
-      const float mean = st4.x, rstd = st4.y, qdef = st4.z;        // qdef: only written (and read) with dropout on
-      __syncwarp();
-      if (lane == 0) mbar_arrive(smem_u32(&bars->st_free[buf]));
-      const float mr = -mean * rstd;
-      // ---- epilogue of this group's slabs: y = LN(x) * gain (+ bias) [post-op], in place, TMA store
+
+    // ---- store side, per slab: G = P . V^T (gain | bias), y = LN(x) * g (+ b) [post-op] in place, TMA store of the half slab
+    float pnz[2] = {0.f, 0.f};
+    if (has_noise)
+#pragma unroll
+      for (int i = 0; i < 2; ++i) pnz[i] = __ldg(P.pnoise + (size_t)bimg * P.pnoise_bstride + tok[i]) * pstr;
+    float rgb[2][3] = {{0.f, 0.f, 0.f}, {0.f, 0.f, 0.f}};
+    const float* psc_img = P.post_scale ? scale_s + (spar * NV + 1) * C : nullptr;
+    const float* wr_img = scale_s + (spar * NV + (CF::RGB_OK ? 2 : 0)) * C;        // tRGB weights (read when has_rgb)
+    if (!TWO_PASS) { stage = stage0; ph = ph0; }   // single pass: walk this tile's slots again
 #pragma unroll 1
-      for (int s = g; s < NS; s += 2) {
-        const uint32_t ctr = it * SPT + (TWO_PASS ? NS : 0) + s;
-        const uint32_t actr = it * NS + s;
-        const int stage = (int)(ctr % (uint32_t)nst);
-        const int a = (int)(actr % NACC);
-        // acc_full first: GEMM2(s) was issued after GEMM1 of this tile completed (single-pass: every slab of the tile has
-        // landed) and, in two-pass mode, after the MMA warp saw this slab's pass-2 fill -- so the slab_full wait below can
-        // never be a phase early; it is kept for the async-proxy -> generic-proxy visibility of the TMA write.
-        mbar_wait(smem_u32(&bars->acc_full[a]), (actr / NACC) & 1u);
-        mbar_wait(smem_u32(&bars->slab_full[stage]), (ctr / (uint32_t)nst) & 1u);
-        tc_fence_after();
-        float gv[32], bv[MODE == GF_INT_BOTH ? 32 : 1];
-        const uint32_t t_acc = tmem + lane_addr + COL_ACC + a * 64;
-        tmem_ld16(t_acc, gv);
-        tmem_ld16(t_acc + 16, gv + 16);
-        if constexpr (MODE == GF_INT_BOTH) { tmem_ld16(t_acc + 32, bv); tmem_ld16(t_acc + 48, bv + 16); }
-        tmem_wait_ld();
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(smem_u32(&bars->acc_empty[a]));
-        if (P.dp.thr) {                                // dropout broke sum q = 1: re-add the constants the fold put into V^T
-          const float4* cbg = reinterpret_cast<const float4*>(P.cb + s * SLAB_CH);
+    for (int s = 0; s < NS; ++s) {
+      if (TWO_PASS) mbar_wait(smem_u32(&bars->slab_full[stage]), ph);
+      float gv[16], bv[MODE == GF_INT_BOTH ? 16 : 1];
+      const uint64_t dvg = dV + (uint64_t)((s * 32 * CF::V_ROW_BYTES) >> 4);
+      wgmma_fence();
 #pragma unroll
-          for (int c = 0; c < 8; ++c) {
-            const float4 v = __ldg(cbg + c);
-            gv[c * 4] = fmaf(qdef, v.x, gv[c * 4]); gv[c * 4 + 1] = fmaf(qdef, v.y, gv[c * 4 + 1]);
-            gv[c * 4 + 2] = fmaf(qdef, v.z, gv[c * 4 + 2]); gv[c * 4 + 3] = fmaf(qdef, v.w, gv[c * 4 + 3]);
-          }
-          if constexpr (MODE == GF_INT_BOTH) {
-            const float4* cbb = reinterpret_cast<const float4*>(P.cb + C + s * SLAB_CH);
+      for (int kk = 0; kk < NJ; ++kk) wgmma_rs_n32(gv, pa[kk], dvg + kk * 2, kk ? 1u : 0u);
+      if constexpr (MODE == GF_INT_BOTH) {
+        const uint64_t dvb = dV + (uint64_t)(((C + s * 32) * CF::V_ROW_BYTES) >> 4);
 #pragma unroll
-            for (int c = 0; c < 8; ++c) {
-              const float4 v = __ldg(cbb + c);
-              bv[c * 4] = fmaf(qdef, v.x, bv[c * 4]); bv[c * 4 + 1] = fmaf(qdef, v.y, bv[c * 4 + 1]);
-              bv[c * 4 + 2] = fmaf(qdef, v.z, bv[c * 4 + 2]); bv[c * 4 + 3] = fmaf(qdef, v.w, bv[c * 4 + 3]);
+        for (int kk = 0; kk < NJ; ++kk) wgmma_rs_n32(bv, pa[kk], dvb + kk * 2, kk ? 1u : 0u);
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      fence_regs<16>(gv);
+      if constexpr (MODE == GF_INT_BOTH) fence_regs<16>(bv);
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        const int r = rA + 8 * i;
+        const float mr = -mean[i] * rstd[i];
+        uint8_t* slab = smem + CF::OFF_RING + stage * SLAB_BYTES + r * 128;
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          const int cl = 8 * j + 2 * qd;                            // channel inside the slab
+          const int ch = s * SLAB_CH + cl;
+          float2* px = reinterpret_cast<float2*>(slab + ((((cl >> 2) ^ (r & 7))) << 4) + (cl & 3) * 4);
+          float2 x = *px;
+          float g0 = gv[4 * j + 2 * i], g1 = gv[4 * j + 2 * i + 1];
+          float b0 = 0.f, b1 = 0.f;
+          if constexpr (MODE == GF_INT_BOTH) { b0 = bv[4 * j + 2 * i]; b1 = bv[4 * j + 2 * i + 1]; }
+          if (dp_on) {                             // dropout broke sum q = 1: re-add the constants the fold put into V^T
+            const float2 cg = __ldg(reinterpret_cast<const float2*>(P.cb + ch));
+            g0 = fmaf(qdef[i], cg.x, g0); g1 = fmaf(qdef[i], cg.y, g1);
+            if constexpr (MODE == GF_INT_BOTH) {
+              const float2 cbb = __ldg(reinterpret_cast<const float2*>(P.cb + C + ch));
+              b0 = fmaf(qdef[i], cbb.x, b0); b1 = fmaf(qdef[i], cbb.y, b1);
             }
           }
-        }
-        uint8_t* slab = smem + CF::OFF_RING + stage * SLAB_BYTES + row_off;
-        const float4* isc = P.in_scale ? reinterpret_cast<const float4*>(scale_s + spar * NV * C + s * SLAB_CH) : nullptr;
-        const float4* psc = P.post_scale ? reinterpret_cast<const float4*>(scale_s + (spar * NV + 1) * C + s * SLAB_CH) : nullptr;
-        const float4* wrv = reinterpret_cast<const float4*>(scale_s + (spar * NV + (CF::RGB_OK ? 2 : 0)) * C + s * SLAB_CH);   // tRGB weights (read when has_rgb)
-#pragma unroll
-        for (int c = 0; c < 8; ++c) {
-          float4* px = reinterpret_cast<float4*>(slab + ((c ^ sw) << 4));
-          float4 x = *px;
-          if (isc) { const float4 d = isc[c]; x.x *= d.x; x.y *= d.y; x.z *= d.z; x.w *= d.w; }
-          float xn0 = fmaf(x.x, rstd, mr), xn1 = fmaf(x.y, rstd, mr), xn2 = fmaf(x.z, rstd, mr), xn3 = fmaf(x.w, rstd, mr);
-          // modulation with the post-op's per-token noise riding on the same FMA (pnz_t = 0 without a post-op)
+          if (isc_img) { const float2 d = *reinterpret_cast<const float2*>(isc_img + ch); x.x *= d.x; x.y *= d.y; }
+          const float xn0 = fmaf(x.x, rstd[i], mr), xn1 = fmaf(x.y, rstd[i], mr);
+          // modulation with the post-op's per-token noise riding on the same FMA (pnz = 0 without a post-op)
           if constexpr (MODE == GF_INT_MUL) {
-            x.x = fmaf(xn0, gv[c * 4 + 0], pnz_t); x.y = fmaf(xn1, gv[c * 4 + 1], pnz_t); x.z = fmaf(xn2, gv[c * 4 + 2], pnz_t); x.w = fmaf(xn3, gv[c * 4 + 3], pnz_t);
+            x.x = fmaf(xn0, g0, pnz[i]); x.y = fmaf(xn1, g1, pnz[i]);
           } else if constexpr (MODE == GF_INT_ADD) {
-            x.x = (xn0 + pnz_t) + gv[c * 4 + 0]; x.y = (xn1 + pnz_t) + gv[c * 4 + 1]; x.z = (xn2 + pnz_t) + gv[c * 4 + 2]; x.w = (xn3 + pnz_t) + gv[c * 4 + 3];
+            x.x = (xn0 + pnz[i]) + g0; x.y = (xn1 + pnz[i]) + g1;
           } else {
-            x.x = fmaf(xn0, gv[c * 4 + 0], bv[c * 4 + 0] + pnz_t); x.y = fmaf(xn1, gv[c * 4 + 1], bv[c * 4 + 1] + pnz_t);
-            x.z = fmaf(xn2, gv[c * 4 + 2], bv[c * 4 + 2] + pnz_t); x.w = fmaf(xn3, gv[c * 4 + 3], bv[c * 4 + 3] + pnz_t);
+            x.x = fmaf(xn0, g0, b0 + pnz[i]); x.y = fmaf(xn1, g1, b1 + pnz[i]);
           }
           if (P.has_post) {
-            const float4 pb = *reinterpret_cast<const float4*>(pbias_s + s * SLAB_CH + c * 4);   // broadcast read
-            x.x += pb.x; x.y += pb.y; x.z += pb.z; x.w += pb.w;
+            const float2 pb = *reinterpret_cast<const float2*>(pbias_s + ch);
+            x.x += pb.x; x.y += pb.y;
             // gain * leaky-ReLU(v) = v * (0.6 gain) + |v| * (0.4 gain)  (linear: act_a = gain, act_b = 0): two instructions
             x.x = fmaf(fabsf(x.x), act_b, x.x * act_a); x.y = fmaf(fabsf(x.y), act_b, x.y * act_a);
-            x.z = fmaf(fabsf(x.z), act_b, x.z * act_a); x.w = fmaf(fabsf(x.w), act_b, x.w * act_a);
-            if (has_rgb) {                                   // tRGB reads the layer output proper: before the next layer's style scale
-              const float4 w0 = wrv[c], w1 = wrv[(C >> 2) + c], w2 = wrv[2 * (C >> 2) + c];       // shared-memory broadcasts
-              rgb0 = fmaf(x.x, w0.x, fmaf(x.y, w0.y, fmaf(x.z, w0.z, fmaf(x.w, w0.w, rgb0))));
-              rgb1 = fmaf(x.x, w1.x, fmaf(x.y, w1.y, fmaf(x.z, w1.z, fmaf(x.w, w1.w, rgb1))));
-              rgb2 = fmaf(x.x, w2.x, fmaf(x.y, w2.y, fmaf(x.z, w2.z, fmaf(x.w, w2.w, rgb2))));
+            if (has_rgb) {                         // tRGB reads the layer output proper: before the next layer's style scale
+              const float2 w0 = *reinterpret_cast<const float2*>(wr_img + ch), w1 = *reinterpret_cast<const float2*>(wr_img + C + ch),
+                           w2 = *reinterpret_cast<const float2*>(wr_img + 2 * C + ch);
+              rgb[i][0] = fmaf(x.x, w0.x, fmaf(x.y, w0.y, rgb[i][0]));
+              rgb[i][1] = fmaf(x.x, w1.x, fmaf(x.y, w1.y, rgb[i][1]));
+              rgb[i][2] = fmaf(x.x, w2.x, fmaf(x.y, w2.y, rgb[i][2]));
             }
-            if (psc) { const float4 q4 = psc[c]; x.x *= q4.x; x.y *= q4.y; x.z *= q4.z; x.w *= q4.w; }
+            if (psc_img) { const float2 q2 = *reinterpret_cast<const float2*>(psc_img + ch); x.x *= q2.x; x.y *= q2.y; }
           }
           *px = x;
         }
-        fence_proxy_async();                       // generic-proxy writes -> visible to the TMA (async proxy)
-        named_bar_sync(2 + g, 128);
-        if (leader) {
-          tma_store_2d(&tmO, s_ring + stage * SLAB_BYTES, s * SLAB_CH, (int)(tile * P.rows));
-          tma_commit();
-          if (pending_stage >= 0) {
-            tma_wait_read1();                      // the previous store has finished reading its slab
-            mbar_arrive_n(smem_u32(&bars->slab_empty[pending_stage]), EMPTY_COUNT);
-          }
-          pending_stage = stage;
+      }
+      fence_proxy_async();                         // generic-proxy writes -> visible to the TMA (async proxy)
+      named_bar_sync(1 + wg, 128);
+      if (leader) {
+        tma_store_2d(tmO, s_ring + stage * SLAB_BYTES + half_off, s * SLAB_CH, (int)(tile * P.rows) + wg * HALF);
+        tma_commit();
+        if (pending_stage >= 0) {
+          tma_wait_read1();                        // the previous store has finished reading its slab
+          mbar_arrive(smem_u32(&bars->slab_empty[pending_stage]));
         }
+        pending_stage = stage;
       }
-      if (has_rgb) {
-        // a token's channels are split over the two epilogue groups: group 1 hands its partial sums to group 0, which adds the
-        // bias and writes the three planes (32 consecutive tokens per warp: 128-byte coalesced stores)
-        float* pb = rgbp + buf * 3 * TILE;
-        if (g == 1) {
-          mbar_wait(smem_u32(&bars->rgb_free[buf]), bphase ^ 1u);
-          pb[row] = rgb0; pb[TILE + row] = rgb1; pb[2 * TILE + row] = rgb2;
-          __syncwarp();
-          if (lane == 0) mbar_arrive(smem_u32(&bars->rgb_full[buf]));
-        } else {
-          mbar_wait(smem_u32(&bars->rgb_full[buf]), bphase);
-          rgb0 += pb[row]; rgb1 += pb[TILE + row]; rgb2 += pb[2 * TILE + row];
-          __syncwarp();
-          if (lane == 0) mbar_arrive(smem_u32(&bars->rgb_free[buf]));
-          if (row < P.rows) {
-            float* o = P.rgb_out + (size_t)b * 3 * P.n + (size_t)t_cur * P.rows + row;
-            o[0] = rgb0 + rgb_b0; o[P.n] = rgb1 + rgb_b1; o[2 * (size_t)P.n] = rgb2 + rgb_b2;
-          }
+      if (++stage == nst) { stage = 0; ph ^= 1u; }
+    }
+    if (leader) {                                  // no slab stays held across tiles
+      tma_wait_read0();
+      mbar_arrive(smem_u32(&bars->slab_empty[pending_stage]));
+      pending_stage = -1;
+    }
+    if (has_rgb) {                                 // a row's channels are split over its quad
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        const float s0 = quad_sum(rgb[i][0]), s1 = quad_sum(rgb[i][1]), s2 = quad_sum(rgb[i][2]);
+        const int r = rA + 8 * i;
+        if (qd == 0 && r < P.rows) {
+          float* o = P.rgb_out + (size_t)bimg * 3 * P.n + (size_t)t_cur * P.rows + r;
+          o[0] = s0 + rgb_b0; o[P.n] = s1 + rgb_b1; o[2 * (size_t)P.n] = s2 + rgb_b2;
         }
-      }
-      if (has_scales && img_last) {                  // this warp has read the image's scale vectors for the last time
-        __syncwarp();
-        if (lane == 0) mbar_arrive(smem_u32(&bars->sc_free[spar]));
-      }
-      if (img_last) ++imgc;
-      if (leader && P.drain_each_tile && pending_stage >= 0) {   // small rings: no slab may stay held across tiles
-        tma_wait_read0();
-        mbar_arrive_n(smem_u32(&bars->slab_empty[pending_stage]), EMPTY_COUNT);
-        pending_stage = -1;
       }
     }
-    if (leader) tma_wait_all();
+    // the named barrier of the last slab has ordered every warp's reads of K' / V^T / the scale vectors before this point
+    if (leader && has_scales && img_last) mbar_arrive(smem_u32(&bars->sc_free[spar]));
+    if (img_last) ++imgc;
+    if (img_last) {
+      new_img = true;
+      if (leader && tile + 1 < tile_end) mbar_arrive(smem_u32(&bars->kv_free));
+    }
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "n"(TMEM_COLS) : "memory");
-  }
+  if (leader) tma_wait_all();
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -659,13 +524,16 @@ static int launch(const Layout& L, const gf_attn_desc* d, const float* X, float*
   constexpr bool TWO = two_pass_shape<NS>();
   int nst = stages_for<KP, NS, MODE>(device_smem_optin());
   if (const char* e = getenv("GF_TC_MAX_STAGES")) { const int v = atoi(e); if (v >= min_stages<NS>() && v < nst) nst = v; }   // tuning aid: ring-depth sensitivity
-  if (nst < min_stages<NS>()) { set_error("tcgen05 path: shared memory too small for C=%d KP=%d mode=%d", L.C, KP, MODE); return GF_ERR_UNSUPPORTED; }
-  CUtensorMap tmX, tmO, tmK, tmV;
+  if (nst < min_stages<NS>()) { set_error("tensor path: shared memory too small for C=%d KP=%d mode=%d", L.C, KP, MODE); return GF_ERR_UNSUPPORTED; }
+  CUtensorMap tmX, tmO0, tmO1, tmK, tmV;
   int rc;
   const uint64_t rows = (uint64_t)L.B * L.n;
   const int trows = L.n < TILE ? L.n : TILE;                  // one image per tile when the grid is smaller than a tile
+  // each consumer warpgroup stores its own rows: [0, 64) and [64, trows) of the tile
+  const int nwg = trows > HALF ? 2 : 1;
   if ((rc = make_map(&tmX, X, rows, L.C, trows, SLAB_CH, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
-  if ((rc = make_map(&tmO, Xout, rows, L.C, trows, SLAB_CH, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
+  if ((rc = make_map(&tmO0, Xout, rows, L.C, trows < HALF ? trows : HALF, SLAB_CH, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
+  if ((rc = make_map(&tmO1, Xout, rows, L.C, nwg == 2 ? trows - HALF : 8, SLAB_CH, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
   if ((rc = make_map(&tmK, ws + L.w_Kp, (uint64_t)L.B * KP, L.C, KP, SLAB_CH, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
   const uint32_t vrows = CF::COUT < 256 ? CF::COUT : 256;
   if ((rc = make_map(&tmV, ws + L.w_Vt, (uint64_t)L.B * CF::COUT, KP, vrows, KP, KP == 32 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B))) return rc;
@@ -674,10 +542,7 @@ static int launch(const Layout& L, const gf_attn_desc* d, const float* X, float*
   P.n = L.n; P.H = L.H; P.W = L.W; P.k = L.k; P.Cout = L.Cout; P.B = L.B;
   P.norm_layer = d->norm == GF_NORM_LAYER ? 1 : 0;
   P.nstages = nst;
-  // Ring slots are handed out strictly round-robin.  A store leader keeps its last slab one store longer (release lag);
-  // across a tile boundary that is only safe when the next tile never needs that slot: single-pass with nst >= NS + 2.
-  // A two-pass tile wraps the ring several times, so it always drains at tile end.
-  P.drain_each_tile = TWO ? 1 : (nst < NS + 2 ? 1 : 0);
+  P.nwg = nwg;
   P.tiles_per_image = (L.n + TILE - 1) / TILE;
   P.rows = trows;
   P.total_tiles = (long long)L.B * P.tiles_per_image;
@@ -695,9 +560,9 @@ static int launch(const Layout& L, const gf_attn_desc* d, const float* X, float*
   GF_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
   long long grid = device_sms();
   if (grid > P.total_tiles) grid = P.total_tiles;
-  kern<<<(unsigned)grid, NUM_THREADS, smem_bytes, st>>>(tmX, tmO, tmK, tmV, P);
+  kern<<<(unsigned)grid, NUM_THREADS, smem_bytes, st>>>(tmX, tmO0, tmO1, tmK, tmV, P);
   GF_LAUNCH_OK();
-  set_path(GF_PATH_TCGEN05_TF32);
+  set_path(GF_PATH_WGMMA_TF32);
   return GF_OK;
 }
 

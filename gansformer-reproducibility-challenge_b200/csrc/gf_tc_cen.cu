@@ -1,29 +1,21 @@
-// gf_tc_cen.cu -- duplex pass A (latents attend to the grid, softmax over the n grid cells) on the tensor path.
+// gf_tc_cen.cu -- duplex pass A (latents attend to the grid, softmax over the n grid cells) on the Hopper tensor path.
 //
 // Replaces, on the reference side (expected src/training/network.py, not in the checkout): the k-means / centroid branch
 // of transformer_layer (image -> latents attention).  Algorithm = oracle/folded.py centroid_pass():
 //     L[t,j] = x_t . M_j + pos(t,j);   A[j,:] = softmax_t L[:,j];   Xbar[j,:] = sum_t A[j,t] x_t
-// streamed once over X with an online softmax (lazy rescaling), split over `nsplit` CTAs per image whose partials
-// (acc[KP][C], m[KP], l[KP]) are merged by centroid_merge_kernel (gf_simt.cu).
+// streamed once over X with an online softmax, split over `nsplit` CTAs per image whose partials (acc[KP][C], m[KP], l[KP])
+// are merged by centroid_merge_kernel (gf_simt.cu).
 //
-// grid (nsplit, B, C/C2), 8 warps, one 128-token tile per step:
-//   warp 0   TMA producer of ring 1: the X slabs (128 tokens x 32 channels) with SWIZZLE_128B -- X as the K-major A operand
-//            of GEMM1 (contraction over channels).  This is the fetch that comes from HBM; the ring is deep and a slab is
-//            recycled as soon as its 4 MMAs have retired.
-//   warp 1   TMA producer of ring 2: the same data again (an L2 hit), 64 channels per stage, with
-//            SWIZZLE_128B_ATOM_32B -- X as the MN-major A operand of GEMM2 (contraction over tokens; for 32-bit MN-major
-//            operands that swizzle, UMMA layout SWIZZLE_128B_BASE32B, is the only one the tensor core accepts, and a
-//            K-major operand with it faults, so the two GEMMs cannot share one copy).
-//   warp 6   GEMM1  S[128 tok, KP]  = X . M^T                  (M=128, N=KP, K=8 per MMA; 4 MMAs per slab), up to two tiles ahead
-//   warp 7   GEMM2  D2[64 ch, KP]  += X_stage^T . E            (M=64 channels, N=KP, K=8 tokens per MMA; 16 MMAs per stage)
-//            Both issuers run warp-converged with every operand derived from kernel parameters / __shfl_sync so that the
-//            descriptors live in uniform registers and each tcgen05.mma is ONE instruction (elect.sync-predicated); issued
-//            from an `if (lane == 0)` branch the same MMA costs ~16 SASS instructions (tools/probes/mma_issue_probe.cu).
-//   warps 2-5 row warps (thread = token): positional logits, S from TMEM, lazy-rescale vote, E = 2^(s - m) rounded to TF32
-//            and written TRANSPOSED into shared memory (the K-major B operand of GEMM2), softmax denominators accumulated
-//            in registers (reduced once at the end), rare rescale of the TMEM accumulators, final flush of the partials.
-// Every mbarrier has exactly one waiting role, which observes every phase in order (the precondition of parity waits).
-// HBM traffic: X read once (+ one L2 re-read).
+// grid (nsplit, B, C / C2), 5 warps, one 64-token tile per step:
+//   warp 4     TMA producer: M of the image once, then the X slabs (64 tokens x 32 channels, SWIZZLE_128B) into a ring.
+//   warps 0-3  one consumer warpgroup:
+//              GEMM1  S[64 tok, KP] = X . M^T    (wgmma, A = slab, B = M, both K-major in shared memory)
+//              while the MMAs run, the slabs of this CTA's channel share are transposed into X^T[C2 ch][64 tok]: GEMM2
+//              contracts over tokens, and wgmma takes 32-bit operands K-major only
+//              online softmax over the tokens (column maxima across the warpgroup), E = 2^(s - m) rounded to TF32 written
+//              as E^T[latent][token] (rows KP .. 63 stay zero), accumulators rescaled in registers when a maximum moves
+//              GEMM2  D[64 (KP used), C2] += E^T . X   (wgmma, A = E^T, B = X^T)
+// HBM traffic: X read once per channel share.
 #include <stdlib.h>
 #include "gf_common.cuh"
 #include "gf_tc_common.cuh"
@@ -33,105 +25,63 @@ namespace tcc {
 
 using namespace tc;
 
-constexpr int TILE = 128;
+constexpr int TILE = 64;
 constexpr int SLAB_CH = 32;
-constexpr int SLAB_BYTES = TILE * SLAB_CH * 4;      // 16 KB: ring-1 stage
-constexpr int HG_BYTES = 2 * SLAB_BYTES;            // 32 KB: ring-2 stage = 64 channels ("half group")
-constexpr int MAX_ST1 = 8, MAX_ST2 = 3;
-constexpr int NUM_THREADS = 256;     // warp 0 producer 1, warp 1 producer 2, 2-5 row warps, 6 GEMM1, 7 GEMM2
-constexpr int TMEM_COLS = 256;
-constexpr int COL_S = 0;          // S[2]: 2 x 32 columns
-constexpr int COL_D2 = 64;        // Xbar^T accumulators: one 32-column block per 64 channels (<= 4 blocks)
-constexpr float TAU = 8.f;        // lazy rescale threshold (natural-log units): exp(8) ~ 3e3 of headroom is harmless in fp32
+constexpr int SLAB_BYTES = TILE * SLAB_CH * 4;      // 8 KB
+constexpr int MAX_ST = 8;
+constexpr int NUM_THREADS = 160;                    // warps 0-3 consumers, warp 4 producer
+constexpr int ET_BYTES = 2 * 64 * 128;              // E^T: two 32-token chunks of [64 rows x 128 B]
 
 struct Params {
   const float* Rt; const float* Ct; float* part;
-  float* xbar; const float* in_scale; int in_ld;     // one split per image: the kernel writes the normalised Xbar [B,k,C] itself
-  int n, H, W, k, nsplit, tiles_per_image, nst1, nst2;
-  int lead;                  // ring 1 may run at most `lead` tiles ahead of the completed GEMM2s (L2 reuse distance of ring 2)
+  int n, H, W, k, nsplit, tiles_per_image, nst;
 };
 
 struct Bars {
-  uint64_t full1[MAX_ST1], empty1[MAX_ST1];
-  uint64_t full2[MAX_ST2], empty2[MAX_ST2];
-  uint64_t m_full, done;
-  uint64_t s_full[2], s_free[2], e_full[2], e_free[2];
-  uint32_t tmem_base;
-  uint32_t pad;
+  uint64_t full[MAX_ST], empty[MAX_ST];
+  uint64_t m_full;
 };
 
-// NS = slabs of GEMM1 (all C channels); NS2 = slabs of GEMM2 handled by this CTA (C/32 or, for C = 512, half of them:
-// blockIdx.z selects the channel half, both CTAs recompute the cheap GEMM1 + softmax)
+// NS = slabs of GEMM1 (all C channels); NS2 = slabs of GEMM2 handled by this CTA (blockIdx.z selects the channel share)
 template <int KP, int NS, int NS2 = (NS > 8 ? NS / 2 : NS)>
 struct Cfg {
   static constexpr int C = NS * SLAB_CH;
-  static constexpr int NHG = NS2 / 2;                        // ring-2 stages per tile
+  static constexpr int C2 = NS2 * SLAB_CH;
   static constexpr int M_BYTES = KP * C * 4;                 // NS chunks of [KP rows x 128 B]
-  static constexpr int E_CHUNK = KP * 128;                   // one 32-token chunk of E^T: [KP rows x 128 B]
-  static constexpr int E_BYTES = 4 * E_CHUNK;                // 128 tokens
+  static constexpr int XT_BYTES = 2 * C2 * 128;              // two 32-token chunks of [C2 rows x 128 B]
   static constexpr int OFF_M = 0;
-  static constexpr int OFF_E = OFF_M + M_BYTES;              // 2 buffers
-  static constexpr int OFF_SMALL = OFF_E + 2 * E_BYTES;      // red[4][KP], mref[KP], resc[KP], flags
-  static constexpr int SMALL_BYTES = (4 * KP + 2 * KP + 4) * 4;
+  static constexpr int OFF_XT = OFF_M + M_BYTES;
+  static constexpr int OFF_ET = OFF_XT + XT_BYTES;
+  static constexpr int OFF_SMALL = OFF_ET + ET_BYTES;        // red[4][KP], mref[KP], resc[KP]
+  static constexpr int SMALL_BYTES = 6 * KP * 4;
   static constexpr int OFF_BARS = (OFF_SMALL + SMALL_BYTES + 15) / 16 * 16;
   static constexpr int OFF_RING = (OFF_BARS + (int)sizeof(Bars) + 1023) / 1024 * 1024;
   static constexpr int FIXED_BYTES = OFF_RING;
 };
 
-// kind::tf32, fp32 accumulate; a_mn / b_mn: operand is MN-major
-__host__ __device__ constexpr uint32_t idesc_tf32(int M, int N, int a_mn, int b_mn) {
-  return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)a_mn << 15) | ((uint32_t)b_mn << 16) | ((uint32_t)(N >> 3) << 17) |
-         ((uint32_t)(M >> 4) << 24);
-}
-// MN-major 32-bit operand, UMMA layout SWIZZLE_128B_BASE32B (= TMA SWIZZLE_128B_ATOM_32B, cute Swizzle<2,5,2>):
-// 32 contiguous MN elements (128 B) per K row, 4 K rows per 512-byte atom (32-byte chunks XOR row % 4);
-// leading byte offset = next block of 32 MN elements, stride byte offset = next 4 K rows.
-constexpr uint32_t LAYOUT_SW128_BASE32B = 1;
-__device__ __forceinline__ uint64_t umma_desc_mn(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr >> 4) & 0x3FFF);
-  d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
-  d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)LAYOUT_SW128_BASE32B << 61;
-  return d;
-}
-
 template <int KP, int NS, int NS2>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
-centroid_tc_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmX2,
-                   const __grid_constant__ CUtensorMap tmM, const Params P) {
+centroid_tc_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmM, const Params P) {
   using CF = Cfg<KP, NS, NS2>;
-  constexpr int C = CF::C;
-  constexpr int C2 = NS2 * SLAB_CH;                  // accumulator channels of this CTA
-  constexpr int NHG = CF::NHG;
-  const int zoff = blockIdx.z * C2;                   // first channel of this CTA's GEMM2 share
+  constexpr int C = CF::C, C2 = CF::C2;
+  constexpr int NJ = KP / 8;
+  constexpr int NC2 = C2 / 32;                                // 32-channel chunks of the GEMM2 accumulator
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  const uint32_t pad = (1024u - (smem_u32(smem_raw) & 1023u)) & 1023u;
-  uint8_t* smem = smem_raw + pad;
-  const uint32_t s_base = smem_u32(smem_raw) + pad;
-  const uint32_t s_m = s_base + CF::OFF_M, s_e = s_base + CF::OFF_E, s_ring1 = s_base + CF::OFF_RING;
-  const int nst1 = P.nst1, nst2 = P.nst2;
-  const uint32_t s_ring2 = s_ring1 + (uint32_t)nst1 * SLAB_BYTES;
+  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
+  const uint32_t s_base = smem_u32(smem);
+  const uint32_t s_m = s_base + CF::OFF_M, s_xt = s_base + CF::OFF_XT, s_et = s_base + CF::OFF_ET, s_ring = s_base + CF::OFF_RING;
   Bars* bars = reinterpret_cast<Bars*>(smem + CF::OFF_BARS);
-  const uint32_t s_bars = s_base + CF::OFF_BARS;
-  auto bar = [&](const uint64_t* p) -> uint32_t { return smem_u32(p); };
-#ifdef GF_DEBUG_WATCHDOG
-#ifdef GF_DEBUG_WATCHDOG     // bring-up builds only: record where a barrier wait timed out (tools/hang_debug.py)
-  if (threadIdx.x == 0 && blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0 && g_dbg_buf) g_dbg_buf[1] = s_bars;
-#endif
-#endif
   float* red = reinterpret_cast<float*>(smem + CF::OFF_SMALL);      // [4][KP]
-  float* mref = red + 4 * KP;                                       // [KP]
-  float* resc = mref + KP;                                          // [KP]
-  volatile int* trigf = reinterpret_cast<volatile int*>(resc + KP);  // [2] per-tile-parity trigger flags
-  volatile int* g2done = trigf + 2;                                  // tiles whose GEMM2 is known complete (row warps -> producer 1)
-  const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);   // provably warp-uniform
+  float* mref = red + 4 * KP;                                       // [KP] running maxima (log2 units)
+  float* resc = mref + KP;                                          // [KP] rescale factors of this tile
+  const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);
   const int lane = threadIdx.x & 31;
   const int b = blockIdx.y, sp = blockIdx.x;
+  const int zoff = blockIdx.z * C2;                                 // first channel of this CTA's GEMM2 share
   const int per = (P.tiles_per_image + P.nsplit - 1) / P.nsplit;
   const int tile_beg = sp * per, tile_end = min(P.tiles_per_image, tile_beg + per);
   const int ntiles = tile_end - tile_beg;
+  const int nst = P.nst;
   float* part = P.part + ((size_t)b * P.nsplit + sp) * KP * (C + 4);
 
   if (ntiles <= 0) {                          // empty split: neutral partial
@@ -143,384 +93,278 @@ centroid_tc_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constan
     return;
   }
 
+  for (int i = threadIdx.x; i < ET_BYTES / 16; i += NUM_THREADS) reinterpret_cast<float4*>(smem + CF::OFF_ET)[i] = make_float4(0.f, 0.f, 0.f, 0.f);
   if (threadIdx.x < KP) { mref[threadIdx.x] = -INFINITY; resc[threadIdx.x] = 1.f; }
-  if (threadIdx.x < 3) trigf[threadIdx.x] = 0;                       // trigf[0..1] and g2done
-  if (warp == 0 && lane == 0) {
-    prefetch_tmap(&tmX); prefetch_tmap(&tmX2); prefetch_tmap(&tmM);
-#pragma unroll
-    for (int i = 0; i < MAX_ST1; ++i) { mbar_init(bar(&bars->full1[i]), 1); mbar_init(bar(&bars->empty1[i]), 1); }
-#pragma unroll
-    for (int i = 0; i < MAX_ST2; ++i) { mbar_init(bar(&bars->full2[i]), 1); mbar_init(bar(&bars->empty2[i]), 1); }
-    mbar_init(bar(&bars->m_full), 1); mbar_init(bar(&bars->done), 1);
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(bar(&bars->s_full[i]), 1);
-      mbar_init(bar(&bars->s_free[i]), 4);
-      mbar_init(bar(&bars->e_full[i]), 4);
-      mbar_init(bar(&bars->e_free[i]), 1);
-    }
+  if (warp == 4 && lane == 0) {
+    prefetch_tmap(&tmX); prefetch_tmap(&tmM);
+    for (int i = 0; i < nst; ++i) { mbar_init(smem_u32(&bars->full[i]), 1); mbar_init(smem_u32(&bars->empty[i]), 1); }
+    mbar_init(smem_u32(&bars->m_full), 1);
     fence_barrier_init();
   }
-  if (warp == 6) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(bar((const uint64_t*)&bars->tmem_base)), "n"(TMEM_COLS) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = __shfl_sync(0xffffffffu, bars->tmem_base, 0);
 
-  if (warp == 0) {
-    // =============================== producer 1: HBM -> ring 1 (K-major copy for GEMM1) ===============================
+  if (warp == 4) {
+    // =============================== TMA producer ===============================
     if (lane == 0) {
-      const uint32_t mb = bar(&bars->m_full);
+      const uint32_t mb = smem_u32(&bars->m_full);
       mbar_expect_tx(mb, (uint32_t)CF::M_BYTES);
 #pragma unroll
       for (int s = 0; s < NS; ++s) tma_load_2d(s_m + s * (KP * 128), &tmM, mb, s * SLAB_CH, b * KP);
-      int stage = 0; uint32_t ph = 0;
-      for (int it = 0; it < ntiles; ++it) {
-        const int row0 = b * P.n + (tile_beg + it) * TILE;       // short image (n < TILE): the box runs into the next image, masked below
-        // Bound the run-ahead: ring 2 (warp 1) fetches the same bytes again right before GEMM2 and must find them in L2.  The
-        // reuse distance is (lead of this fetch over GEMM2) x tile bytes x resident CTAs; beyond ~48 MB the B200's L2 has
-        // dropped the lines (tools/probes/l2_reuse_probe.cu) and X is read from HBM twice (1.7x at res 128 before this bound).
-        if (it - *g2done > P.lead) {
-          const long long t0 = clock64();
-          while (it - *g2done > P.lead)
-            if (clock64() - t0 > 4000000000ll) __trap();          // a protocol bug must trap, not hang the GPU
-        }
-        for (int s = 0; s < NS; ++s) {
-          mbar_wait(bar(&bars->empty1[stage]), ph ^ 1u);
-          const uint32_t fb = bar(&bars->full1[stage]);
-          mbar_expect_tx(fb, SLAB_BYTES);
-          tma_load_2d(s_ring1 + stage * SLAB_BYTES, &tmX, fb, s * SLAB_CH, row0);
-          if (++stage == nst1) { stage = 0; ph ^= 1u; }
+      uint32_t ctr = 0;
+      for (int t = tile_beg; t < tile_end; ++t) {
+        const int row0 = b * P.n + t * TILE;       // the rows past a short image's end are masked by the consumers
+        for (int s = 0; s < NS; ++s, ++ctr) {
+          const int stage = (int)(ctr % (uint32_t)nst);
+          mbar_wait(smem_u32(&bars->empty[stage]), ((ctr / (uint32_t)nst) & 1u) ^ 1u);
+          const uint32_t fb = smem_u32(&bars->full[stage]);
+          mbar_expect_tx(fb, (uint32_t)SLAB_BYTES);
+          tma_load_2d(s_ring + stage * SLAB_BYTES, &tmX, fb, s * SLAB_CH, row0);
         }
       }
     }
-  } else if (warp == 1) {
-    // =============================== producer 2: L2 -> ring 2 (MN-major copy for GEMM2) ===============================
-    if (lane == 0) {
-      int stage = 0; uint32_t ph = 0;
-      for (int it = 0; it < ntiles; ++it) {
-        const int row0 = b * P.n + (tile_beg + it) * TILE;
-        for (int hg = 0; hg < NHG; ++hg) {
-          mbar_wait(bar(&bars->empty2[stage]), ph ^ 1u);
-          const uint32_t fb = bar(&bars->full2[stage]);
-          mbar_expect_tx(fb, HG_BYTES);
-          tma_load_2d(s_ring2 + stage * HG_BYTES, &tmX2, fb, zoff + hg * 64, row0);
-          tma_load_2d(s_ring2 + stage * HG_BYTES + SLAB_BYTES, &tmX2, fb, zoff + hg * 64 + SLAB_CH, row0);
-          if (++stage == nst2) { stage = 0; ph ^= 1u; }
-        }
+    return;
+  }
+
+  // =============================== consumer warpgroup ===============================
+  const int w = warp, gid = lane >> 2, qd = lane & 3;
+  const int tid = threadIdx.x;
+  const bool leader = tid == 0;
+  const uint64_t dM = gmma_desc(s_m, 1024, LAYOUT_SW128);
+  float acc2[NC2][16];
+#pragma unroll
+  for (int c = 0; c < NC2; ++c)
+#pragma unroll
+    for (int i = 0; i < 16; ++i) acc2[c][i] = 0.f;
+  float lp[NJ][2];                            // this thread's share of the denominators of its columns
+#pragma unroll
+  for (int j = 0; j < NJ; ++j) { lp[j][0] = 0.f; lp[j][1] = 0.f; }
+  mbar_wait(smem_u32(&bars->m_full), 0);
+  int stage = 0; uint32_t ph = 0;
+  for (int t = tile_beg; t < tile_end; ++t) {
+    // positional logits of this thread's rows (tokens 16 w + gid, + 8) and columns (latents 8 jb + 2 qd + e)
+    float pos[NJ][4];
+    bool valid[2];
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      const int tk = t * TILE + 16 * w + gid + 8 * i;
+      valid[i] = tk < P.n;
+      const int tok = min(tk, P.n - 1);
+      const int h = tok / P.W, x = tok - h * P.W;
+      const float* rt = P.Rt + ((size_t)b * P.H + h) * KP + 2 * qd;
+      const float* ct = P.Ct + ((size_t)b * P.W + x) * KP + 2 * qd;
+#pragma unroll
+      for (int j = 0; j < NJ; ++j) {
+        const float2 r = __ldg(reinterpret_cast<const float2*>(rt + 8 * j)), c = __ldg(reinterpret_cast<const float2*>(ct + 8 * j));
+        pos[j][2 * i] = r.x + c.x; pos[j][2 * i + 1] = r.y + c.y;
       }
     }
-  } else if (warp == 6) {
-    // =============================== GEMM1 issuer (warp-converged, uniform operands) ===============================
-    constexpr uint32_t IDESC1 = idesc_tf32(TILE, KP, 0, 0);
-    mbar_wait(bar(&bars->m_full), 0);
-    tc_fence_after();
-    const uint64_t dM0 = umma_desc(s_m, 1024, LAYOUT_SW128);
-    const uint64_t dRing = umma_desc(s_ring1, 1024, LAYOUT_SW128);
-    int stage = 0; uint32_t ph = 0;
-    for (int it = 0; it < ntiles; ++it) {
-      const int buf = it & 1;
-      if (it >= 2) {                                                  // S[buf] was read by the row warps for tile it-2
-        mbar_wait(bar(&bars->s_free[buf]), (uint32_t)(((it - 2) >> 1) & 1));
-        tc_fence_after();
-      }
-      const uint32_t d_s = tmem + COL_S + buf * 32;
+    // ---- GEMM1 over all slabs; the slabs of this CTA's channel share are transposed into X^T meanwhile
+    float sacc[KP / 2];
 #pragma unroll 1
-      for (int s = 0; s < NS; ++s) {
-        mbar_wait(bar(&bars->full1[stage]), ph);
-        tc_fence_after();
-        const uint64_t da = dRing + (uint64_t)(stage * (SLAB_BYTES >> 4));
-        const uint64_t db = dM0 + (uint64_t)(s * ((KP * 128) >> 4));
+    for (int s = 0; s < NS; ++s) {
+      mbar_wait(smem_u32(&bars->full[stage]), ph);
+      const uint32_t sa = s_ring + stage * SLAB_BYTES;
+      const uint64_t da = gmma_desc(sa, 1024, LAYOUT_SW128);
+      const uint64_t db = dM + (uint64_t)(s * ((KP * 128) >> 4));
+      wgmma_fence();
 #pragma unroll
-        for (int kk = 0; kk < 4; ++kk) umma_ss_elect(d_s, da + kk * 2, db + kk * 2, IDESC1, (s | kk) ? 1u : 0u);
-        umma_commit_elect(bar(&bars->empty1[stage]));
-        if (++stage == nst1) { stage = 0; ph ^= 1u; }
+      for (int kk = 0; kk < 4; ++kk) {
+        if constexpr (KP == 32) wgmma_ss_n32(sacc, da + kk * 2, db + kk * 2, (s | kk) ? 1u : 0u);
+        else wgmma_ss_n16(sacc, da + kk * 2, db + kk * 2, (s | kk) ? 1u : 0u);
       }
-      umma_commit_elect(bar(&bars->s_full[buf]));
-    }
-  } else if (warp == 7) {
-    // =============================== GEMM2 issuer (warp-converged, uniform operands) ===============================
-    constexpr uint32_t IDESC2 = idesc_tf32(64, KP, 1, 0);             // A = X stage, MN-major; B = E^T, K-major
-    const uint64_t dRing = umma_desc_mn(s_ring2, SLAB_BYTES, 512);
-    const uint64_t dE0 = umma_desc(s_e, 1024, LAYOUT_SW128);
-    int stage = 0; uint32_t ph = 0;
-    for (int it = 0; it < ntiles; ++it) {
-      const int buf = it & 1;
-      mbar_wait(bar(&bars->e_full[buf]), (uint32_t)((it >> 1) & 1));
-      tc_fence_after();
-      const uint64_t de = dE0 + (uint64_t)(buf * (CF::E_BYTES >> 4));
-      const uint32_t acc0 = it ? 1u : 0u;
-#pragma unroll 1
-      for (int hg = 0; hg < NHG; ++hg) {
-        mbar_wait(bar(&bars->full2[stage]), ph);
-        tc_fence_after();
-        const uint64_t dx = dRing + (uint64_t)(stage * (HG_BYTES >> 4));
-        const uint32_t d2 = tmem + COL_D2 + hg * 32;
+      wgmma_commit();
+      const int cbase = s * SLAB_CH - zoff;
+      if (cbase >= 0 && cbase < C2) {
+        // thread: token tok = tid / 2, channels 16 (tid & 1) .. + 15 of the slab -> X^T[channel][token]
+        const int tok = tid >> 1, tch = tok >> 5, tin = tok & 31;
+        const uint8_t* src = smem + CF::OFF_RING + stage * SLAB_BYTES + tok * 128;
+        uint8_t* dstc = smem + CF::OFF_XT + tch * (C2 * 128);
 #pragma unroll
-        for (int kk = 0; kk < 16; ++kk)                               // 8 tokens (two 4-row swizzle atoms) per MMA
-          umma_ss_elect(d2, dx + (uint64_t)(kk * 64), de + (uint64_t)(((kk >> 2) * CF::E_CHUNK + (kk & 3) * 32) >> 4), IDESC2,
-                        kk ? 1u : acc0);
-        umma_commit_elect(bar(&bars->empty2[stage]));
-        if (++stage == nst2) { stage = 0; ph ^= 1u; }
+        for (int q4 = 0; q4 < 4; ++q4) {
+          const int c4 = (tid & 1) * 4 + q4;
+          const float4 v = *reinterpret_cast<const float4*>(src + ((c4 ^ (tok & 7)) << 4));
+          const float vv[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+          for (int e = 0; e < 4; ++e) {
+            const int cl = cbase + c4 * 4 + e;
+            *reinterpret_cast<float*>(dstc + cl * 128 + ((((tin >> 2) ^ (cl & 7))) << 4) + (tin & 3) * 4) = vv[e];
+          }
+        }
       }
-      umma_commit_elect(bar(&bars->e_free[buf]));
-    }
-    umma_commit_elect(bar(&bars->done));
-  } else {
-    // =============================== row warps ===============================
-    // One warp per scheduler and nothing to hide latency with: the loop is written for few instructions and no exposed
-    // loads -- next tile's positional logits are prefetched, references live in registers (pre-multiplied by log2 e),
-    // exp is one ex2.approx, the swizzled store offsets are precomputed.
-    const int q = warp & 3;                                         // TMEM lane quadrant == 32-token chunk of the tile
-    const int row = q * 32 + lane;
-    const uint32_t lane_addr = (uint32_t)(q * 32) << 16;
-    const int rtid = (warp - 2) * 32 + lane;                        // 0..127 inside the row-warp group
-    constexpr float LOG2E = 1.4426950408889634f;
-    auto load_pos = [&](int it, float* dst) {
-      const int tok = min((tile_beg + it) * TILE + row, P.n - 1);   // clamped: rows past a short image are masked
-      const int h = tok / P.W, w = tok - h * P.W;
-      const float4* rt = reinterpret_cast<const float4*>(P.Rt + ((size_t)b * P.H + h) * KP);
-      const float4* ct = reinterpret_cast<const float4*>(P.Ct + ((size_t)b * P.W + w) * KP);
-#pragma unroll
-      for (int j4 = 0; j4 < KP / 4; ++j4) {
-        const float4 r = __ldg(rt + j4), c = __ldg(ct + j4);
-        dst[j4 * 4 + 0] = r.x + c.x; dst[j4 * 4 + 1] = r.y + c.y; dst[j4 * 4 + 2] = r.z + c.z; dst[j4 * 4 + 3] = r.w + c.w;
-      }
-    };
-    float pos[KP];                                                  // positional logits of the current tile
-    float ml[KP];                                                   // running references * log2(e); padded latents: 0
-    float lsum[KP];                                                 // this token row's share of the softmax denominators
-    load_pos(0, pos);
-#pragma unroll
-    for (int j = 0; j < KP; ++j) { ml[j] = j < P.k ? -INFINITY : 0.f; lsum[j] = 0.f; }
-    uint32_t soff[8];                                               // byte offset of this token inside row j of a chunk
-#pragma unroll
-    for (int jj = 0; jj < 8; ++jj) soff[jj] = (uint32_t)((((lane >> 2) ^ jj) << 4) + (lane & 3) * 4);
-    for (int it = 0; it < ntiles; ++it) {
-      const int buf = it & 1;
-      const uint32_t bph = (uint32_t)((it >> 1) & 1);
-      mbar_wait(bar(&bars->s_full[buf]), bph);
-      tc_fence_after();
-      float sv[KP];
-      tmem_ld16(tmem + lane_addr + COL_S + buf * 32, sv);
-      if constexpr (KP == 32) tmem_ld16(tmem + lane_addr + COL_S + buf * 32 + 16, sv + 16);
-      tmem_wait_ld();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(bar(&bars->s_free[buf]));          // GEMM1 of tile it+2 may overwrite S[buf]
-      // t_j = (logit - reference) * log2(e); the trigger test needs only its maximum over this thread's latents
-      float ex = -INFINITY;
-      const bool valid = (tile_beg + it) * TILE + row < P.n;        // false only for the rows past a short image: E = 0
-#pragma unroll
-      for (int j = 0; j < KP; ++j) {
-        sv[j] = valid ? sv[j] + pos[j] : -INFINITY;      // logits in log2 units: log2 e is folded into M / Rt2 / Ct2 (gf_fold.cu)
-        ex = fmaxf(ex, sv[j] - ml[j]);                              // first tile: +inf -> trigger
-      }
-      if (it + 1 < ntiles) load_pos(it + 1, pos);                   // prefetch: consumed one tile later
-      const bool trig = __any_sync(0xffffffffu, ex > TAU * LOG2E);
-      if (lane == 0 && trig) trigf[buf] = 1;
-      if (rtid == 0) trigf[buf ^ 1] = 0;                            // clean flag for the next tile
+      wgmma_wait<0>();
       named_bar_sync(1, 128);
-      const bool full = trigf[buf] != 0;
-      if (full) {   // rare: some logit jumped more than TAU above its reference (always on the first tile)
-#pragma unroll
-        for (int j = 0; j < KP; ++j) {
-          float v = sv[j];
-#pragma unroll
-          for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
-          if (lane == 0) red[(warp - 2) * KP + j] = v;
-        }
-        named_bar_sync(1, 128);
-        if (rtid < KP) {
-          const float tm = fmaxf(fmaxf(red[rtid], red[KP + rtid]), fmaxf(red[2 * KP + rtid], red[3 * KP + rtid]));
-          const float mo = mref[rtid];                              // log2 units; -inf before the first tile
-          float mn = mo, f = 1.f;
-          if (rtid < P.k && (tm > mo + TAU * LOG2E || mo == -INFINITY)) {
-            mn = tm;
-            f = (mo == -INFINITY) ? 1.f : exp2f(mo - mn);
-          }
-          mref[rtid] = mn;
-          resc[rtid] = f;
-        }
-        named_bar_sync(1, 128);
-#pragma unroll
-        for (int j = 0; j < KP; ++j) { ml[j] = j < P.k ? mref[j] : 0.f; lsum[j] *= resc[j]; }
-      }
-      // ---- E = 2^(t_j) rounded to TF32 (so that the tensor core's operand truncation is exact and the register-side
-      //      denominators see the same values), written transposed (E^T[latent][token], K-major SW128, 32-token chunks).
-      // buffer `buf` was last read by GEMM2(it-2), whose completion this thread observed during tile it-1 (below)
-      uint8_t* eb = smem + CF::OFF_E + buf * CF::E_BYTES + q * CF::E_CHUNK;
-#pragma unroll
-      for (int j = 0; j < KP; ++j) {
-        float e;
-        asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e) : "f"(sv[j] - ml[j]));
-        e = cvt_tf32(e);
-        lsum[j] += e;
-        *reinterpret_cast<float*>(eb + j * 128 + soff[j & 7]) = e;
-      }
-      // ---- every tile: observe the completion of GEMM2(it-1) (parity bookkeeping must not skip phases); then, if a
-      //      running maximum moved, rescale the accumulators before GEMM2(it) adds to them
-      if (it > 0) {
-        mbar_wait(bar(&bars->e_free[buf ^ 1]), (uint32_t)(((it - 1) >> 1) & 1));
-        tc_fence_after();
-        if (rtid == 0) *g2done = it;                                  // GEMM2 of tiles < it complete: producer 1 may fetch tile it + lead
-      }
-      if (full && it > 0) {
-        // M=64 accumulators: channel c of a 64-channel block lives in TMEM lane (c % 16) + 32 * (c / 16): lanes 0-15 of
-        // every quadrant; columns = latents, so the factor varies along the columns
-        float v[16];
-#pragma unroll 1
-        for (int c0 = 0; c0 < NHG * 32; c0 += 32) {
-#pragma unroll
-          for (int hh = 0; hh < KP / 16; ++hh) {
-            tmem_ld16(tmem + lane_addr + COL_D2 + c0 + hh * 16, v);
-            tmem_wait_ld();
-#pragma unroll
-            for (int i = 0; i < 16; ++i) v[i] *= resc[hh * 16 + i];
-            tmem_st16(tmem + lane_addr + COL_D2 + c0 + hh * 16, v);
-          }
-        }
-        tmem_wait_st();
-      }
-      fence_proxy_async();                                          // E^T (generic proxy) -> tensor core (async proxy)
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(bar(&bars->e_full[buf]));
+      if (leader) mbar_arrive(smem_u32(&bars->empty[stage]));
+      if (++stage == nst) { stage = 0; ph ^= 1u; }
     }
-    // ---- flush: partial accumulators, running maxima and denominators of this split
+    fence_regs<KP / 2>(sacc);
+    // ---- logits (log2 units: log2 e is folded into M / Rt2 / Ct2, gf_fold.cu), column maxima over the tile's tokens
+    float cm[NJ][2];
 #pragma unroll
-    for (int j = 0; j < KP; ++j) {
-      float v = lsum[j];
+    for (int j = 0; j < NJ; ++j)
 #pragma unroll
-      for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-      if (lane == 0) red[(warp - 2) * KP + j] = v;
+      for (int e = 0; e < 2; ++e) {
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+          float& v = sacc[4 * j + 2 * i + e];
+          v = valid[i] ? v + pos[j][2 * i + e] : -INFINITY;
+        }
+        float m = fmaxf(sacc[4 * j + e], sacc[4 * j + 2 + e]);
+        m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 4));
+        m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 8));
+        m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 16));
+        cm[j][e] = m;
+      }
+    if (gid == 0)
+#pragma unroll
+      for (int j = 0; j < NJ; ++j) { red[w * KP + 8 * j + 2 * qd] = cm[j][0]; red[w * KP + 8 * j + 2 * qd + 1] = cm[j][1]; }
+    named_bar_sync(1, 128);
+    if (tid < KP) {
+      const float tm = fmaxf(fmaxf(red[tid], red[KP + tid]), fmaxf(red[2 * KP + tid], red[3 * KP + tid]));
+      const float mo = mref[tid];
+      float mn = mo, f = 1.f;
+      if (tid < P.k && tm > mo) { mn = tm; f = mo == -INFINITY ? 1.f : exp2f(mo - mn); }
+      mref[tid] = mn;
+      resc[tid] = f;
     }
     named_bar_sync(1, 128);
-    if (rtid < KP) {
-      const int j = rtid;
-      const float lj = red[j] + red[KP + j] + red[2 * KP + j] + red[3 * KP + j];
-      if (blockIdx.z == 0) {
-        part[(size_t)j * (C + 4) + C] = j < P.k ? mref[j] * 0.6931471805599453f : -INFINITY;   // log2 -> natural units
-        part[(size_t)j * (C + 4) + C + 1] = lj;
-        part[(size_t)j * (C + 4) + C + 2] = 0.f;
-        part[(size_t)j * (C + 4) + C + 3] = 0.f;
+    // ---- E = 2^(s - m) rounded to TF32 (the tensor core's operand truncation is then exact and the denominators see the same
+    //      values), written transposed: E^T[latent][token], K-major SW128, 32-token chunks
+#pragma unroll
+    for (int j = 0; j < NJ; ++j)
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const int col = 8 * j + 2 * qd + e;
+        const float mj = mref[col];
+        lp[j][e] *= resc[col];
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+          const int tok = 16 * w + gid + 8 * i, tch = tok >> 5, tin = tok & 31;
+          const float sv = sacc[4 * j + 2 * i + e];
+          const float ev = (col < P.k && valid[i]) ? cvt_tf32(exp2f(sv - mj)) : 0.f;
+          lp[j][e] += ev;
+          *reinterpret_cast<float*>(smem + CF::OFF_ET + tch * (64 * 128) + col * 128 + ((((tin >> 2) ^ (col & 7))) << 4) + (tin & 3) * 4) = ev;
+        }
       }
-      resc[j] = 1.f / lj;                          // (resc is free now) normalisation for the direct Xbar write
-    }
-    named_bar_sync(1, 128);
-    mbar_wait(bar(&bars->done), 0);
-    tc_fence_after();
+    // ---- rescale the accumulators whose maximum moved (rows = latents 16 w + gid, + 8)
     {
-      float v[16];
-#pragma unroll 1
-      for (int hg = 0; hg < NHG; ++hg) {
+      const int j0 = 16 * w + gid, j1 = j0 + 8;
+      const float f0 = j0 < KP ? resc[j0] : 1.f, f1 = j1 < KP ? resc[j1] : 1.f;
 #pragma unroll
-        for (int hh = 0; hh < KP / 16; ++hh) {
-          tmem_ld16(tmem + lane_addr + COL_D2 + hg * 32 + hh * 16, v);
-          tmem_wait_ld();
-          if (lane < 16) {
-            const int ch = zoff + hg * 64 + q * 16 + lane;
-            if (P.xbar) {        // single split: Xbar = acc / l (* load-side scale), no merge kernel
-              const float sc = 1.000352220f * (P.in_scale ? P.in_scale[(size_t)b * P.in_ld + ch] : 1.f);
-              float* dst = P.xbar + (size_t)b * P.k * C + ch;
+      for (int c = 0; c < NC2; ++c)
 #pragma unroll
-              for (int i = 0; i < 16; ++i)
-                if (hh * 16 + i < P.k) dst[(size_t)(hh * 16 + i) * C] = v[i] * sc * resc[hh * 16 + i];
-            } else {
-              float* dst = part + ch;
-#pragma unroll
-              for (int i = 0; i < 16; ++i) dst[(size_t)(hh * 16 + i) * (C + 4)] = v[i] * 1.000352220f;   // X truncation bias (gf_fold.cu)
-            }
-          }
+        for (int jb = 0; jb < 4; ++jb) {
+          acc2[c][4 * jb] *= f0; acc2[c][4 * jb + 1] *= f0; acc2[c][4 * jb + 2] *= f1; acc2[c][4 * jb + 3] *= f1;
         }
+    }
+    fence_proxy_async();                      // E^T and X^T (generic proxy) -> wgmma (async proxy)
+    named_bar_sync(1, 128);
+    // ---- GEMM2: D += E^T . X over the tile's 64 tokens (8 k-blocks: two 32-token chunks of 4)
+#pragma unroll
+    for (int c = 0; c < NC2; ++c) fence_regs<16>(acc2[c]);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < 8; ++kk) {
+      const uint64_t da = gmma_desc(s_et + (kk >> 2) * (64 * 128) + (kk & 3) * 32, 1024, LAYOUT_SW128);
+#pragma unroll
+      for (int c = 0; c < NC2; ++c) {
+        const uint64_t db = gmma_desc(s_xt + (kk >> 2) * (C2 * 128) + c * (32 * 128) + (kk & 3) * 32, 1024, LAYOUT_SW128);
+        wgmma_ss_n32(acc2[c], da, db, 1u);
       }
     }
+    wgmma_commit();
+    wgmma_wait<0>();
+#pragma unroll
+    for (int c = 0; c < NC2; ++c) fence_regs<16>(acc2[c]);
+    named_bar_sync(1, 128);                   // E^T / X^T may be rewritten by the next tile
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 6) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "n"(TMEM_COLS) : "memory");
+  // ---- flush: partial accumulators, running maxima and denominators of this split
+#pragma unroll
+  for (int j = 0; j < NJ; ++j)
+#pragma unroll
+    for (int e = 0; e < 2; ++e) {
+      float v = lp[j][e];
+      v += __shfl_xor_sync(0xffffffffu, v, 4);
+      v += __shfl_xor_sync(0xffffffffu, v, 8);
+      v += __shfl_xor_sync(0xffffffffu, v, 16);
+      if (gid == 0) red[w * KP + 8 * j + 2 * qd + e] = v;
+    }
+  named_bar_sync(1, 128);
+  if (tid < KP && blockIdx.z == 0) {
+    const int j = tid;
+    part[(size_t)j * (C + 4) + C] = j < P.k ? mref[j] * 0.6931471805599453f : -INFINITY;   // log2 -> natural units
+    part[(size_t)j * (C + 4) + C + 1] = red[j] + red[KP + j] + red[2 * KP + j] + red[3 * KP + j];
+    part[(size_t)j * (C + 4) + C + 2] = 0.f;
+    part[(size_t)j * (C + 4) + C + 3] = 0.f;
+  }
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    const int j = 16 * w + gid + 8 * i;
+    if (j < KP) {
+      float* dst = part + (size_t)j * (C + 4) + zoff + 2 * qd;
+#pragma unroll
+      for (int c = 0; c < NC2; ++c)
+#pragma unroll
+        for (int jb = 0; jb < 4; ++jb)          // X truncation bias of the tensor core (gf_fold.cu)
+          *reinterpret_cast<float2*>(dst + c * 32 + 8 * jb) =
+              make_float2(acc2[c][4 * jb + 2 * i] * 1.000352220f, acc2[c][4 * jb + 2 * i + 1] * 1.000352220f);
+    }
   }
 }
 
 template <int KP, int NS>
-static void stages_for(int smem_limit, int* n1, int* n2) {
-  const int avail = smem_limit - Cfg<KP, NS>::FIXED_BYTES - 1024;
-  int s2 = 2, s1 = (avail - s2 * HG_BYTES) / SLAB_BYTES;
-  if (s1 > MAX_ST1) {                                         // room to spare: deepen ring 2 first
-    s2 = MAX_ST2;
-    s1 = (avail - s2 * HG_BYTES) / SLAB_BYTES;
-    if (s1 > MAX_ST1) s1 = MAX_ST1;
-    if (s1 < 6) { s2 = 2; s1 = (avail - s2 * HG_BYTES) / SLAB_BYTES; if (s1 > MAX_ST1) s1 = MAX_ST1; }
-  }
-  *n1 = s1; *n2 = s2;
+static int stages_for(int smem_limit) {
+  const int s = (smem_limit - Cfg<KP, NS>::FIXED_BYTES - 1024) / SLAB_BYTES;
+  return s > MAX_ST ? MAX_ST : s;
 }
 
 template <int KP, int NS>
-static int launch(const Layout& L, const float* X, float* ws, cudaStream_t st, const float* in_scale, int in_scale_ld) {
+static int launch(const Layout& L, const float* X, float* ws, cudaStream_t st) {
   using CF = Cfg<KP, NS>;
   constexpr int NS2 = NS > 8 ? NS / 2 : NS;
-  int n1, n2;
-  stages_for<KP, NS>(device_smem_optin(), &n1, &n2);
-  if (n1 < 2) { set_error("tcgen05 centroid pass: shared memory too small for C=%d KP=%d", L.C, KP); return GF_ERR_UNSUPPORTED; }
-  CUtensorMap tmX, tmX2, tmM;
+  const int nst = stages_for<KP, NS>(device_smem_optin());
+  if (nst < 2) { set_error("tensor-core centroid pass: shared memory too small for C=%d KP=%d", L.C, KP); return GF_ERR_UNSUPPORTED; }
+  CUtensorMap tmX, tmM;
   int rc;
   if ((rc = make_map(&tmX, X, (uint64_t)L.B * L.n, L.C, TILE, SLAB_CH, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
-  if ((rc = make_map(&tmX2, X, (uint64_t)L.B * L.n, L.C, TILE, SLAB_CH, CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B))) return rc;
   if ((rc = make_map(&tmM, ws + L.w_M, (uint64_t)L.B * KP, L.C, KP, SLAB_CH, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
   Params P;
   P.Rt = ws + L.w_Rt2; P.Ct = ws + L.w_Ct2; P.part = ws + L.w_PART;
-  P.xbar = L.nsplit_cen == 1 ? ws + L.w_XBAR : nullptr; P.in_scale = in_scale; P.in_ld = in_scale_ld;
   P.n = L.n; P.H = L.H; P.W = L.W; P.k = L.k; P.nsplit = L.nsplit_cen; P.tiles_per_image = (L.n + TILE - 1) / TILE;
-  P.nst1 = n1; P.nst2 = n2;
-  {
-    // L2 reuse-distance budget of the ring-2 re-fetch: (lead - 1/2) tiles x tile bytes x resident CTAs <= ~30 MB
-    static const int forced = []() { const char* e = getenv("GF_CEN_LEAD"); return e ? atoi(e) : 0; }();   // tuning aid, read once
-    const long long ctas = (long long)L.nsplit_cen * L.B * (NS / NS2);
-    const double resident = (double)(ctas < num_sms() ? ctas : num_sms());
-    int lead = (int)(30.0e6 / ((double)TILE * L.C * 4 * resident) + 0.5);
-    if (NS > 8) lead = 1 << 20;            // C = 512: ring 1 holds half a tile and cannot run ahead (measured: no re-fetch misses)
-    P.lead = forced > 0 ? forced : (lead < 2 ? 2 : (lead > 8 && NS <= 8 ? 8 : lead));
-  }
-  const int smem_bytes = CF::FIXED_BYTES + n1 * SLAB_BYTES + n2 * HG_BYTES + 1024;
-#ifdef GF_DEBUG_WATCHDOG     // bring-up builds only (-DGF_DEBUG_WATCHDOG): a host-pinned buffer that records where a barrier wait timed out
-#ifdef GF_DEBUG_WATCHDOG     // bring-up builds only: record where a barrier wait timed out (tools/hang_debug.py)
-  if (const char* dbg = getenv("GF_DEBUG_PTR")) tc::set_debug_buffer(reinterpret_cast<unsigned int*>(strtoull(dbg, nullptr, 0)));
-#endif
-#endif
+  P.nst = nst;
+  const int smem_bytes = CF::FIXED_BYTES + nst * SLAB_BYTES + 1024;
   auto kern = centroid_tc_kernel<KP, NS, NS2>;
   GF_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
-  kern<<<dim3(L.nsplit_cen, L.B, NS / NS2), NUM_THREADS, smem_bytes, st>>>(tmX, tmX2, tmM, P);
+  kern<<<dim3(L.nsplit_cen, L.B, NS / NS2), NUM_THREADS, smem_bytes, st>>>(tmX, tmM, P);
   GF_LAUNCH_OK();
   return GF_OK;
 }
 
 template <int KP, int NS>
-static bool fits(int limit) { int n1, n2; stages_for<KP, NS>(limit, &n1, &n2); return n1 >= 2; }
+static bool fits(int limit) { return stages_for<KP, NS>(limit) >= 2; }
+
+template <int KP>
+static bool fits_ns(int ns, int limit) {
+  return ns == 2 ? fits<KP, 2>(limit) : ns == 4 ? fits<KP, 4>(limit) : ns == 8 ? fits<KP, 8>(limit) : fits<KP, 16>(limit);
+}
+
+template <int KP>
+static int launch_ns(int ns, const Layout& L, const float* X, float* ws, cudaStream_t st) {
+  return ns == 2 ? launch<KP, 2>(L, X, ws, st) : ns == 4 ? launch<KP, 4>(L, X, ws, st) : ns == 8 ? launch<KP, 8>(L, X, ws, st) : launch<KP, 16>(L, X, ws, st);
+}
 
 }  // namespace tcc
 
 bool tc_centroid_supported(const Layout& L, const gf_attn_desc* d) {
-  static const bool disabled = getenv("GF_DISABLE_TC") != nullptr || getenv("GF_DISABLE_TC_CENTROID") != nullptr;
-  if (disabled || (d->flags & GF_FLAG_FP32_EXACT)) return false;
+  if (d->flags & GF_FLAG_FP32_EXACT) return false;
   if (L.C != 64 && L.C != 128 && L.C != 256 && L.C != 512) return false;   // C = 512: two CTAs share the channels
-  if ((L.n % tcc::TILE != 0 && !(L.n < tcc::TILE && L.n % 8 == 0)) || L.B > 65535) return false;
-  if ((long long)L.B * L.n > 0x7fffffffll) return false;
+  if (L.B > 65535 || (long long)L.B * L.n > 0x7fffffffll) return false;
   const int limit = tc::device_smem_optin();
-  const int ns = L.C / 32;
-  if (L.KP == 16) return ns == 2 ? tcc::fits<16, 2>(limit) : ns == 4 ? tcc::fits<16, 4>(limit) : ns == 8 ? tcc::fits<16, 8>(limit) : tcc::fits<16, 16>(limit);
-  return ns == 2 ? tcc::fits<32, 2>(limit) : ns == 4 ? tcc::fits<32, 4>(limit) : ns == 8 ? tcc::fits<32, 8>(limit) : tcc::fits<32, 16>(limit);
+  return L.KP == 16 ? tcc::fits_ns<16>(L.C / 32, limit) : tcc::fits_ns<32>(L.C / 32, limit);
 }
 
-int centroid_pass_tc(const Layout& L, const gf_attn_desc* d, const float* X, float* ws, cudaStream_t st, const float* in_scale, int in_scale_ld) {
-  (void)d;
-  const int ns = L.C / 32;
-  if (L.KP == 16) return ns == 2 ? tcc::launch<16, 2>(L, X, ws, st, in_scale, in_scale_ld) : ns == 4 ? tcc::launch<16, 4>(L, X, ws, st, in_scale, in_scale_ld) : ns == 8 ? tcc::launch<16, 8>(L, X, ws, st, in_scale, in_scale_ld) : tcc::launch<16, 16>(L, X, ws, st, in_scale, in_scale_ld);
-  return ns == 2 ? tcc::launch<32, 2>(L, X, ws, st, in_scale, in_scale_ld) : ns == 4 ? tcc::launch<32, 4>(L, X, ws, st, in_scale, in_scale_ld) : ns == 8 ? tcc::launch<32, 8>(L, X, ws, st, in_scale, in_scale_ld) : tcc::launch<32, 16>(L, X, ws, st, in_scale, in_scale_ld);
+int centroid_pass_tc(const Layout& L, const float* X, float* ws, cudaStream_t st) {
+  return L.KP == 16 ? tcc::launch_ns<16>(L.C / 32, L, X, ws, st) : tcc::launch_ns<32>(L.C / 32, L, X, ws, st);
 }
 
 }  // namespace gf

@@ -2,13 +2,12 @@
 //     C[M,N] = alpha * A[M,K] . B[K,N] + E[(row % emod), :] + v[:]          (A, B row-major, lda = K, ldb = N)
 // used (TF32 mode only) for KPALL = keys . AK + CK, MALL = Y . AM + CM and the duplex centroids Xbar . Wv2 + bv2
 // (reference side, expected src/training/network.py: the K / V dense_layer calls of transformer_layer).  M = B*k is a few
-// thousand rows, so the CUDA-core SGEMM (gf_fold.cu) spent ~50 us per product at C = 512 -- a third of a small duplex
-// layer.  One 128 x 64 output tile per CTA, BK = 32:
-//   warp 0  TMA producer: A tile [128 x 32] SWIZZLE_128B (K-major operand), B tile [32 x 64] as two [32 x 32] boxes with
-//           SWIZZLE_128B_ATOM_32B (B is row-major [K,N] = MN-major for the tensor core; see gf_tc_cen.cu)
-//   warp 1  MMA issuer, warp-converged (uniform-register descriptors): 4 tcgen05.mma (M=128, N=64, K=8) per stage
-//   warps 2-5  epilogue: TMEM -> registers -> alpha, bias rows -> global (thread = output row)
-// Out-of-range rows / columns / k are zero-filled by TMA and masked at the store.  Operands are truncated to TF32 by the
+// thousand rows, far too few for the CUDA-core SGEMM (gf_fold.cu) to fill the GPU at C = 512.
+// One 64 x 64 output tile per CTA (one warpgroup), BK = 32, two shared-memory buffers:
+//   all 128 threads stage the next A tile [64 x 32] and the next B tile TRANSPOSED to [64 n x 32 k] (wgmma takes 32-bit
+//   operands K-major only; B row-major [K,N] is N-major) into 128-byte-swizzled K-major layouts while the current
+//   tile's 8 wgmma m64n32k8 run; the epilogue goes from registers to global (alpha, bias rows).
+// Out-of-range rows / columns / k are zero-filled at staging and masked at the store.  Operands are truncated to TF32 by the
 // tensor core; alpha carries the mean-truncation compensation of both operands (gf_fold.cu: GF_TF32_TRUNC_COMP).
 #include <stdlib.h>
 #include "gf_common.cuh"
@@ -19,140 +18,106 @@ namespace tcg {
 
 using namespace tc;
 
-constexpr int BM = 128, BN = 64, BK = 32;
-constexpr int A_BYTES = BM * BK * 4;               // 16 KB
-constexpr int B_BYTES = BK * BN * 4;               // 8 KB: two 4 KB blocks of 32 n
-constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-constexpr int NSTAGES = 6;
-constexpr int NUM_THREADS = 192;
-constexpr int TMEM_COLS = 64;
+constexpr int BM = 64, BN = 64, BK = 32;
+constexpr int TILE_BYTES = 64 * 128;              // [64 rows x 32 fp32], either operand
+constexpr int NUM_THREADS = 128;
 
-struct Bars {
-  uint64_t full[NSTAGES], empty[NSTAGES];
-  uint64_t acc_full;
-  uint32_t tmem_base, pad;
-};
-
-__device__ __forceinline__ uint64_t desc_mn(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr >> 4) & 0x3FFF);
-  d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
-  d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)1 << 61;                          // SWIZZLE_128B_BASE32B
-  return d;
+__device__ __forceinline__ uint32_t sw_off(int row, int k) {    // K-major SWIZZLE_128B offset of (row, k), k < 32
+  return (uint32_t)(row * 128 + ((((k >> 2) ^ (row & 7))) << 4) + (k & 3) * 4);
 }
 
-__global__ void __launch_bounds__(NUM_THREADS, 1)
-gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, float* __restrict__ Cm, int ldc,
+__global__ void __launch_bounds__(NUM_THREADS)
+gemm_tc_kernel(const float* __restrict__ A, const float* __restrict__ B, float* __restrict__ Cm, int ldc,
                int M, int N, int K, float alpha, const float* __restrict__ E, int lde, int emod, const float* __restrict__ v) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  const uint32_t pad = (1024u - (smem_u32(smem_raw) & 1023u)) & 1023u;
-  const uint32_t s_base = smem_u32(smem_raw) + pad;
-  Bars* bars = reinterpret_cast<Bars*>(smem_raw + pad + NSTAGES * STAGE_BYTES);
-  const uint32_t s_bars = s_base + NSTAGES * STAGE_BYTES;
-  auto bar = [&](const void* p) -> uint32_t { return s_bars + (uint32_t)((const uint8_t*)p - (const uint8_t*)bars); };
-  const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);
-  const int lane = threadIdx.x & 31;
+  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
+  const uint32_t s_base = smem_u32(smem);                      // [buf][A | B]
+  const int tid = threadIdx.x, w = tid >> 5, lane = tid & 31, gid = lane >> 2, qd = lane & 3;
   const int n0 = blockIdx.x * BN, m0 = blockIdx.y * BM;
   const int nk = (K + BK - 1) / BK;
 
-  if (warp == 0 && lane == 0) {
-    prefetch_tmap(&tmA); prefetch_tmap(&tmB);
-    for (int i = 0; i < NSTAGES; ++i) { mbar_init(bar(&bars->full[i]), 1); mbar_init(bar(&bars->empty[i]), 1); }
-    mbar_init(bar(&bars->acc_full), 1);
-    fence_barrier_init();
-  }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(bar(&bars->tmem_base)), "n"(TMEM_COLS) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = __shfl_sync(0xffffffffu, bars->tmem_base, 0);
-
-  if (warp == 0) {
-    if (lane == 0) {
-      int stage = 0; uint32_t ph = 0;
-      for (int kt = 0; kt < nk; ++kt) {
-        mbar_wait(bar(&bars->empty[stage]), ph ^ 1u);
-        const uint32_t fb = bar(&bars->full[stage]);
-        const uint32_t sa = s_base + stage * STAGE_BYTES;
-        mbar_expect_tx(fb, STAGE_BYTES);
-        tma_load_2d(sa, &tmA, fb, kt * BK, m0);
-        tma_load_2d(sa + A_BYTES, &tmB, fb, n0, kt * BK);
-        tma_load_2d(sa + A_BYTES + 4096, &tmB, fb, n0 + 32, kt * BK);
-        if (++stage == NSTAGES) { stage = 0; ph ^= 1u; }
-      }
-    }
-  } else if (warp == 1) {
-    // instruction descriptor: tf32 x tf32 -> f32, A K-major, B MN-major, N = 64, M = 128
-    constexpr uint32_t IDESC = (1u << 4) | (2u << 7) | (2u << 10) | (1u << 16) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);
-    const uint64_t dA0 = umma_desc(s_base, 1024, LAYOUT_SW128);
-    const uint64_t dB0 = desc_mn(s_base + A_BYTES, 4096, 512);
-    int stage = 0; uint32_t ph = 0;
-    for (int kt = 0; kt < nk; ++kt) {
-      mbar_wait(bar(&bars->full[stage]), ph);
-      tc_fence_after();
-      const uint64_t da = dA0 + (uint64_t)(stage * (STAGE_BYTES >> 4));
-      const uint64_t db = dB0 + (uint64_t)(stage * (STAGE_BYTES >> 4));
+  float4 ra[4], rb[4];
+  auto load = [&](int kt) {
+    const int k0 = kt * BK;
 #pragma unroll
-      for (int kk = 0; kk < 4; ++kk) umma_ss_elect(tmem, da + kk * 2, db + (uint64_t)(kk * 64), IDESC, (kt | kk) ? 1u : 0u);
-      umma_commit_elect(bar(&bars->empty[stage]));
-      if (++stage == NSTAGES) { stage = 0; ph ^= 1u; }
+    for (int i = 0; i < 4; ++i) {
+      const int idx = tid + NUM_THREADS * i;
+      const int ar = idx >> 3, ac = (idx & 7) * 4;              // A: row, first k
+      ra[i] = (m0 + ar < M && k0 + ac < K) ? __ldg(reinterpret_cast<const float4*>(A + (size_t)(m0 + ar) * K + k0 + ac))
+                                           : make_float4(0.f, 0.f, 0.f, 0.f);
+      const int bk = idx >> 4, bn = (idx & 15) * 4;             // B: k row, first n
+      rb[i] = (k0 + bk < K && n0 + bn < N) ? __ldg(reinterpret_cast<const float4*>(B + (size_t)(k0 + bk) * N + n0 + bn))
+                                           : make_float4(0.f, 0.f, 0.f, 0.f);
     }
-    umma_commit_elect(bar(&bars->acc_full));
-  } else {
-    const int q = warp & 3;
-    const int row = m0 + q * 32 + lane;
-    const uint32_t lane_addr = (uint32_t)(q * 32) << 16;
-    mbar_wait(bar(&bars->acc_full), 0);
-    tc_fence_after();
+  };
+  auto store = [&](int buf) {
+    uint8_t* sa = smem + buf * 2 * TILE_BYTES;
+    uint8_t* sb = sa + TILE_BYTES;
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const int idx = tid + NUM_THREADS * i;
+      const int ar = idx >> 3, ac = (idx & 7) * 4;
+      *reinterpret_cast<float4*>(sa + sw_off(ar, ac)) = ra[i];
+      const int bk = idx >> 4, bn = (idx & 15) * 4;
+      *reinterpret_cast<float*>(sb + sw_off(bn, bk)) = rb[i].x;
+      *reinterpret_cast<float*>(sb + sw_off(bn + 1, bk)) = rb[i].y;
+      *reinterpret_cast<float*>(sb + sw_off(bn + 2, bk)) = rb[i].z;
+      *reinterpret_cast<float*>(sb + sw_off(bn + 3, bk)) = rb[i].w;
+    }
+    fence_proxy_async();                                         // generic-proxy writes -> wgmma (async proxy)
+  };
+
+  float acc[2][16];
+#pragma unroll
+  for (int h = 0; h < 2; ++h)
+#pragma unroll
+    for (int i = 0; i < 16; ++i) acc[h][i] = 0.f;
+  load(0);
+  store(0);
+  __syncthreads();
+  for (int kt = 0; kt < nk; ++kt) {
+    const int buf = kt & 1;
+    const uint32_t sa = s_base + buf * 2 * TILE_BYTES, sb = sa + TILE_BYTES;
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) {
+      const uint64_t da = gmma_desc(sa + kk * 32, 1024, LAYOUT_SW128);
+      wgmma_ss_n32(acc[0], da, gmma_desc(sb + kk * 32, 1024, LAYOUT_SW128), 1u);
+      wgmma_ss_n32(acc[1], da, gmma_desc(sb + 32 * 128 + kk * 32, 1024, LAYOUT_SW128), 1u);
+    }
+    wgmma_commit();
+    if (kt + 1 < nk) {                                           // the other buffer was released by the barrier of the last step
+      load(kt + 1);
+      store(buf ^ 1);
+    }
+    wgmma_wait<0>();
+    __syncthreads();
+  }
+  fence_regs<16>(acc[0]); fence_regs<16>(acc[1]);
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    const int row = m0 + 16 * w + gid + 8 * i;
+    if (row >= M) continue;
     const float* erow = E ? E + (size_t)(row % emod) * lde : nullptr;
     float* crow = Cm + (size_t)row * ldc;
-#pragma unroll 1
-    for (int c0 = 0; c0 < BN; c0 += 16) {
-      float acc[16];
-      tmem_ld16(tmem + lane_addr + c0, acc);
-      tmem_wait_ld();
-      if (row < M) {
-        const int cb = n0 + c0;
-        if (cb + 16 <= N && (ldc & 3) == 0) {
 #pragma unroll
-          for (int i4 = 0; i4 < 4; ++i4) {
-            float4 r;
-            r.x = alpha * acc[i4 * 4 + 0]; r.y = alpha * acc[i4 * 4 + 1]; r.z = alpha * acc[i4 * 4 + 2]; r.w = alpha * acc[i4 * 4 + 3];
-            const int c = cb + i4 * 4;
-            if (erow) { r.x += erow[c]; r.y += erow[c + 1]; r.z += erow[c + 2]; r.w += erow[c + 3]; }
-            if (v) { r.x += v[c]; r.y += v[c + 1]; r.z += v[c + 2]; r.w += v[c + 3]; }
-            *reinterpret_cast<float4*>(crow + c) = r;
-          }
-        } else {
+    for (int h = 0; h < 2; ++h)
 #pragma unroll
-          for (int i = 0; i < 16; ++i) {
-            const int c = cb + i;
-            if (c < N) crow[c] = alpha * acc[i] + (erow ? erow[c] : 0.f) + (v ? v[c] : 0.f);
-          }
+      for (int jb = 0; jb < 4; ++jb)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int c = n0 + h * 32 + 8 * jb + 2 * qd + e;
+          if (c < N) crow[c] = alpha * acc[h][4 * jb + 2 * i + e] + (erow ? erow[c] : 0.f) + (v ? v[c] : 0.f);
         }
-      }
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "n"(TMEM_COLS) : "memory");
   }
 }
 
 }  // namespace tcg
 
-// lda == K and ldb == N (dense row-major operands); returns GF_ERR_UNSUPPORTED when the shape cannot be described to TMA
+// lda == K and ldb == N (dense row-major operands), rows of A and B 16-byte aligned
 bool gemm_tc_ok(int M, int N, int K, const float* A, const float* B, const float* Cm, int ldc) {
-  static const bool disabled = getenv("GF_DISABLE_TC") != nullptr || getenv("GF_DISABLE_TC_GEMM") != nullptr;
-  if (disabled || M < 1 || N < 32 || K < 4) return false;
-  if ((K & 3) || (N & 3)) return false;                                   // TMA: row strides are multiples of 16 bytes
+  if (M < 1 || N < 32 || K < 4) return false;
+  if ((K & 3) || (N & 3)) return false;
   if (((uintptr_t)A & 15) || ((uintptr_t)B & 15) || ((uintptr_t)Cm & 15) || (ldc & 3)) return false;
   return true;
 }
@@ -160,16 +125,12 @@ bool gemm_tc_ok(int M, int N, int K, const float* A, const float* B, const float
 int gemm_tc(cudaStream_t st, int M, int N, int K, const float* A, const float* B, float* Cm, int ldc, float alpha,
             const float* E, int lde, int emod, const float* v) {
   using namespace tcg;
-  CUtensorMap tmA, tmB;
-  int rc;
-  if ((rc = tc::make_map(&tmA, A, (uint64_t)M, (uint64_t)K, BM, BK, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
-  if ((rc = tc::make_map(&tmB, B, (uint64_t)K, (uint64_t)N, BK, 32, CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B))) return rc;
-  const int smem_bytes = NSTAGES * STAGE_BYTES + (int)sizeof(Bars) + 1024;
-  GF_CUDA_OK(cudaFuncSetAttribute(gemm_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));   // per device: set on every call
+  const int smem_bytes = 4 * TILE_BYTES + 1024;
+  GF_CUDA_OK(cudaFuncSetAttribute(gemm_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
   if (emod < 1) emod = 1;
   // both operands are truncated to TF32 by the tensor core: compensate the mean truncation bias of each (0.7213 * 2^-11)
   const float comp = 1.000352220f * 1.000352220f;
-  gemm_tc_kernel<<<dim3((N + BN - 1) / BN, (M + BM - 1) / BM), NUM_THREADS, smem_bytes, st>>>(tmA, tmB, Cm, ldc, M, N, K, alpha * comp, E, lde, emod, v);
+  gemm_tc_kernel<<<dim3((N + BN - 1) / BN, (M + BM - 1) / BM), NUM_THREADS, smem_bytes, st>>>(A, B, Cm, ldc, M, N, K, alpha * comp, E, lde, emod, v);
   GF_LAUNCH_OK();
   return GF_OK;
 }

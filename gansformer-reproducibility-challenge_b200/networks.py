@@ -79,7 +79,7 @@ def modulated_conv2d(x: torch.Tensor, weight: torch.Tensor, styles: torch.Tensor
 
     Identical in exact arithmetic to modulating the weights per sample (the reference's grouped-conv form);
     avoids B separate weight tensors.  weight [O, I, kh, kw]; styles [B, I].  The two scalings and the FIR blur of the
-    upsampling path are the native ops of ops.py (gf_ops.h).  The stride-1 3x3 convolution runs on the library's own tcgen05
+    upsampling path are the native ops of ops.py (gf_ops.h).  The stride-1 3x3 convolution runs on the library's own wgmma
     implicit-GEMM kernel (wt_packed, row f1) when TF32 convolutions are allowed and the shape is eligible, else on cuDNN; the
     polyphase up-convolutions are cuDNN.
     w_eff / wsq: optional cached equalised-LR weight (already transposed for up=2) and its squared sum over the taps.
@@ -98,7 +98,7 @@ def modulated_conv2d(x: torch.Tensor, weight: torch.Tensor, styles: torch.Tensor
         x = ops.chan_scale(x, styles)
     if up == 1:
         if wt_packed is not None:
-            x = ops.conv3x3_native(x, wt_packed)                      # row f1: own tcgen05 implicit-GEMM kernel (TF32)
+            x = ops.conv3x3_native(x, wt_packed)                      # row f1: own wgmma implicit-GEMM kernel (TF32)
         else:
             x = F.conv2d(x, w_eff, padding=kh // 2)
         if defer_demod:
@@ -225,7 +225,7 @@ class SynthesisLayer(nn.Module):
         """prescaled: x already carries this layer's style scale.  post_scale [B,C]: the NEXT convolution's style scale,
         folded into this layer's store (only honoured -- and only passed by SynthesisNetwork -- when `fusable`).
         rgb: dict(rgb_w [B,3,C], rgb_bias [3], rgb_out [B,3,H,W]) -- the block's tRGB computed by the attention kernel's store side
-        from the layer output (fused path on the tcgen05 kernel only; SynthesisNetwork checks)."""
+        from the layer output (fused path on the wgmma kernel only; SynthesisNetwork checks)."""
         if styles is None:
             styles = self.affine(w_glob)
         w_eff = wsq = phases = packed = None
@@ -397,7 +397,7 @@ class SynthesisNetwork(nn.Module):
                     post_scale = styles_all[li + 1]
                 rgb_args = None
                 if j == nl - 1 and layer.fusable(x) and not return_features and not os.environ.get("GF_NO_TORGB_EPILOGUE"):
-                    # last layer of the block on the tcgen05 path (C <= 256, or 512 with k <= 16): the attention kernel's store side computes the
+                    # last layer of the block on the wgmma path (C <= 256, or 512 with k <= 16): the attention kernel's store side computes the
                     # tRGB planes from the layer output and writes x * (next block's style): the tRGB pass disappears
                     C_ = layer.weight.shape[0]
                     tg = self.torgbs[bi]

@@ -1,4 +1,4 @@
-"""Host wrappers of the memory-bound companion ops (include/gf_ops.h): the B200-native equivalents of the
+"""Host wrappers of the memory-bound companion ops (include/gf_ops.h): the sm_90a equivalents of the
 reference's native ops ``dnnlib/tflib/ops/upfirdn_2d.cu`` and ``fused_bias_act.cu`` (expected upstream; not in the
 checkout) in the forms the generator uses, plus channel scaling (style modulation / demodulation).
 
@@ -331,7 +331,7 @@ def conv3x3_pack(weight: torch.Tensor, scale: float = 1.0) -> torch.Tensor:
 
 
 def conv3x3_native(x: torch.Tensor, wt: torch.Tensor) -> torch.Tensor:
-    """3x3 stride-1 zero-padded convolution on the tcgen05 implicit-GEMM kernel (row f1, TF32): x [B, I, H, W] (channels-last
+    """3x3 stride-1 zero-padded convolution on the wgmma implicit-GEMM kernel (row f1, TF32): x [B, I, H, W] (channels-last
     storage), wt from conv3x3_pack -> [B, O, H, W] (channels-last storage).  CUDA fp32 inference only."""
     xv = _nhwc_view(x)
     B, H, W, I = xv.shape

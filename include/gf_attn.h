@@ -1,5 +1,5 @@
 /*
- * gf_attn.h -- C ABI of the B200-native GANsformer bipartite-attention hot path.
+ * gf_attn.h -- C ABI of the H100 (sm_90a) GANsformer bipartite-attention hot path.
  *
  * Drop-in boundary (SURVEY.md section 8b).  The reference has no FFI for this path: its attention block
  * is Python/TensorFlow graph code, expected at src/training/network.py (transformer_layer, integrate,
@@ -43,7 +43,7 @@ enum { GF_NORM_NONE = 0, GF_NORM_LAYER = 1, GF_NORM_INSTANCE = 2, GF_NORM_BATCH 
 enum { GF_INT_MUL = 0, GF_INT_ADD = 1, GF_INT_BOTH = 2 };
 /* desc.flags */
 enum {
-  GF_FLAG_FP32_EXACT = 1,   /* force the CUDA-core fp32-FMA kernel (tight-tolerance mode); default = tcgen05 TF32 */
+  GF_FLAG_FP32_EXACT = 1,   /* force the CUDA-core fp32-FMA kernel (tight-tolerance mode); default = wgmma TF32 */
   GF_FLAG_CENTROIDS_IN = 2, /* duplex: skip pass A, take centroids_inout as input (iterative=True upstream) */
   GF_FLAG_TABLES_READY = 4, /* duplex: the pass-A query tables and V^T are already in ws (gf_attn_prologue_batch ran for this layer) */
   GF_FLAG_CENTROIDS_INIT = 16, /* duplex: `iterative` -- centroids_inout holds the previous attention layer's centroids on entry; the
@@ -53,7 +53,7 @@ enum {
                                Y <- LN(Y) (1 + dense(Cen, wi2l) + bi2l); values of pass B from the modulated latents */
 };
 /* which kernel family served the last forward on this thread (gf_attn_last_path) */
-enum { GF_PATH_NONE = 0, GF_PATH_SIMT_FP32 = 1, GF_PATH_TCGEN05_TF32 = 2 };
+enum { GF_PATH_NONE = 0, GF_PATH_SIMT_FP32 = 1, GF_PATH_WGMMA_TF32 = 2 };
 
 /* Shape/config of one attention layer call.  Mirrors the kwargs of the reference's
  * transformer_layer(dim, pos_dim, from_tensor, to_tensor, from_len, to_len, num_heads, integration, norm, kmeans...) */
@@ -89,7 +89,7 @@ typedef struct gf_attn_postop {
   /* fused tRGB (the 1x1 modulated convolution, no demodulation, that follows the last layer of a resolution block):
    *   rgb_out[b][o][t] = sum_c x''[b,t,c] * rgb_w[b][o][c] + rgb_bias[o],  o < 3,  x'' = the layer output BEFORE post_scale.
    * rgb_w [B][3][C] contiguous (weight * style * 1/sqrt(C) per sample), 16-byte aligned; rgb_bias [3] or NULL; rgb_out [B][3][H*W]
-   * planar.  All NULL = off.  Served by the tcgen05 path only (gf_attn_tc_eligible) for C <= 256, or C = 512 with k <= 16; other
+   * planar.  All NULL = off.  Served by the tensor-core (wgmma) path only (gf_attn_tc_eligible) for C <= 256, or C = 512 with k <= 16; other
    * shapes and the CUDA-core path return UNSUPPORTED. */
   const float* rgb_w;
   const float* rgb_bias;
@@ -98,7 +98,7 @@ typedef struct gf_attn_postop {
    * att_dp and the survivors are scaled by 1 / (1 - att_dp).  The mask is Philox4x32-10 of (token, column block, dp_salt, step) keyed
    * by the seed; dp_state points to DEVICE memory {uint64 seed, uint64 step} read when the kernel runs (bump `step` on the device
    * between training steps: a replayed CUDA graph then draws fresh masks).  Both kernel families serve it with the same mask (the
-   * tcgen05 kernel drops the probabilities before they become GEMM2's operand); the attention map output is the probabilities
+   * wgmma kernel drops the probabilities before they become GEMM2's operand); the attention map output is the probabilities
    * BEFORE dropout.  att_dp = 0 or dp_state = NULL: off. */
   float att_dp;
   uint32_t dp_salt;
@@ -131,7 +131,7 @@ int gf_attn_last_centroid_path(void);
 /* Number of kernels this library has launched in this process (all threads); bench.py reports the delta. */
 long long gf_attn_launch_count(void);
 
-/* 1 when gf_attn_simplex_fwd / stage T of this layer runs on the tcgen05 (TF32) kernel, 0 when the CUDA-core kernel serves it
+/* 1 when gf_attn_simplex_fwd / stage T of this layer runs on the wgmma (TF32) kernel, 0 when the CUDA-core kernel serves it
  * (GF_FLAG_FP32_EXACT, instance / batch norm, C not in {64,128,256,512}, ragged n); negative gf_status on a bad descriptor. */
 int gf_attn_tc_eligible(const gf_attn_desc* desc);
 

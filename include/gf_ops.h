@@ -1,7 +1,7 @@
 /*
  * gf_ops.h -- C ABI of the memory-bound companions of the attention hot path (SURVEY.md row f3).
  *
- * B200-native equivalents of the reference's two native CUDA ops -- dnnlib/tflib/ops/fused_bias_act.cu and
+ * sm_90a equivalents of the reference's two native CUDA ops -- dnnlib/tflib/ops/fused_bias_act.cu and
  * dnnlib/tflib/ops/upfirdn_2d.cu (expected upstream locations; NOT in the reference checkout,
  * /root/reference/.SUBMODULES.json:2) -- restricted to the uses the generator makes of them, plus the
  * activation-scaling form of StyleGAN2's weight (de)modulation.  Channels-last fp32, raw device pointers,
@@ -87,7 +87,7 @@ int gf_torgb_scale_nhwc(const float* x, const float* w, const float* styles, int
 int gf_mapping_fwd(const float* z, const float* w, const float* b, const float* w_avg, float psi, float* out,
                    int B, int k, int D, int L, void* stream);
 
-/* Row f1, first kernel: the 3x3 stride-1 convolution of the synthesis layers (zero padding 1) as a tcgen05 implicit GEMM in TF32,
+/* Row f1, first kernel: the 3x3 stride-1 convolution of the synthesis layers (zero padding 1) as a wgmma implicit GEMM in TF32,
  * channels-last: y[b,h,w,o] = sum_{dy,dx,i} x[b,h+dy-1,w+dx-1,i] * wt[dy*3+dx][o][i].  This is the convolution inside the reference's
  * modulated_conv2d_layer in its activation-scaling form (x already carries the style, demodulation is applied by the consumer).
  * wt comes from gf_conv3x3_pack_weights (w [Cout,Cin,3,3] * scale -> [9][Cout][Cin], rounded to TF32).

@@ -1,10 +1,10 @@
-"""GPU parity tests (run on a B200: ``pytest -m gpu``).  Every call goes through the C ABI (libgf_attn.so).
+"""GPU parity tests (run on an H100: ``pytest -m gpu``).  Every call goes through the C ABI (libgf_attn.so).
 
 Oracle = oracle/bipartite.py in float64 (in-repo restatement; reference source unavailable; PARITY UNPINNED).
 
 Tolerances (stated here, per the task contract):
   * fp32-FMA mode (GF_FLAG_FP32_EXACT, CUDA-core kernel):   |y - y64| <= 1e-5 + 1e-4 |y64|      (SURVEY 8c)
-  * TF32 tensor-core mode (tcgen05 kind::tf32, default):    |y - y64| <= 1e-4 + 1.25e-3 max|y64| + 2e-3 |y64|  and  rel-RMS <= 1e-3
+  * TF32 tensor-core mode (wgmma tf32, default):    |y - y64| <= 1e-4 + 1.25e-3 max|y64| + 2e-3 |y64|  and  rel-RMS <= 1e-3
     (frozen in tests/tolerances.json by tools/calibrate_tolerances.py: the SURVEY 8c contract formula plus a scale term --
      measured worst need 6.4e-4 max|y64|, worst rel-RMS 5.5e-4.)
 """
@@ -98,7 +98,9 @@ def test_layer_matches_golden(gf, cuda_dev, idx, exact):
                                     num_heads=c.get("num_heads", 1))
     if exact:
         assert path == "simt_fp32"
-    check_close(out, torch.from_numpy(gold[name + "/out"]), path, name + "/out", tol_scale=1.5 if c.get("kmeans_iters", 1) > 1 else 1.0)
+    sel = torch.from_numpy(mg.out_sample_index(out.numel()))
+    check_close(out.reshape(-1).cpu()[sel], torch.from_numpy(gold[name + "/out"]), path, name + "/out",
+                tol_scale=1.5 if c.get("kmeans_iters", 1) > 1 else 1.0)
     a_atol = 1e-6 if path == "simt_fp32" else 2e-3
     assert (att.cpu().double() - torch.from_numpy(gold[name + "/att"]).double()).abs().max() <= a_atol + (1e-4 if exact else 5e-3)
     if c["duplex"]:
@@ -159,7 +161,7 @@ def test_persistent_schedule_many_tiles(gf, cuda_dev, C, H, W, k, B, integration
     w = ob.init_params(C, D, k, p, integration, False, seed=17, bias_std=0.3)
     ref, ratt, _ = ob.transformer_layer(x, y, w, integration=integration, return_att=True)
     out, att, _, path = run_layer(gf, cuda_dev, x, y, w, integration=integration, norm="layer", duplex=False, use_pos=True, exact=False)
-    assert path == "tcgen05_tf32"
+    assert path == "wgmma_tf32"
     check_close(out, ref.permute(0, 2, 3, 1), path, "many-tiles")
     assert (att.cpu().double() - ratt).abs().max() <= 5e-3
 
@@ -177,7 +179,7 @@ def test_duplex_layer_vs_oracle(gf, cuda_dev, shape, exact):
     nrm = None if norm == "none" else norm
     ref, ratt, rcen = ob.transformer_layer(x, y, w, integration=integration, norm=nrm, duplex=True, return_att=True)
     out, att, cen, path = run_layer(gf, cuda_dev, x, y, w, integration=integration, norm=nrm, duplex=True, use_pos=True, exact=exact)
-    cpath = gf._lib.last_centroid_path()                            # pass A: tcgen05 TF32 where eligible, else CUDA cores
+    cpath = gf._lib.last_centroid_path()                            # pass A: wgmma TF32 where eligible, else CUDA cores
     if exact:
         assert cpath == "simt_fp32"
     check_close(cen, rcen, cpath, "duplex/centroids")
@@ -211,12 +213,12 @@ def test_short_tiles_small_grid(gf, cuda_dev, C, H, W, k, B, integration, duplex
     w = ob.init_params(C, D, k, p, integration, duplex, seed=19, bias_std=0.3)
     ref, ratt, rcen = ob.transformer_layer(x, y, w, integration=integration, duplex=duplex, return_att=True)
     out, att, cen, path = run_layer(gf, cuda_dev, x, y, w, integration=integration, norm="layer", duplex=duplex, use_pos=True, exact=False)
-    assert path == "tcgen05_tf32"
+    assert path == "wgmma_tf32"
     check_close(out, ref.permute(0, 2, 3, 1), path, "short-tiles")
     assert (att.cpu().double() - ratt).abs().max() <= 5e-3
     if duplex:
-        assert gf._lib.last_centroid_path() == "tcgen05_tf32"
-        check_close(cen, rcen, "tcgen05_tf32", "short-tiles/centroids")
+        assert gf._lib.last_centroid_path() == "wgmma_tf32"
+        check_close(cen, rcen, gf._lib.last_centroid_path(), "short-tiles/centroids")
 
 
 def test_prepare_then_token_stage_equals_one_call(gf, cuda_dev):
@@ -360,7 +362,7 @@ def test_generator_end_to_end(gf, cuda_dev, duplex, exact):
                                               mapping_layers=4, return_att=True, return_features=True)
     assert img.shape == (4, 3, 64, 64) and len(atts) == 8
     check_image(img, ref, "fp32" if exact else "tf32", f"e2e-64/duplex={duplex}")
-    e2e = TOLERANCES["e2e"]["simt_fp32" if exact else "tcgen05_tf32"]
+    e2e = TOLERANCES["e2e"]["simt_fp32" if exact else "wgmma_tf32"]
     for a, r in zip(atts, ratts):
         assert (a.double().cpu() - r).abs().max() <= e2e["att_abs"]
 
@@ -368,7 +370,7 @@ def test_generator_end_to_end(gf, cuda_dev, duplex, exact):
 def check_image(img, ref64, mode, what, scale=1.0):
     """End-to-end image bound of SURVEY 8c, for an image whose range is set by random weights instead of [-1, 1]: the
     bounds are relative to the reference's peak |value|.  max-abs <= max_abs_rel_peak * peak, PSNR >= psnr_db, rel-RMS."""
-    e2e = TOLERANCES["e2e"]["simt_fp32" if mode == "fp32" else "tcgen05_tf32"]
+    e2e = TOLERANCES["e2e"]["simt_fp32" if mode == "fp32" else "wgmma_tf32"]
     got, ref64 = img.detach().double().cpu(), ref64.detach().double().cpu()
     assert got.shape == ref64.shape and torch.isfinite(got).all()
     err = (got - ref64).abs()
@@ -411,15 +413,15 @@ def test_benchmarked_generators_vs_oracle(gf, cuda_dev, cfg):
     z = torch.randn(cfg["B"], cfg["k"] + 1, 32, generator=torch.Generator().manual_seed(1))
     with torch.no_grad():
         img = G(z.to(cuda_dev)).clone()                                        # the benchmarked path (all fusions on)
-        assert gf._lib.last_path() == "tcgen05_tf32"
+        assert gf._lib.last_path() == "wgmma_tf32"
         if cfg["duplex"]:
-            assert gf._lib.last_centroid_path() == "tcgen05_tf32"
+            assert gf._lib.last_centroid_path() == "wgmma_tf32"
         img2, atts, feats = G(z.to(cuda_dev), return_att=True, return_features=True)
     ref, ratts, rfeats = og.generator_forward(G.state_dict(), z, resolution=cfg["res"], components_num=cfg["k"], latent_dim=32,
                                               duplex=cfg["duplex"], return_att=True, return_features=True)
     check_image(img, ref, "tf32", cfg["id"] + "/image")
     check_image(img2, ref, "tf32", cfg["id"] + "/image-features-path")
-    e2e = TOLERANCES["e2e"]["tcgen05_tf32"]
+    e2e = TOLERANCES["e2e"]["wgmma_tf32"]
     assert len(feats) == len(rfeats) == cfg["layers"] and len(atts) == cfg["layers"]
     for li, (f, r) in enumerate(zip(feats, rfeats)):
         f = f.double().cpu()
@@ -721,7 +723,7 @@ def test_generator_512_config5_shape_class(gf, cuda_dev):
         img = G(z).clone()
         rep = G.graphed(2)(z).clone()
     assert img.shape == (2, 3, 512, 512) and torch.isfinite(img).all()
-    assert gf._lib.last_path() == "tcgen05_tf32"
+    assert gf._lib.last_path() == "wgmma_tf32"
     assert (img - rep).abs().max() <= 2e-3 * max(1.0, img.abs().max().item())
     layer = G.synthesis.layers[-1].attention                              # C = 64, 512x512 grid, k = 32
     g = torch.Generator().manual_seed(3)
@@ -856,9 +858,9 @@ def test_fused_torgb_epilogue(gf, cuda_dev, C, H, W, k, duplex, integration):
                 in_scale=f(d_in), post_scale=f(ps), rgb_w=f(rgb_w).contiguous(), rgb_bias=f(rgb_b), rgb_out=rgb_out)
     with torch.no_grad():
         out, _, _ = attn(x64.permute(0, 2, 3, 1).contiguous().float().to(cuda_dev), f(y64), postop=post, need_centroids=False)
-    assert gf._lib.last_path() == "tcgen05_tf32"
-    check_close(out, ref_out.permute(0, 2, 3, 1), "tcgen05_tf32", "torgb-epilogue/out", tol_scale=2.0)
-    check_close(rgb_out, ref_rgb, "tcgen05_tf32", "torgb-epilogue/rgb", tol_scale=2.0)
+    assert gf._lib.last_path() == "wgmma_tf32"
+    check_close(out, ref_out.permute(0, 2, 3, 1), "wgmma_tf32", "torgb-epilogue/out", tol_scale=2.0)
+    check_close(rgb_out, ref_rgb, "wgmma_tf32", "torgb-epilogue/rgb", tol_scale=2.0)
     # the CUDA-core path refuses the fusion loudly
     attn32 = make_layer(gf, cuda_dev, C, D, k, p, integration, "layer", duplex, True, True, w)
     with torch.no_grad(), pytest.raises(RuntimeError, match="tRGB"):
@@ -1005,7 +1007,7 @@ def test_generator_duplex_extensions_end_to_end(gf, cuda_dev, exact):
     sc = 3.0 if exact else 6.0
     check_image(img, ref, "fp32" if exact else "tf32", "duplex-ext/image", scale=sc)
     check_image(img_fused, ref, "fp32" if exact else "tf32", "duplex-ext/image-fused", scale=sc)
-    e2e = TOLERANCES["e2e"]["simt_fp32" if exact else "tcgen05_tf32"]
+    e2e = TOLERANCES["e2e"]["simt_fp32" if exact else "wgmma_tf32"]
     for a, r in zip(atts, ratts):
         assert (a.double().cpu() - r).abs().max() <= sc * e2e["att_abs"]
     ref_nocarry = og.generator_forward(G.state_dict(), z, resolution=64, components_num=8, latent_dim=32, duplex=True, mapping_layers=4,
@@ -1099,7 +1101,7 @@ def test_attention_dropout_forward_and_backward(gf, cuda_dev, C, H, W, k, integr
 @pytest.mark.parametrize("C,H,W,k,integration,norm", [(128, 16, 16, 16, "mul", "layer"), (256, 16, 24, 20, "mul", "layer"), (128, 8, 16, 8, "both", "layer"),
                                                       (512, 8, 16, 8, "add", "none"), (64, 8, 8, 4, "mul", "layer")])
 def test_attention_dropout_on_the_tensor_path(gf, cuda_dev, C, H, W, k, integration, norm):
-    """att_dp on the tcgen05 kernel (training forward of the default path): against the oracle given the SAME Philox mask, with the
+    """att_dp on the wgmma kernel (training forward of the default path): against the oracle given the SAME Philox mask, with the
     fused post-op around it; and the gradients through that forward (stage-T backward kernel, same mask) against the oracle's."""
     from importlib import import_module
     from oracle import philox as ph
@@ -1125,8 +1127,8 @@ def test_attention_dropout_on_the_tensor_path(gf, cuda_dev, C, H, W, k, integrat
     attn.train()
     with torch.no_grad():
         out, att, _ = attn(xg, yg, return_att=True)
-    assert gf._lib.last_path() == "tcgen05_tf32"
-    check_close(out, ref.detach().permute(0, 2, 3, 1), "tcgen05_tf32", "dropout-tc/forward", tol_scale=2.0)
+    assert gf._lib.last_path() == "wgmma_tf32"
+    check_close(out, ref.detach().permute(0, 2, 3, 1), "wgmma_tf32", "dropout-tc/forward", tol_scale=2.0)
     assert (att.cpu().double() - ratt.detach()).abs().max() <= 2e-3           # pre-dropout probabilities, TF32 logits
     gout = torch.randn(ref.shape, generator=g, dtype=torch.float64)
     ref.backward(gout)
@@ -1148,13 +1150,13 @@ def test_attention_dropout_on_the_tensor_path(gf, cuda_dev, C, H, W, k, integrat
     post.update(attn.dropout_postop(cuda_dev))
     with torch.no_grad():
         outp, _, _ = attn(xg, yg, postop=post, need_centroids=False)
-    assert gf._lib.last_path() == "tcgen05_tf32"
-    check_close(outp, refp.permute(0, 2, 3, 1), "tcgen05_tf32", "dropout-tc/postop", tol_scale=2.0)
+    assert gf._lib.last_path() == "wgmma_tf32"
+    check_close(outp, refp.permute(0, 2, 3, 1), "wgmma_tf32", "dropout-tc/postop", tol_scale=2.0)
 
 
 @pytest.mark.parametrize("B,H,W,Cin,Cout", [(2, 16, 16, 64, 64), (3, 32, 16, 128, 128), (1, 8, 32, 256, 256), (2, 24, 48, 96, 192), (1, 64, 64, 32, 512)])
 def test_conv3x3_implicit_gemm(gf, cuda_dev, B, H, W, Cin, Cout):
-    """Row f1: the tcgen05 implicit-GEMM 3x3 convolution (TF32, zero padding by TMA out-of-bounds fill) against the oracle's
+    """Row f1: the wgmma implicit-GEMM 3x3 convolution (TF32, zero padding by TMA out-of-bounds fill) against the oracle's
     convolution (oracle/generator.py::_modconv without modulation) in float64."""
     from importlib import import_module
     ops = import_module("gansformer-reproducibility-challenge_b200.ops")
@@ -1177,7 +1179,7 @@ def test_conv3x3_implicit_gemm(gf, cuda_dev, B, H, W, Cin, Cout):
 
 def test_generator_with_own_tf32_convolutions(gf, cuda_dev, monkeypatch):
     """The benchmarked path end to end: TF32 convolutions allowed, so the five stride-1 3x3 convolutions of the 256^2 generator run on
-    the library's own tcgen05 implicit-GEMM kernel (row f1) and the rest on cuDNN TF32 -- image vs the fp64 oracle within the
+    the library's own wgmma implicit-GEMM kernel (row f1) and the rest on cuDNN TF32 -- image vs the fp64 oracle within the
     SURVEY 8c end-to-end bound (5e-3 of the peak, 60 dB), and against the same network with cuDNN TF32 convolutions everywhere."""
     G = _benchmark_generator(gf, cuda_dev, 256, 16, False)
     z = torch.randn(2, 17, 32, generator=torch.Generator().manual_seed(1))

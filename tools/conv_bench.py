@@ -1,4 +1,4 @@
-"""Row f1: the tcgen05 implicit-GEMM 3x3 convolution (gf_conv3x3_nhwc_tf32) against cuDNN (TF32 and fp32) on the stride-1 convolution
+"""Row f1: the wgmma implicit-GEMM 3x3 convolution (gf_conv3x3_nhwc_tf32) against cuDNN (TF32 and fp32) on the stride-1 convolution
 shapes of the 256^2 generator (batch 32): correctness vs fp32 cuDNN, time, TFLOP/s."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
