@@ -399,6 +399,18 @@ class BipartiteAttention(nn.Module):
             return {}
         return dict(att_dp=self.att_dp, dp_salt=self.dp_salt, dp_state=dropout_state(device))
 
+    def _check_dropout_supported(self, centroids_init=None) -> None:
+        """Attention dropout in training mode runs on single-head layers: simplex, or duplex with kmeans_iters == 1, norm layer /
+        none and no carried-in centroids (`iterative`).  Anything else raises NotImplementedError."""
+        if not (self.training and self.att_dp > 0.0):
+            return
+        if self.num_heads == 1 and not self.duplex:
+            return
+        if self.num_heads == 1 and self.kmeans_iters == 1 and self.norm in ("layer", None, "none") and centroids_init is None:
+            return
+        raise NotImplementedError("attention dropout is implemented for single-head layers: simplex, or duplex with kmeans_iters == 1, "
+                                  "norm layer / none and no iterative centroid carry")
+
     def forward(self, x: torch.Tensor, y: torch.Tensor, centroids: Optional[torch.Tensor] = None,
                 return_att: bool = False, out: Optional[torch.Tensor] = None, postop: Optional[dict] = None,
                 stage: str = "all", need_centroids: bool = True, centroids_init: Optional[torch.Tensor] = None):
@@ -407,16 +419,14 @@ class BipartiteAttention(nn.Module):
         if torch.is_grad_enabled() and (x.requires_grad or y.requires_grad or any(p.requires_grad for p in self.parameters())):
             if postop is not None:
                 raise RuntimeError("the fused post-op is inference-only; apply noise/bias/activation outside when training")
-            if self.att_dp > 0.0 and self.training and (self.duplex or self.num_heads != 1):
-                raise NotImplementedError("attention dropout is implemented for single-head simplex layers")
+            self._check_dropout_supported(centroids_init)
             if centroids_init is not None:
                 raise RuntimeError("iterative centroid carry (centroids_init) is an inference feature in this build")
             from .autograd import bipartite_attention_autograd
             return bipartite_attention_autograd(self, x, y, centroids, return_att)
         dp = self.dropout_postop(x.device)
         if dp:
-            if self.duplex or self.num_heads != 1:
-                raise NotImplementedError("attention dropout is implemented for single-head simplex layers")
+            self._check_dropout_supported(centroids_init if self.iterative else None)
             postop = {**(postop or {"act": "linear", "gain": 1.0}), **dp}
         return bipartite_attention_forward(x, y, self.param_dict(), self._plan, integration=self.integration,
                                            norm=self.norm, duplex=self.kmeans_iters if self.duplex else 0, num_heads=self.num_heads,

@@ -3,7 +3,10 @@
 Forward = the C-ABI CUDA kernels.  Backward of a simplex layer with layer norm (or none): the hand-written stage-T
 backward kernel ``gf_attn_simplex_bwd`` (activation gradient + the per-token gradients of logits / control signal), two
 batched GEMMs for the reductions over tokens, and torch autograd through the tiny per-image tables of stages W and I
-(``folded_tables``).  Everything else (duplex, instance / batch norm, CPU tensors): PyTorch autograd through a
+(``folded_tables``).  Backward of a duplex layer (one k-means iteration, layer norm / none) whose forward ran with attention
+dropout: the same stage-T kernel with keys from the centroids, plus the pass-A kernels ``gf_attn_centroid_stats`` /
+``gf_attn_centroid_bwd`` and autograd through the pass-A tables (``centroid_tables``), see ``_duplex_kernel_backward``.
+Everything else (duplex without dropout, instance / batch norm, multi-head, CPU tensors): PyTorch autograd through a
 recomputation of the direct-form algebra with torch ops (``composite_forward``).
 """
 from __future__ import annotations
@@ -92,10 +95,39 @@ def composite_forward(x, y, p, *, integration, norm, duplex, use_pos, centroids=
     return out.reshape(B, H, W, C), cen
 
 
-def folded_tables(y, p, *, H, W, C, integration, use_pos):
+def centroid_tables(y, p, H, W, C, use_pos):
+    """Duplex pass A in differentiable torch ops: (latents y [B,k,D], raw parameters) -> the tables of the centroid softmax,
+    M [B,KP,C] (zero rows in the padded latents), Rt2 [B,H,KP] (-inf in the padded latents), Ct2 [B,W,KP], such that the logit
+    of token (h, w) for latent j is x.M_j + Rt2[h,j] + Ct2[w,j].  Same algebra as duplex_tables in csrc/gf_fold.cu, in natural-log
+    units and without TF32 rounding: M_j = Qy_j Wk2_e^T / sqrt(C), the positional terms Qy_j (Pg Wpk2_e)^T / sqrt(C) split into
+    their row and column halves; bk2 is constant over the tokens and cancels in the softmax."""
+    B, k, _ = y.shape
+    KP = 16 if k <= 16 else 32
+    s = 1.0 / math.sqrt(C)
+    qy = y @ _e(p["wq2"]) + p["bq2"]
+    if use_pos:
+        qy = qy + (p["pos_latent"] @ _e(p["wpq2"]))[None]
+    M = torch.nn.functional.pad((qy @ _e(p["wk2"]).t()) * s, (0, 0, 0, KP - k))
+    if use_pos:
+        half = p["pos_latent"].shape[1] // 2
+        row, col = _axis(H, half, y.device).to(y.dtype), _axis(W, half, y.device).to(y.dtype)
+        qp = (qy @ _e(p["wpk2"]).t()) * s                                # [B, k, pd]
+        rt = torch.einsum("hp,bjp->bhj", row, qp[:, :, :half])
+        ct = torch.einsum("wp,bjp->bwj", col, qp[:, :, half:])
+    else:
+        rt = torch.zeros(B, H, k, device=y.device, dtype=y.dtype)
+        ct = torch.zeros(B, W, k, device=y.device, dtype=y.dtype)
+    Rt2 = torch.cat([rt, torch.full((B, H, KP - k), -math.inf, device=y.device, dtype=y.dtype)], dim=2) if KP > k else rt
+    Ct2 = torch.nn.functional.pad(ct, (0, KP - k))
+    return M.contiguous(), Rt2.contiguous(), Ct2.contiguous()
+
+
+def folded_tables(y, p, *, H, W, C, integration, use_pos, centroids=None, img2ltnt=False):
     """Stages W + I in differentiable torch ops: (latents y [B,k,D], raw parameters) -> the per-image tables stage T and its
     backward consume, in the workspace layout: Kp [B,KP,C], Vt [B,Cout,KP], Rt [B,H,KP] (-inf in the padded latents),
-    Ct [B,W,KP].  Same algebra as csrc/gf_fold.cu (simplex)."""
+    Ct [B,W,KP].  Same algebra as csrc/gf_fold.cu.  Simplex: keys from the latents through wk.  Duplex (centroids [B,k,C] given):
+    keys from the centroids through wkc; with img2ltnt the values come from the latents modulated by the centroids,
+    LN(y) (1 + centroids Wi2l_e + bi2l)."""
     B, k, _ = y.shape
     KP = 16 if k <= 16 else 32
     s = 1.0 / math.sqrt(C)
@@ -108,7 +140,8 @@ def folded_tables(y, p, *, H, W, C, integration, use_pos):
     kconst = p["bk"][None, :].expand(k, C)
     if use_pos:
         kconst = kconst + p["pos_latent"] @ _e(p["wpk"])
-    kp_all = y @ (_e(p["wk"]) @ qfold) + (kconst @ qfold)[None]          # [B, k, C + pd + 1]
+    ksrc, wk = (y, p["wk"]) if centroids is None else (centroids, p["wkc"])
+    kp_all = ksrc @ (_e(wk) @ qfold) + (kconst @ qfold)[None]            # [B, k, C + pd + 1]
     Kp = torch.nn.functional.pad(kp_all[:, :, :C], (0, 0, 0, KP - k))
     kap0 = kp_all[:, :, C + pd]
     if use_pos:
@@ -125,7 +158,11 @@ def folded_tables(y, p, *, H, W, C, integration, use_pos):
     cv = p["bv"] @ wo + p["bo"]
     if integration in ("mul", "both"):
         cv = cv + torch.cat([torch.ones(C, device=y.device, dtype=y.dtype), torch.zeros(cv.numel() - C, device=y.device, dtype=y.dtype)])
-    v = y @ (_e(p["wv"]) @ wo) + cv                                      # [B, k, Cout]
+    yv = y
+    if centroids is not None and img2ltnt:
+        ym = y.mean(dim=2, keepdim=True)
+        yv = (y - ym) * torch.rsqrt(((y - ym) ** 2).mean(dim=2, keepdim=True) + 1e-8) * (1.0 + centroids @ _e(p["wi2l"]) + p["bi2l"])
+    v = yv @ (_e(p["wv"]) @ wo) + cv                                     # [B, k, Cout]
     Vt = torch.nn.functional.pad(v.transpose(1, 2), (0, KP - k))
     cb = cv - p["bv"] @ wo                       # bo (+1 on the gain half): the constants attention dropout leaves unscaled
     return Kp.contiguous(), Vt.contiguous(), Rt.contiguous(), Ct.contiguous(), cb.contiguous()
@@ -133,6 +170,11 @@ def folded_tables(y, p, *, H, W, C, integration, use_pos):
 
 def _kernel_backward_ok(m, x) -> bool:
     return (not m.duplex) and m.norm in ("layer", None, "none") and m.num_heads == 1 and x.is_cuda and x.dtype == torch.float32
+
+
+def _duplex_kernel_backward_ok(m, x) -> bool:
+    return m.duplex and m.kmeans_iters == 1 and m.norm in ("layer", None, "none") and m.num_heads == 1 and x.is_cuda \
+        and x.dtype == torch.float32
 
 
 class _FusedAttention(torch.autograd.Function):
@@ -158,8 +200,11 @@ class _FusedAttention(torch.autograd.Function):
         x, y, *params = ctx.saved_tensors
         if _kernel_backward_ok(m, x):
             return (None, None, None, None, *_kernel_backward(m, ctx.names, x, y, params, g_out, ctx.dropout))
+        if ctx.dropout and _duplex_kernel_backward_ok(m, x):
+            return (None, None, None, None, *_duplex_kernel_backward(m, ctx.names, x, y, params, g_out, ctx.dropout, ctx.centroids))
         if ctx.dropout:
-            raise NotImplementedError("attention dropout needs the stage-T backward kernel (single-head simplex, layer norm / none)")
+            raise NotImplementedError("attention dropout needs the backward kernels: single-head layers with norm layer / none, "
+                                      "simplex or duplex with kmeans_iters == 1")
         with torch.enable_grad():
             xs = x.detach().requires_grad_(True)
             ys = y.detach().requires_grad_(True)
@@ -173,21 +218,112 @@ class _FusedAttention(torch.autograd.Function):
 
 def _kernel_backward(m, names, x, y, params, g_out, dropout=None):
     """d(loss)/d(x, y, params) of a simplex layer through gf_attn_simplex_bwd (see the module docstring)."""
-    import ctypes
-    from . import _lib
     B, H, W, C = x.shape
-    n, k = H * W, y.shape[1]
     with torch.enable_grad():
         ys = y.detach().requires_grad_(True)
         ps = [p.detach().requires_grad_(True) for p in params]
-        Kp, Vt, Rt, Ct, cb = folded_tables(ys, dict(zip(names, ps)), H=H, W=W, C=C, integration=m.integration, use_pos=m.use_pos)
+        tables = folded_tables(ys, dict(zip(names, ps)), H=H, W=W, C=C, integration=m.integration, use_pos=m.use_pos)
+    dX, outs, grads = _stage_t_backward(m, x, y.shape[1], y.shape[2], g_out, tables, dropout)
+    gy, *gp = torch.autograd.grad(outs, [ys, *ps], grads, allow_unused=True)
+    return (dX, gy, *gp)
+
+
+def _duplex_kernel_backward(m, names, x, y, params, g_out, dropout=None, centroids=None):
+    """d(loss)/d(x, y, params) of a duplex layer (one k-means iteration, norm layer / none):
+      1. gf_attn_centroid_stats recomputes pass A in fp32 from the tables of ``centroid_tables``: Xbar [B,k,C], lse [B,KP];
+      2. Cen = Xbar Wv2_e + bv2 in torch (Xbar a leaf) and the stage-T tables from it (``folded_tables`` with centroids);
+      3. stage T's backward (gf_attn_simplex_bwd_ex with a simplex descriptor of the same shape, same dropout), its token
+         reductions and autograd over the tables: dX, and the gradients of y, the parameters and Xbar;
+      4. r = dXbar . Xbar, then gf_attn_centroid_bwd adds the pass-A part into dX and gives dS of the pass-A logits;
+      5. dM = dS^T X, dRt2 / dCt2 = sums of dS, and autograd over the pass-A tables.
+    With ``centroids`` given, pass A did not run in the forward: steps 1, 4 and 5 are skipped and the centroids get no gradient."""
+    B, H, W, C = x.shape
+    k, D = y.shape[1], y.shape[2]
+    xc = x.detach().contiguous()
+    with torch.enable_grad():
+        ys = y.detach().requires_grad_(True)
+        ps = [p.detach().requires_grad_(True) for p in params]
+        pdict = dict(zip(names, ps))
+        if centroids is None:
+            cen_tabs = centroid_tables(ys, pdict, H, W, C, m.use_pos)
+            xbar, lse = _centroid_stats(m, xc, k, D, *(t.detach() for t in cen_tabs))
+            xbar.requires_grad_(True)
+            cen = xbar @ _e(pdict["wv2"]) + pdict["bv2"]
+        else:
+            cen = centroids.detach()
+        tables = folded_tables(ys, pdict, H=H, W=W, C=C, integration=m.integration, use_pos=m.use_pos, centroids=cen, img2ltnt=m.img2ltnt)
+    dX, outs, grads = _stage_t_backward(m, x, k, D, g_out, tables, dropout)
+    leaves = [ys, *ps] + ([xbar] if centroids is None else [])
+    g1 = list(torch.autograd.grad(outs, leaves, grads, allow_unused=True))
+    if centroids is None:
+        dxbar = g1.pop().contiguous()
+        r = (dxbar * xbar.detach()).sum(dim=2).contiguous()                # [B, k]
+        dS = _centroid_bwd(m, xc, k, D, *(t.detach() for t in cen_tabs), lse, dxbar, r, dX)
+        KP = dS.shape[2]
+        dM = torch.bmm(dS.transpose(1, 2), xc.reshape(B, H * W, C))     # [B, KP, C]
+        dS4 = dS.reshape(B, H, W, KP)
+        Mt, Rt2, Ct2 = cen_tabs
+        g2 = torch.autograd.grad([Mt, Rt2, Ct2], [ys, *ps], [dM, dS4.sum(dim=2), dS4.sum(dim=1)], allow_unused=True)
+        g1 = [a if b is None else (b if a is None else a + b) for a, b in zip(g1, g2)]
+        i = 1 + names.index("bk2")     # constant over the tokens, bk2 cancels in pass A's softmax: its gradient is exactly 0
+        g1[i] = torch.zeros_like(params[i - 1])
+    return (dX, *g1)
+
+
+def _duplex_desc(m, x, k, D):
+    from . import _lib
+    B, H, W, C = x.shape
+    return _lib.make_desc(B, H, W, C, k, D, heads=1, norm=m.norm, integration=m.integration,
+                          pos_dim=m.pos_dim if m.use_pos else 0, duplex=1, flags=0)
+
+
+def _centroid_stats(m, xc, k, D, Mt, Rt2, Ct2):
+    """gf_attn_centroid_stats: pass A recomputed in fp32 -> (Xbar [B,k,C], lse [B,KP])."""
+    import ctypes
+    from . import _lib
+    B, _, _, C = xc.shape
+    desc = _duplex_desc(m, xc, k, D)
+    xbar = torch.empty((B, k, C), dtype=torch.float32, device=xc.device)
+    lse = torch.empty((B, Mt.shape[1]), dtype=torch.float32, device=xc.device)
+    part = torch.empty(_lib.workspace_bytes(desc), dtype=torch.uint8, device=xc.device)       # split-n partials
+    with torch.cuda.device(xc.device):
+        _lib.check(_lib.load().gf_attn_centroid_stats(ctypes.byref(desc), xc.data_ptr(), Mt.data_ptr(), Rt2.data_ptr(), Ct2.data_ptr(),
+                                                      xbar.data_ptr(), lse.data_ptr(), part.data_ptr(),
+                                                      ctypes.c_void_p(torch.cuda.current_stream(xc.device).cuda_stream)),
+                   "gf_attn_centroid_stats")
+    return xbar, lse
+
+
+def _centroid_bwd(m, xc, k, D, Mt, Rt2, Ct2, lse, dxbar, r, dX):
+    """gf_attn_centroid_bwd: adds the pass-A part of the activation gradient into dX; returns dS [B,n,KP] of the pass-A logits."""
+    import ctypes
+    from . import _lib
+    B, H, W, C = xc.shape
+    desc = _duplex_desc(m, xc, k, D)
+    dS = torch.empty((B, H * W, Mt.shape[1]), dtype=torch.float32, device=xc.device)
+    with torch.cuda.device(xc.device):
+        _lib.check(_lib.load().gf_attn_centroid_bwd(ctypes.byref(desc), xc.data_ptr(), Mt.data_ptr(), Rt2.data_ptr(), Ct2.data_ptr(),
+                                                    lse.data_ptr(), dxbar.data_ptr(), r.data_ptr(), dX.data_ptr(), dS.data_ptr(),
+                                                    ctypes.c_void_p(torch.cuda.current_stream(xc.device).cuda_stream)),
+                   "gf_attn_centroid_bwd")
+    return dS
+
+
+def _stage_t_backward(m, x, k, D, g_out, tables, dropout):
+    """gf_attn_simplex_bwd_ex and the reductions over the tokens: returns dX and the (tables, gradients) pairs autograd takes
+    back through stages W and I."""
+    import ctypes
+    from . import _lib
+    B, H, W, C = x.shape
+    n = H * W
+    Kp, Vt, Rt, Ct, cb = tables
     KP, Cout = Kp.shape[1], Vt.shape[1]
     xc, gc = x.detach().contiguous(), g_out.detach().contiguous()
     dX = torch.empty_like(xc)
     dS = torch.empty((B, n, KP), dtype=torch.float32, device=x.device)
     P = torch.empty_like(dS)
     dCtl = torch.empty((B, n, Cout), dtype=torch.float32, device=x.device)
-    desc = _lib.make_desc(B, H, W, C, k, y.shape[2], heads=1, norm=m.norm, integration=m.integration,
+    desc = _lib.make_desc(B, H, W, C, k, D, heads=1, norm=m.norm, integration=m.integration,
                           pos_dim=m.pos_dim if m.use_pos else 0, duplex=False, flags=0)
     with torch.cuda.device(x.device):
         dpo = dropout or {}
@@ -206,8 +342,7 @@ def _kernel_backward(m, names, x, y, params, g_out, dropout=None):
     if dpo:                                      # ctl = sum_j q_j (Vt_j - cb) + cb: the constants' own gradient
         outs.append(cb)
         grads.append((dCtl * (1.0 - P.sum(dim=2, keepdim=True))).sum(dim=(0, 1)))
-    gy, *gp = torch.autograd.grad(outs, [ys, *ps], grads, allow_unused=True)
-    return (dX, gy, *gp)
+    return dX, outs, grads
 
 
 def bipartite_attention_autograd(module, x, y, centroids, return_att):

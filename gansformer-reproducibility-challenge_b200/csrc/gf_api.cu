@@ -273,6 +273,10 @@ int gf_attn_duplex_fwd_ex(const gf_attn_desc* desc, const float* X, const float*
                      post ? post->in_scale_ld : 0, !keys_from_cen,
                      cen_in || L.img2ltnt || ((desc->flags & GF_FLAG_CENTROIDS_INIT) && !(desc->flags & GF_FLAG_TABLES_READY)))))
     return rc;
+  // attention dropout: the token kernels re-add the constants of the control signal as (1 - sum q) * CB, read from ws (the simplex
+  // prologue writes it there; the duplex key path does not)
+  if (post && post->att_dp != 0.f && post->dp_state)
+    GF_CUDA_OK(cudaMemcpyAsync(ws + L.w_CB, folded + L.f_CB, sizeof(float) * L.Cout, cudaMemcpyDeviceToDevice, st));
   return token_pass(L, desc, X, Xout, att, ws, post, st);
 }
 

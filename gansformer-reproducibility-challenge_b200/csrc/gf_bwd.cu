@@ -12,6 +12,10 @@
 //     dK'[b] = dS[b]^T X[b],   dV^T[b] = dCtl[b]^T P[b],   dRt = sum_w dS,   dCt = sum_h dS,
 // and the chain rule through stages I and W is torch autograd over tiny [B,k,*] tensors.
 // Replaces ~45 full passes over [B,n,C]-sized tensors of the direct-form autograd composite by 8.
+//
+// Also here: the backward of duplex pass A (centroid_bwd_kernel, gf_attn_centroid_stats / gf_attn_centroid_bwd).  Stage T of a
+// duplex layer is the computation above with keys from the centroids, so a duplex layer's backward is token_bwd_kernel, then
+// centroid_bwd_kernel adding the pass-A part of dX.
 #include <string.h>
 #include "gf_common.cuh"
 
@@ -252,6 +256,131 @@ __global__ void __launch_bounds__(BTM) token_bwd_kernel(const BwdParams P) {
   }
 }
 
+// ---- backward of duplex pass A (the centroid pass: the latents attend to the grid, softmax over the n tokens) ------------------
+// Forward (oracle/folded.py centroid_pass):  s[t,j] = x_t.M_j + Rt2[h,j] + Ct2[w,j];  A[t,j] = exp(s[t,j] - lse_j);
+//     Xbar_j = sum_t A[t,j] x_t.
+// Given dXbar and r_j = dXbar_j.Xbar_j, two sweeps over the 32-channel chunks of a 128-token tile (thread = token, fp32 FMA):
+//     sweep 1:  s_j, g_j = x_t.dXbar_j;   then a_j = A[t,j], ds_j = a_j (g_j - r_j)       -> dS [B,n,KP]
+//     sweep 2:  dX_t += sum_j a_j dXbar_j + sum_j ds_j M_j                                (in place, on top of stage T's dX)
+// The reductions over tokens are the caller's: dM = dS^T X, dRt2 = sum_w dS, dCt2 = sum_h dS.  Reads X once and dX once, writes dX
+// and dS: with stage T's backward and the recompute of the statistics, about 16 [B,n,C]-sized passes for a duplex layer.
+struct CenBwdParams {
+  const float* X; const float* M; const float* Rt; const float* Ct; const float* lse; const float* dXbar; const float* r;
+  float* dX; float* dS;
+  int n, H, W, C, k;
+};
+
+template <int KP>
+__global__ void __launch_bounds__(BTM) centroid_bwd_kernel(const CenBwdParams P) {
+  __shared__ __align__(16) float xs[BTM][BXS];       // x chunk (sweep 1), dX chunk (sweep 2)
+  __shared__ __align__(16) float ms[KP * BCH];       // M chunk: [KP][32] in sweep 1, [32][KP] in sweep 2
+  __shared__ __align__(16) float gs[KP * BCH];       // dXbar chunk, same two layouts; zero rows for the padded latents
+
+  const int b = blockIdx.y, t0 = blockIdx.x * BTM, tid = threadIdx.x, t = t0 + tid;
+  const int n = P.n, C = P.C, k = P.k;
+  const bool valid = t < n;
+  const float* Xb = P.X + (size_t)b * n * C;
+  const float* Mb = P.M + (size_t)b * KP * C;
+  const float* Gb = P.dXbar + (size_t)b * k * C;
+  float* dXb = P.dX + (size_t)b * n * C;
+
+  float s[KP], g[KP];
+  {
+    const int h = valid ? t / P.W : 0, w = valid ? t % P.W : 0;
+    const float* rt = P.Rt + ((size_t)b * P.H + h) * KP;
+    const float* ct = P.Ct + ((size_t)b * P.W + w) * KP;
+#pragma unroll
+    for (int j = 0; j < KP; ++j) { s[j] = rt[j] + ct[j]; g[j] = 0.f; }
+  }
+  // ---- sweep 1: logits of pass A and g = x.dXbar
+  {
+    float (*mk)[BCH] = reinterpret_cast<float (*)[BCH]>(ms);
+    float (*gk)[BCH] = reinterpret_cast<float (*)[BCH]>(gs);
+    for (int c0 = 0; c0 < C; c0 += BCH) {
+      __syncthreads();
+      bwd_load_chunk(xs, Xb, t0, n, C, c0);
+      for (int i = tid; i < KP * BCH / 4; i += BTM) {
+        const int j = i / (BCH / 4), c4 = (i % (BCH / 4)) * 4;
+        *reinterpret_cast<float4*>(&mk[j][c4]) = __ldg(reinterpret_cast<const float4*>(Mb + (size_t)j * C + c0 + c4));
+        *reinterpret_cast<float4*>(&gk[j][c4]) = j < k ? __ldg(reinterpret_cast<const float4*>(Gb + (size_t)j * C + c0 + c4))
+                                                       : make_float4(0.f, 0.f, 0.f, 0.f);
+      }
+      __syncthreads();
+#pragma unroll
+      for (int c4 = 0; c4 < BCH; c4 += 4) {
+        const float4 x = *reinterpret_cast<const float4*>(&xs[tid][c4]);
+#pragma unroll
+        for (int j = 0; j < KP; ++j) {
+          const float4 mv = *reinterpret_cast<const float4*>(&mk[j][c4]);
+          const float4 gv = *reinterpret_cast<const float4*>(&gk[j][c4]);
+          s[j] = fmaf(x.x, mv.x, fmaf(x.y, mv.y, fmaf(x.z, mv.z, fmaf(x.w, mv.w, s[j]))));
+          g[j] = fmaf(x.x, gv.x, fmaf(x.y, gv.y, fmaf(x.z, gv.z, fmaf(x.w, gv.w, g[j]))));
+        }
+      }
+    }
+  }
+  // ---- probabilities of pass A (softmax over the tokens, from the merged log-denominators) and the gradient of their logits
+#pragma unroll
+  for (int j = 0; j < KP; ++j) {
+    const float l = __ldg(P.lse + (size_t)b * KP + j);
+    const float a = (l == -INFINITY) ? 0.f : expf(s[j] - l);     // padded latents (Rt2 = lse = -inf) stay inert
+    const float rj = j < k ? __ldg(P.r + (size_t)b * k + j) : 0.f;
+    s[j] = a;                                                    // s = a from here on
+    g[j] = a * (g[j] - rj);                                      // g = ds from here on
+  }
+  if (valid) {
+    float4* ds4 = reinterpret_cast<float4*>(P.dS + ((size_t)b * n + t) * KP);
+#pragma unroll
+    for (int j4 = 0; j4 < KP / 4; ++j4) ds4[j4] = make_float4(g[j4 * 4], g[j4 * 4 + 1], g[j4 * 4 + 2], g[j4 * 4 + 3]);
+  }
+  // ---- sweep 2: dX += a.dXbar + ds.M
+  float (*mt)[KP] = reinterpret_cast<float (*)[KP]>(ms);
+  float (*gt)[KP] = reinterpret_cast<float (*)[KP]>(gs);
+  for (int c0 = 0; c0 < C; c0 += BCH) {
+    __syncthreads();
+#pragma unroll
+    for (int it = 0; it < BTM / 16; ++it) {            // plain loads: this kernel writes dX
+      const int row = it * 16 + (tid >> 3), c4 = (tid & 7) * 4;
+      float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+      if (t0 + row < n) v = *reinterpret_cast<const float4*>(dXb + (size_t)(t0 + row) * C + c0 + c4);
+      *reinterpret_cast<float4*>(&xs[row][c4]) = v;
+    }
+    for (int i = tid; i < KP * BCH / 4; i += BTM) {    // transposed: [channel][latent]
+      const int j = i / (BCH / 4), c4 = (i % (BCH / 4)) * 4;
+      const float4 mv = __ldg(reinterpret_cast<const float4*>(Mb + (size_t)j * C + c0 + c4));
+      const float4 gv = j < k ? __ldg(reinterpret_cast<const float4*>(Gb + (size_t)j * C + c0 + c4)) : make_float4(0.f, 0.f, 0.f, 0.f);
+      mt[c4][j] = mv.x; mt[c4 + 1][j] = mv.y; mt[c4 + 2][j] = mv.z; mt[c4 + 3][j] = mv.w;
+      gt[c4][j] = gv.x; gt[c4 + 1][j] = gv.y; gt[c4 + 2][j] = gv.z; gt[c4 + 3][j] = gv.w;
+    }
+    __syncthreads();
+#pragma unroll 2
+    for (int cc = 0; cc < BCH; ++cc) {
+      float dx = xs[tid][cc];
+#pragma unroll
+      for (int j4 = 0; j4 < KP; j4 += 4) {
+        const float4 mv = *reinterpret_cast<const float4*>(&mt[cc][j4]);
+        const float4 gv = *reinterpret_cast<const float4*>(&gt[cc][j4]);
+        dx = fmaf(s[j4], gv.x, fmaf(g[j4], mv.x, dx));
+        dx = fmaf(s[j4 + 1], gv.y, fmaf(g[j4 + 1], mv.y, dx));
+        dx = fmaf(s[j4 + 2], gv.z, fmaf(g[j4 + 2], mv.z, dx));
+        dx = fmaf(s[j4 + 3], gv.w, fmaf(g[j4 + 3], mv.w, dx));
+      }
+      xs[tid][cc] = dx;                                // own row only
+    }
+    __syncthreads();
+    bwd_store_chunk(dXb, xs, t0, n, C, c0);
+  }
+}
+
+// The configurations the pass-A backward serves: a duplex layer with one k-means iteration, norm layer / none, B <= 65535 (grid.y).
+static int centroid_bwd_config(const char* who, const gf_attn_desc* desc, const Layout& L) {
+  if (!L.duplex) { set_error("%s: desc.duplex is 0 (pass A belongs to duplex layers)", who); return GF_ERR_INVALID; }
+  if (desc->duplex != 1) { set_error("%s: one k-means iteration (desc.duplex = 1) is supported, got %d", who, desc->duplex); return GF_ERR_UNSUPPORTED; }
+  if (desc->norm != GF_NORM_LAYER && desc->norm != GF_NORM_NONE) { set_error("%s: norm must be layer or none", who); return GF_ERR_UNSUPPORTED; }
+  if (L.B > 65535) { set_error("%s: B > 65535", who); return GF_ERR_UNSUPPORTED; }
+  return GF_OK;
+}
+
 }  // namespace gf
 
 using namespace gf;
@@ -294,6 +423,39 @@ extern "C" int gf_attn_simplex_bwd_ex(const gf_attn_desc* desc, const float* X, 
     GF_CUDA_OK(cudaFuncSetAttribute(token_bwd_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     token_bwd_kernel<32><<<grid, BTM, smem, st>>>(P);
   }
+  GF_LAUNCH_OK();
+  return GF_OK;
+}
+
+extern "C" int gf_attn_centroid_stats(const gf_attn_desc* desc, const float* X, const float* M, const float* Rt2, const float* Ct2,
+                                      float* Xbar, float* lse, void* ws, void* stream) {
+  Layout L;
+  int rc = make_layout(desc, &L);
+  if (rc) return rc;
+  if (!X || !M || !Rt2 || !Ct2 || !Xbar || !lse || !ws) { set_error("gf_attn_centroid_stats: null pointer"); return GF_ERR_INVALID; }
+  if ((rc = centroid_bwd_config("gf_attn_centroid_stats", desc, L))) return rc;
+  if ((rc = check_device())) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
+  float* part = (float*)ws;                            // split-n partials [B][nsplit][KP][C + 4]
+  if ((rc = centroid_partials_simt(L, X, M, Rt2, Ct2, part, st))) return rc;
+  return centroid_merge_into(L, part, Xbar, lse, st);
+}
+
+extern "C" int gf_attn_centroid_bwd(const gf_attn_desc* desc, const float* X, const float* M, const float* Rt2, const float* Ct2,
+                                    const float* lse, const float* dXbar, const float* r, float* dX, float* dS, void* stream) {
+  Layout L;
+  int rc = make_layout(desc, &L);
+  if (rc) return rc;
+  if (!X || !M || !Rt2 || !Ct2 || !lse || !dXbar || !r || !dX || !dS) { set_error("gf_attn_centroid_bwd: null pointer"); return GF_ERR_INVALID; }
+  if ((rc = centroid_bwd_config("gf_attn_centroid_bwd", desc, L))) return rc;
+  if ((rc = check_device())) return rc;
+  CenBwdParams P;
+  P.X = X; P.M = M; P.Rt = Rt2; P.Ct = Ct2; P.lse = lse; P.dXbar = dXbar; P.r = r; P.dX = dX; P.dS = dS;
+  P.n = L.n; P.H = L.H; P.W = L.W; P.C = L.C; P.k = L.k;
+  dim3 grid((L.n + BTM - 1) / BTM, L.B);
+  cudaStream_t st = (cudaStream_t)stream;
+  if (L.KP == 16) centroid_bwd_kernel<16><<<grid, BTM, 0, st>>>(P);
+  else centroid_bwd_kernel<32><<<grid, BTM, 0, st>>>(P);
   GF_LAUNCH_OK();
   return GF_OK;
 }

@@ -136,8 +136,13 @@ int dropout_args(const gf_attn_postop* post, DropoutArgs* out);
 int norm_stats(const Layout& L, const gf_attn_desc* d, const float* X, float* ws, cudaStream_t st);
 int centroid_pass_simt(const Layout& L, const gf_attn_desc* d, const float* X, float* ws, cudaStream_t st,
                        const float* in_scale = nullptr, int in_scale_ld = 0);
+// the CUDA-core pass-A kernel on explicit tables (M [B,KP,C], Rt2 [B,H,KP], Ct2 [B,W,KP], natural-log units): split-n partials into part
+int centroid_partials_simt(const Layout& L, const float* X, const float* M, const float* Rt2, const float* Ct2, float* part, cudaStream_t st);
 // Xbar = merge of the split partials (times the load-side scale, when given)
 int centroid_merge(const Layout& L, float* ws, cudaStream_t st, const float* in_scale = nullptr, int in_scale_ld = 0);
+// the same merge from / to explicit buffers; lse [B,KP] (nullable) receives the log of each latent's softmax denominator
+int centroid_merge_into(const Layout& L, const float* part, float* xbar, float* lse, cudaStream_t st, const float* in_scale = nullptr,
+                        int in_scale_ld = 0);
 // wgmma duplex pass A (gf_tc_cen.cu): partials into ws (same format as the CUDA-core kernel), merged by centroid_merge
 bool tc_centroid_supported(const Layout& L, const gf_attn_desc* d);
 int centroid_pass_tc(const Layout& L, const float* X, float* ws, cudaStream_t st);

@@ -7,8 +7,9 @@ beta2 = 0.99), an exponential moving average of the generator weights, data para
 gradient all-reduce.  Here: one process per GPU, gradients averaged through ONE flat fp32 buffer per network
 (``dist.allreduce_gradients``: NCCL over NVLink/NVSwitch, gloo in the CPU tests) -- the only collective of the system.
 
-The attention layers run their CUDA forward; their backward is the composite of ``autograd.py`` (a hand-written
-backward kernel is the follow-up).  The discriminator is plain PyTorch plumbing (cuDNN convolutions): it is not on
+The attention layers run their CUDA forward.  Their backward (``autograd.py``) is the hand-written stage-T backward kernel for
+simplex layers, the same kernel plus the pass-A backward kernels for duplex layers with attention dropout, and the torch
+composite for the rest (duplex layers without dropout, instance / batch norm, multi-head).  The discriminator is plain PyTorch plumbing (cuDNN convolutions): it is not on
 the hot path.  Path-length regularisation and augmentation are out of scope.
 """
 from __future__ import annotations

@@ -204,6 +204,25 @@ int gf_attn_simplex_bwd_ex(const gf_attn_desc* desc, const float* X, const float
                            const float* Rt, const float* Ct, float* dX, float* dS, float* P, float* dCtl,
                            float att_dp, uint32_t dp_salt, const unsigned long long* dp_state, const float* cb, void* stream);
 
+/* Backward of duplex pass A (the centroid pass, softmax over the n tokens) for desc.duplex = 1 (one k-means iteration), norm
+ * layer / none.  The pass-A tables come from the caller in natural-log units, fp32, un-rounded (not the workspace copies of a
+ * forward call): M [B,KP,C] (zero rows in the padded latents), Rt2 [B,H,KP] (-inf in the padded latents), Ct2 [B,W,KP], with
+ *   s[t,j] = x_t.M_j + Rt2[h,j] + Ct2[w,j],  A[t,j] = softmax over t of s[t,j],  Xbar_j = sum_t A[t,j] x_t.
+ * Neither entry reads a layer's workspace, so the layer may run forward again between its forward and its backward.
+ *
+ * gf_attn_centroid_stats: recomputes pass A in fp32 and writes Xbar [B,k,C] and lse [B,KP] = log sum_t exp s[t,j] (-inf in the
+ * padded latents).  ws: caller-allocated scratch for the split-n partials; gf_attn_workspace_bytes(desc) bytes are enough. */
+int gf_attn_centroid_stats(const gf_attn_desc* desc, const float* X, const float* M, const float* Rt2, const float* Ct2,
+                           float* Xbar, float* lse, void* ws, void* stream);
+
+/* gf_attn_centroid_bwd: given dXbar [B,k,C] and r [B,k] = sum_c dXbar * Xbar, the per-token part of the pass-A backward:
+ *   dS [B,n,KP] = A (x_t.dXbar_j - r_j)             (gradient w.r.t. the pass-A logits; 0 in the padded latents)
+ *   dX [B,n,C] += sum_j A[t,j] dXbar_j + sum_j dS[t,j] M_j   (accumulated in place: pass stage T's activation gradient in)
+ * The caller reduces dM[b] = dS[b]^T X[b], dRt2[b,h,:] = sum_w dS[b,h,w,:], dCt2[b,w,:] = sum_h dS[b,h,w,:].  Deterministic: no
+ * atomics. */
+int gf_attn_centroid_bwd(const gf_attn_desc* desc, const float* X, const float* M, const float* Rt2, const float* Ct2,
+                         const float* lse, const float* dXbar, const float* r, float* dX, float* dS, void* stream);
+
 /* The dropout multipliers themselves, mask [B, H*W, KP] (0 or 1 / (1 - att_dp); KP = 16 for k <= 16, else 32; columns of a
  * multi-head layer: head * seg + j): what the fused kernels apply.  For the composite training path and for tests. */
 int gf_attn_dropout_mask(const gf_attn_desc* desc, float att_dp, uint32_t dp_salt, const unsigned long long* dp_state, float* mask, void* stream);
