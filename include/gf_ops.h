@@ -91,7 +91,7 @@ int gf_mapping_fwd(const float* z, const float* w, const float* b, const float* 
  * channels-last: y[b,h,w,o] = sum_{dy,dx,i} x[b,h+dy-1,w+dx-1,i] * wt[dy*3+dx][o][i].  This is the convolution inside the reference's
  * modulated_conv2d_layer in its activation-scaling form (x already carries the style, demodulation is applied by the consumer).
  * wt comes from gf_conv3x3_pack_weights (w [Cout,Cin,3,3] * scale -> [9][Cout][Cin], rounded to TF32).
- * H % 8 == 0, W % 16 == 0, Cin % 32 == 0, Cout % 64 == 0; 16-byte aligned pointers. */
+ * B, H, W > 0, H % 8 == 0, W % 16 == 0, Cin % 32 == 0, Cout % 64 == 0; 16-byte aligned pointers. */
 int gf_conv3x3_pack_weights(const float* w, float* wt, int Cout, int Cin, float scale, void* stream);
 int gf_conv3x3_nhwc_tf32(const float* x, const float* wt, float* y, int B, int H, int W, int Cin, int Cout, void* stream);
 

@@ -49,6 +49,15 @@ def test_native_op_entry_points_validate_before_touching_the_device(gf):
     assert lib.gf_conv3x3_nhwc_tf32(1, 1, 1, 2, 8, 16, 48, 64, None) == -2 and "Cin % 32" in err()
     assert lib.gf_conv3x3_nhwc_tf32(None, 1, 1, 2, 8, 16, 32, 64, None) == -1 and "null pointer" in err()    # GF_ERR_INVALID
     assert lib.gf_conv3x3_pack_weights(None, None, 4, 4, 1.0, None) == -1
+    # the convolution's remaining checks; the pointers are never dereferenced, every call returns before the device is touched
+    A, X = 0x10000, 0x10004                                                                                 # aligned, 4 off
+    assert lib.gf_conv3x3_nhwc_tf32(A, A, A, 2, 8, 16, 32, 96, None) == -2 and "Cout % 64 == 0" in err() and "Cout=96" in err()
+    for B, H, W in ((0, 8, 16), (-1, 8, 16), (1, 0, 16), (1, -8, 16), (1, 8, 0), (1, 8, -16)):   # 0 and -8 pass H % 8 == 0
+        assert lib.gf_conv3x3_nhwc_tf32(A, A, A, B, H, W, 32, 64, None) == -2 and "positive sizes" in err(), (B, H, W)
+    for x, wt, y in ((X, A, A), (A, X, A), (A, A, X), (A + 8, A, A)):
+        assert lib.gf_conv3x3_nhwc_tf32(x, wt, y, 1, 8, 16, 32, 64, None) == -1 and "16-byte aligned" in err(), (x, wt, y)
+    for Cout, Cin in ((0, 4), (-64, 4), (4, 0)):
+        assert lib.gf_conv3x3_pack_weights(A, A, Cout, Cin, 1.0, None) == -1 and "bad arguments" in err()
     jobs = (gf._lib.GfDemodJob * 1)()
     as_ptr = ctypes.cast(jobs, ctypes.c_void_p)
     assert lib.gf_demod_coef_batch(None, 0, 4, 1e-8, None) == -1 and "1 <= n <= 32" in err()

@@ -161,3 +161,59 @@ def test_attention_dropout_algebra_of_the_oracle():
     out0a, _, _ = ob.transformer_layer(x, y, w, integration="mul", att_mult=zeros)
     out0b, _, _ = ob.transformer_layer(x, y + 3.0, w, integration="mul", att_mult=zeros)
     assert torch.allclose(out0a, out0b, atol=1e-12) and not torch.allclose(out0a, ref, atol=1e-3)
+
+
+def _f32(bits):
+    return torch.tensor([b - (1 << 32) if b >= 1 << 31 else b for b in bits], dtype=torch.int32).view(torch.float32)
+
+
+def _u32(x):
+    return [b & 0xFFFFFFFF for b in x.view(torch.int32).tolist()]
+
+
+def test_tf32_helpers_on_hand_picked_bit_patterns():
+    """oracle/tf32.py: truncation (what the tensor core does to a streamed float32 operand) and round-to-nearest-even (what the
+    library does before an operand reaches the tensor core), on ties, signs, carries into the exponent and signed zeros."""
+    from oracle.tf32 import tf32_rne, tf32_trunc
+    cases = [  # bits in, truncated, rounded to nearest even
+        (0x3F800000, 0x3F800000, 0x3F800000),   # 1.0 is a TF32 value
+        (0x3F801800, 0x3F800000, 0x3F802000),   # 1 + 3 * 2^-12: below halfway drops, above halfway rounds up
+        (0x3F801000, 0x3F800000, 0x3F800000),   # exact tie, even kept bit: stays
+        (0x3F803000, 0x3F802000, 0x3F804000),   # exact tie, odd kept bit: rounds up to even
+        (0x3F800FFF, 0x3F800000, 0x3F800000),   # just below a tie
+        (0x3F801001, 0x3F800000, 0x3F802000),   # just above a tie
+        (0xBF803000, 0xBF802000, 0xBF804000),   # negative: both act on the magnitude, the sign stays
+        (0xBF801000, 0xBF800000, 0xBF800000),   # negative exact tie, even kept bit
+        (0xBF801800, 0xBF800000, 0xBF802000),   # -(1 + 3 * 2^-12)
+        (0x3FFFF000, 0x3FFFE000, 0x40000000),   # tie on an all-ones kept mantissa: carries into the exponent, 2.0
+        (0x3FFFFFFF, 0x3FFFE000, 0x40000000),
+        (0xC07FFFFF, 0xC07FE000, 0xC0800000),   # the same carry, negative: -4.0
+        (0x00000000, 0x00000000, 0x00000000),   # +0
+        (0x80000000, 0x80000000, 0x80000000),   # -0 keeps its sign
+        (0x00001000, 0x00000000, 0x00000000),   # subnormal tie, even kept bit
+        (0x00003000, 0x00002000, 0x00004000),   # subnormal tie, odd kept bit
+        (0x807FFFFF, 0x807FE000, 0x80800000),   # largest negative subnormal carries into the smallest normal
+        (0x7F7FFFFF, 0x7F7FE000, 0x7F800000),   # largest finite float rounds to +inf, as the bit trick on the GPU does
+    ]
+    x = _f32([c[0] for c in cases])
+    assert _u32(tf32_trunc(x)) == [c[1] for c in cases]
+    assert _u32(tf32_rne(x)) == [c[2] for c in cases]
+    assert x.view(torch.int32).tolist() == _f32([c[0] for c in cases]).view(torch.int32).tolist()    # inputs untouched
+
+
+def test_tf32_helpers_match_an_arithmetic_definition():
+    """On random normal values of many magnitudes: rounding x / ulp to an integer, where ulp = 2^(exponent - 10), with numpy's
+    half-to-even rounding or toward zero, gives the same values as the bit tricks.  Shapes are kept; results are TF32 values."""
+    from oracle.tf32 import tf32_low_bits, tf32_rne, tf32_trunc
+    g = torch.Generator().manual_seed(5)
+    x = torch.randn(4, 1000, generator=g) * torch.pow(2.0, torch.randint(-60, 60, (4, 1000), generator=g).float())
+    ties = (x.view(torch.int32) & -0x2000) | 0x1000                                        # every kept-bit parity, exact ties
+    for v in (x, ties.view(torch.float32)):
+        x64 = v.double().numpy()
+        ulp = np.exp2(np.floor(np.log2(np.abs(x64))) - 10)
+        assert np.array_equal(tf32_rne(v).double().numpy(), np.round(x64 / ulp) * ulp)
+        assert np.array_equal(tf32_trunc(v).double().numpy(), np.trunc(x64 / ulp) * ulp)
+        assert tf32_rne(v).shape == v.shape
+        assert (tf32_low_bits(tf32_rne(v)) == 0).all() and (tf32_low_bits(tf32_trunc(v)) == 0).all()
+    with pytest.raises(TypeError):
+        tf32_rne(torch.ones(3, dtype=torch.float64))
