@@ -19,6 +19,7 @@
 //              slot after its third tap; then the tile's outputs go straight from registers to global.
 // Per 32-channel chunk of a BN = 256 tile this moves 3 x 20 KB + 9 x 32 KB from L2 for 9 x 2 MFLOP (0.018 B/FLOP).
 // Persistent grid (one CTA per SM), tiles handed out round-robin with the N tile innermost.
+// Second kernel: upconv_blur_tc_kernel, the upsampling layers' stride-2 transposed convolution + FIR blur + demodulation (below).
 #include <stdlib.h>
 #include <string.h>
 #include "gf_common.cuh"
@@ -175,6 +176,231 @@ conv3x3_tc_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant
 }
 
 // ---------------------------------------------------------------------------------------------------------
+// The upsampling layers: stride-2 transposed 3x3 convolution + [1,3,3,1] FIR blur + demodulation in one kernel
+// ---------------------------------------------------------------------------------------------------------
+// conv_transpose2d with stride 2 (q = 2m + k) splits per dimension into T_even[m] = w[k=0] x[m] + w[k=2] x[m-1] and
+// T_odd[m] = w[k=1] x[m].  "Phase position" (r, c) holds T_even[r] and T_odd[r-1] per dimension, so every tap reads x at a shift of
+// 0 or -1: per 32-channel chunk two activation boxes (column shift 0 and -1) of 9 rows (the 8 phase rows of a step plus one halo
+// row), the row shift being a view at a whole number of swizzle atoms.  The four phase accumulators (ee, eo, oe, oo: row phase,
+// column phase) take the taps
+//   shift (0,0) -> ee(0,0);  (0,-1) -> ee(0,2), eo(0,1);  (-1,0) -> ee(2,0), oe(1,0);  (-1,-1) -> ee(2,2), eo(2,1), oe(1,2), oo(1,1)
+// i.e. nine taps per phase position, the MMA work of a stride-1 3x3 convolution at the low resolution.  The blur, per dimension,
+//   y[2i] = T_odd[i-1] + 3 T_even[i] + 3 T_odd[i] + T_even[i+1],  y[2i+1] = T_even[i] + 3 T_odd[i] + 3 T_even[i+1] + T_odd[i+1]  (/8),
+// needs phase positions i, i+1, i+2 for output pair i; TMA's zero fill makes T_odd[-1], T_odd[H] and T_even[H+1] zero, which is the
+// blur's padding of 1.  Work unit = (image, column strip of 16 phase columns = 14 output column pairs, N tile of 64 channels); it
+// walks down the strip 8 phase rows per step and keeps the last two phase rows in shared memory for the next step's vertical blur,
+// so only the two-column horizontal halo is recomputed.  Epilogue per 16-channel slice: the accumulators go to shared memory,
+// warp k blurs output row pair 8 step - 2 + k (horizontal then vertical, fixed order, see DESIGN §5) and scales once by
+// alpha * gain * d[b, c].
+constexpr int U_PC = 16, U_PR = 8;                     // phase columns of a strip, phase rows of a step
+constexpr int U_OC = U_PC - 2;                         // complete output column pairs per strip
+constexpr int U_BN = 64;                               // output channels per unit: 4 phases x 64 / 2 = 128 accumulators per thread
+constexpr int U_A_BYTES = (U_PR + 1) * U_PC * BK * 4;  // activation box {32 ch, 16 w, 9 h}: 18 KB
+constexpr int U_W_BYTES = U_BN * BK * 4;               // one tap's weight box: 8 KB
+constexpr int U_CS = 68;                               // floats per staged phase position: 4 phases x 16 channels + 4 (bank spread)
+constexpr int U_MAX_A = 4, U_MAX_W = 10;
+
+struct UBars {
+  uint64_t full_a[U_MAX_A], empty_a[U_MAX_A], full_w[U_MAX_W], empty_w[U_MAX_W];
+};
+
+struct UParams {
+  int B, H, W, Cin, Cout;                // H, W: input (low-resolution) size
+  int strips, steps, tiles_n;
+  int total_units;
+  int na, nw;
+  float ag;                              // alpha * gain
+  const float* scale;                    // d [B, Cout]
+};
+
+// tap order inside a 32-channel chunk: box (column shift 0, then -1), row shift, filter tap ky*3+kx, target phase (ee 0, eo 1, oe 2, oo 3)
+__device__ constexpr int U_TAP[9] = {0, 6, 3, 2, 1, 8, 7, 5, 4};
+__device__ constexpr int U_PH[9] = {0, 0, 2, 0, 1, 0, 1, 2, 3};
+__device__ constexpr int U_ROW0[9] = {1, 0, 0, 1, 1, 0, 0, 0, 0};      // 1: row shift 0 (view from box row 1), 0: row shift -1
+__device__ constexpr int U_FIRST[9] = {1, 0, 1, 0, 1, 0, 0, 0, 1};     // first tap of its phase: the accumulator starts there
+
+__global__ void __launch_bounds__(NUM_THREADS, 1)
+upconv_blur_tc_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmW, float* __restrict__ y, const UParams P) {
+  extern __shared__ __align__(1024) uint8_t smem_raw[];
+  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
+  const uint32_t s_a = smem_u32(smem);
+  const uint32_t s_w = s_a + (uint32_t)P.na * U_A_BYTES;
+  float* carry = reinterpret_cast<float*>(smem + (size_t)P.na * U_A_BYTES + (size_t)P.nw * U_W_BYTES);   // [4 slices][2 rows][16][U_CS]
+  float* stage = carry + 4 * 2 * U_PC * U_CS;                                                             // [8 rows][16][U_CS]
+  UBars* bars = reinterpret_cast<UBars*>(stage + U_PR * U_PC * U_CS);
+  const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);
+  const int lane = threadIdx.x & 31;
+
+  if (warp == 8 && lane == 0) {
+    prefetch_tmap(&tmX); prefetch_tmap(&tmW);
+    for (int i = 0; i < P.na; ++i) { mbar_init(smem_u32(&bars->full_a[i]), 1); mbar_init(smem_u32(&bars->empty_a[i]), 2); }
+    for (int i = 0; i < P.nw; ++i) { mbar_init(smem_u32(&bars->full_w[i]), 1); mbar_init(smem_u32(&bars->empty_w[i]), 2); }
+    fence_barrier_init();
+  }
+  __syncthreads();
+
+  // unit index -> (n tile, strip, image); the N tile is innermost so neighbouring CTAs share their input strip in L2
+  auto decode = [&](int u, int& nt, int& st, int& b) {
+    nt = u % P.tiles_n; u /= P.tiles_n;
+    st = u % P.strips; b = u / P.strips;
+  };
+
+  if (warp == 8) {
+    // =============================== TMA producer ===============================
+    if (lane == 0) {
+      int sa = 0, sw = 0; uint32_t pa = 0, pw_ = 0;
+      for (int u = blockIdx.x; u < P.total_units; u += gridDim.x) {
+        int nt, st, b;
+        decode(u, nt, st, b);
+        const int j0 = st * U_OC, n0 = nt * U_BN;
+        for (int s = 0; s < P.steps; ++s) {
+          for (int c0 = 0; c0 < P.Cin; c0 += BK) {
+            for (int t = 0; t < 9; ++t) {
+              if (t == 0 || t == 3) {                      // box of column shift 0 (taps 0-2), then -1 (taps 3-8)
+                mbar_wait(smem_u32(&bars->empty_a[sa]), pa ^ 1u);
+                const uint32_t fa = smem_u32(&bars->full_a[sa]);
+                mbar_expect_tx(fa, (uint32_t)U_A_BYTES);
+                tma_load_4d(s_a + (uint32_t)sa * U_A_BYTES, &tmX, fa, c0, j0 - (t == 3), s * U_PR - 1, b);   // zero fill = padding
+                if (++sa == P.na) { sa = 0; pa ^= 1u; }
+              }
+              mbar_wait(smem_u32(&bars->empty_w[sw]), pw_ ^ 1u);
+              const uint32_t fw = smem_u32(&bars->full_w[sw]);
+              mbar_expect_tx(fw, (uint32_t)U_W_BYTES);
+              tma_load_2d(s_w + (uint32_t)sw * U_W_BYTES, &tmW, fw, c0, U_TAP[t] * P.Cout + n0);
+              if (++sw == P.nw) { sw = 0; pw_ ^= 1u; }
+            }
+          }
+        }
+      }
+    }
+    return;
+  }
+
+  // =============================== consumer warpgroups ===============================
+  const int wg = warp >> 2;                                    // warp k owns phase row k of the step (M rows 16k .. 16k+15)
+  const int gid = lane >> 2, qd = lane & 3;
+  const bool leader = (warp & 3) == 0 && lane == 0;
+  const int cp = lane & 7, cg = lane >> 3;                     // epilogue: channels 2 cp, 2 cp + 1 of a slice; column pairs cg, cg + 4, ...
+  int sa = 0, sw = 0; uint32_t pa = 0, pw_ = 0;
+  for (int u = blockIdx.x; u < P.total_units; u += gridDim.x) {
+    int nt, st, b;
+    decode(u, nt, st, b);
+    const int j0 = st * U_OC, n0 = nt * U_BN;
+    for (int s = 0; s < P.steps; ++s) {
+      float acc[4][U_BN / 2];
+      int prev_w = -1, prev_a = -1;
+      uint32_t a_view = 0;
+#pragma unroll 1
+      for (int c0 = 0; c0 < P.Cin; c0 += BK) {
+#pragma unroll
+        for (int t = 0; t < 9; ++t) {
+          if (t == 0 || t == 3) {
+            mbar_wait(smem_u32(&bars->full_a[sa]), pa);
+            a_view = s_a + (uint32_t)sa * U_A_BYTES + wg * 4 * U_PC * 128;     // this warpgroup's 4 phase rows, row shift -1
+          }
+          mbar_wait(smem_u32(&bars->full_w[sw]), pw_);
+          const uint64_t da = gmma_desc(a_view + U_ROW0[t] * U_PC * 128, 1024, LAYOUT_SW128);
+          const uint64_t db = gmma_desc(s_w + (uint32_t)sw * U_W_BYTES, 1024, LAYOUT_SW128);
+          const uint32_t acc0 = (c0 > 0 || !U_FIRST[t]) ? 1u : 0u;
+          wgmma_fence();
+#pragma unroll
+          for (int kk = 0; kk < 4; ++kk) wgmma_ss<U_BN>(acc[U_PH[t]], da + kk * 2, db + kk * 2, (acc0 | kk) ? 1u : 0u);
+          wgmma_commit();
+          wgmma_wait<1>();                                     // the previous tap's MMAs are done: release its slots
+          if (prev_w >= 0) {
+            named_bar_sync(1 + wg, 128);
+            if (leader) {
+              mbar_arrive(smem_u32(&bars->empty_w[prev_w]));
+              if (prev_a >= 0) mbar_arrive(smem_u32(&bars->empty_a[prev_a]));
+            }
+          }
+          prev_w = sw;
+          prev_a = (t == 2 || t == 8) ? sa : -1;               // last tap reading this box
+          if (++sw == P.nw) { sw = 0; pw_ ^= 1u; }
+          if (t == 2 || t == 8) { if (++sa == P.na) { sa = 0; pa ^= 1u; } }
+        }
+      }
+      wgmma_wait<0>();
+#pragma unroll
+      for (int ph = 0; ph < 4; ++ph) fence_regs<U_BN / 2>(acc[ph]);
+      named_bar_sync(1 + wg, 128);
+      if (leader) {
+        mbar_arrive(smem_u32(&bars->empty_w[prev_w]));
+        mbar_arrive(smem_u32(&bars->empty_a[prev_a]));
+      }
+
+      // ---- epilogue: blur + demodulation, 16 channels at a time ----
+      const int io = s * U_PR - 2 + warp;                      // output row pair of this warp
+#pragma unroll
+      for (int sl = 0; sl < U_BN / 16; ++sl) {
+        float* my_row = stage + warp * U_PC * U_CS;
+#pragma unroll
+        for (int ph = 0; ph < 4; ++ph)
+#pragma unroll
+          for (int jj = 0; jj < 2; ++jj)
+#pragma unroll
+            for (int i = 0; i < 2; ++i)
+              *reinterpret_cast<float2*>(my_row + (gid + 8 * i) * U_CS + ph * 16 + jj * 8 + 2 * qd) =
+                  make_float2(acc[ph][4 * (2 * sl + jj) + 2 * i], acc[ph][4 * (2 * sl + jj) + 2 * i + 1]);
+        named_bar_sync(3, 256);
+        if (io >= 0 && io < P.H) {
+          // staged rows: 10-row index r = 0, 1 -> the previous step's last two phase rows (carry), r >= 2 -> this step's row r - 2
+          auto row = [&](int r) -> const float* {
+            return (r < 2 ? carry + (sl * 2 + r) * U_PC * U_CS : stage + (r - 2) * U_PC * U_CS) + 2 * cp;
+          };
+          const int ch = n0 + sl * 16 + 2 * cp;
+          const float2 d = __ldg(reinterpret_cast<const float2*>(P.scale + (size_t)b * P.Cout + ch));
+          const float2 f = make_float2(P.ag * d.x, P.ag * d.y);
+          const int Wo = 2 * P.W;
+#pragma unroll 1
+          for (int p = cg; p < U_OC && j0 + p < P.W; p += 4) {   // phase column p = output column pair j0 + p
+            float* y0 = y + (((size_t)b * 2 * P.H + 2 * io) * Wo + 2 * (j0 + p)) * P.Cout + ch;
+#pragma unroll 1
+            for (int cb = 0; cb < 2; ++cb) {                   // output column 2 (j0 + p) + cb
+              // horizontal: h = A + 3 B + 3 C + D with column phases E[c] = T_even[p + c], O[c] = T_odd[p + c - 1]:
+              //   cb 0: O[0], E[0], O[1], E[1];  cb 1: E[0], O[1], E[1], O[2]
+              const int oA = cb ? 0 : 16, oB = cb ? U_CS + 16 : 0, oC = cb ? U_CS : U_CS + 16, oD = cb ? 2 * U_CS + 16 : U_CS;
+              float2 e, o;                                     // output rows 2 io, 2 io + 1
+              // five horizontally blurred rows, in the order that fixes the sums: Ho(io), He(io), Ho(io+1), He(io+1), Ho(io+2);
+              // vertical: y[2i] = Ho(i) + 3 He(i) + 3 Ho(i+1) + He(i+1),  y[2i+1] = He(i) + 3 Ho(i+1) + 3 He(i+1) + Ho(i+2)
+#pragma unroll
+              for (int v = 0; v < 5; ++v) {
+                // 10-row index of phase row io + v / 2; v = 0, 2, 4: row phase odd (oe, oo), v = 1, 3: even (ee, eo)
+                const float* base = row(warp + v / 2) + ((v & 1) ? 0 : 32) + p * U_CS;
+                const float2 A = *reinterpret_cast<const float2*>(base + oA), B_ = *reinterpret_cast<const float2*>(base + oB);
+                const float2 C = *reinterpret_cast<const float2*>(base + oC), D = *reinterpret_cast<const float2*>(base + oD);
+                float2 hv;
+                hv.x = ((A.x + 3.f * B_.x) + 3.f * C.x) + D.x;
+                hv.y = ((A.y + 3.f * B_.y) + 3.f * C.y) + D.y;
+                if (v == 0) { e = hv; }
+                else if (v == 1) { e.x += 3.f * hv.x; e.y += 3.f * hv.y; o = hv; }
+                else if (v == 2) { e.x += 3.f * hv.x; e.y += 3.f * hv.y; o.x += 3.f * hv.x; o.y += 3.f * hv.y; }
+                else if (v == 3) { e.x += hv.x; e.y += hv.y; o.x += 3.f * hv.x; o.y += 3.f * hv.y; }
+                else { o.x += hv.x; o.y += hv.y; }
+              }
+              *reinterpret_cast<float2*>(y0 + cb * P.Cout) = make_float2(e.x * 0.015625f * f.x, e.y * 0.015625f * f.y);
+              *reinterpret_cast<float2*>(y0 + (size_t)Wo * P.Cout + cb * P.Cout) = make_float2(o.x * 0.015625f * f.x, o.y * 0.015625f * f.y);
+            }
+          }
+        }
+        named_bar_sync(3, 256);                                // every read of this slice's carry and stage is done
+        if (warp >= U_PR - 2) {                                // the last two phase rows become the next step's carry
+          float* crow = carry + (sl * 2 + warp - (U_PR - 2)) * U_PC * U_CS;
+#pragma unroll
+          for (int ph = 0; ph < 4; ++ph)
+#pragma unroll
+            for (int jj = 0; jj < 2; ++jj)
+#pragma unroll
+              for (int i = 0; i < 2; ++i)
+                *reinterpret_cast<float2*>(crow + (gid + 8 * i) * U_CS + ph * 16 + jj * 8 + 2 * qd) =
+                    make_float2(acc[ph][4 * (2 * sl + jj) + 2 * i], acc[ph][4 * (2 * sl + jj) + 2 * i + 1]);
+        }
+      }
+    }
+  }
+}
+
+// ---------------------------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------------------------
 static int make_map_nhwc(CUtensorMap* m, const void* base, int B, int H, int W, int C, int box_c, int box_w, int box_h) {
@@ -223,6 +449,36 @@ static int launch(const float* x, const float* wt, float* y, int B, int H, int W
   return launch_bn<64>(x, wt, y, B, H, W, Cin, Cout, st);
 }
 
+static int launch_upconv(const float* x, const float* wt, const float* scale, float* y, int B, int H, int W, int Cin, int Cout,
+                         float gain, cudaStream_t st) {
+  CUtensorMap tmX, tmW;
+  int rc;
+  if ((rc = make_map_nhwc(&tmX, x, B, H, W, Cin, BK, U_PC, U_PR + 1))) return rc;
+  if ((rc = make_map(&tmW, wt, (uint64_t)9 * Cout, (uint64_t)Cin, U_BN, BK, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
+  UParams P;
+  P.B = B; P.H = H; P.W = W; P.Cin = Cin; P.Cout = Cout;
+  P.strips = (W + U_OC - 1) / U_OC;
+  P.steps = (H + 2 + U_PR - 1) / U_PR;            // output row pairs 8 s - 2 .. 8 s + 5 per step, 0 .. H - 1 in all
+  P.tiles_n = Cout / U_BN;
+  const long long units = (long long)B * P.strips * P.tiles_n;
+  if (units > (1ll << 30)) { set_error("upconv3x3_blur: too many work units (%lld)", units); return GF_ERR_UNSUPPORTED; }
+  P.total_units = (int)units;
+  P.ag = 1.000352220f * gain;                      // alpha: the tensor core truncates x to TF32 (see launch_bn); the weights are pre-rounded
+  P.scale = scale;
+  const int fixed = 8 * U_PC * U_CS * 4 + U_PR * U_PC * U_CS * 4 + (int)sizeof(UBars) + 1024;   // carry (4 slices x 2 rows), stage, barriers
+  P.na = U_MAX_A;
+  P.nw = (device_smem_optin() - fixed - P.na * U_A_BYTES) / U_W_BYTES;
+  if (P.nw > U_MAX_W) P.nw = U_MAX_W;
+  if (P.nw < 3) { set_error("upconv3x3_blur: shared memory too small"); return GF_ERR_UNSUPPORTED; }
+  const int smem_bytes = fixed + P.na * U_A_BYTES + P.nw * U_W_BYTES;
+  GF_CUDA_OK(cudaFuncSetAttribute(upconv_blur_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
+  long long grid = device_sms();
+  if (grid > P.total_units) grid = P.total_units;
+  upconv_blur_tc_kernel<<<(unsigned)grid, NUM_THREADS, smem_bytes, st>>>(tmX, tmW, y, P);
+  GF_LAUNCH_OK();
+  return GF_OK;
+}
+
 // w [Cout][Cin][3][3] (PyTorch layout) -> wt [9][Cout][Cin], rounded to the nearest TF32
 __global__ void pack_weights_kernel(const float* __restrict__ w, float* __restrict__ wt, int Cout, int Cin, float scale) {
   const size_t total = (size_t)9 * Cout * Cin;
@@ -259,4 +515,19 @@ extern "C" int gf_conv3x3_nhwc_tf32(const float* x, const float* wt, float* y, i
   int rc;
   if ((rc = check_device())) return rc;
   return cv::launch(x, wt, y, B, H, W, Cin, Cout, (cudaStream_t)stream);
+}
+
+extern "C" int gf_upconv3x3_blur_nhwc_tf32(const float* x, const float* wt, const float* scale, float* y, int B, int H, int W, int Cin,
+                                           int Cout, float gain, void* stream) {
+  if (!x || !wt || !scale || !y) { set_error("gf_upconv3x3_blur_nhwc_tf32: null pointer"); return GF_ERR_INVALID; }
+  if (B <= 0 || H <= 0 || W <= 0 || Cin <= 0 || Cout <= 0 || Cin % cv::BK || Cout % cv::U_BN) {
+    set_error("gf_upconv3x3_blur_nhwc_tf32: needs positive sizes, Cin %% 32 == 0, Cout %% 64 == 0 (got B=%d H=%d W=%d Cin=%d Cout=%d)", B, H, W, Cin, Cout);
+    return GF_ERR_UNSUPPORTED;
+  }
+  if (((uintptr_t)x & 15) || ((uintptr_t)wt & 15) || ((uintptr_t)y & 15) || ((uintptr_t)scale & 15)) {
+    set_error("gf_upconv3x3_blur_nhwc_tf32: pointers must be 16-byte aligned"); return GF_ERR_INVALID;
+  }
+  int rc;
+  if ((rc = check_device())) return rc;
+  return cv::launch_upconv(x, wt, scale, y, B, H, W, Cin, Cout, gain, (cudaStream_t)stream);
 }

@@ -33,6 +33,10 @@ def _inference(*params) -> bool:
     return not (torch.is_grad_enabled() and any(p.requires_grad for p in params))
 
 
+# The fused upsampling kernel (gf_upconv3x3_blur_nhwc_tf32) beats the cuDNN polyphase path only from 256^2 outputs up (DESIGN §6:
+# 3.4 vs 4.7 ms at 256^2, 2.7 vs 1.7 ms at 128^2, batch 32; 512^2 not timed): below that the layers keep the cuDNN path.
+UPCONV_FUSED_MIN_RES = 256
+
 CACHE_BYPASS = False      # set by training.Trainer while it captures a CUDA graph: weight-derived tensors must be recomputed
                           # inside the graph on every replay (a replay runs no Python, so a version-keyed cache would go stale)
 
@@ -80,8 +84,9 @@ def modulated_conv2d(x: torch.Tensor, weight: torch.Tensor, styles: torch.Tensor
     Identical in exact arithmetic to modulating the weights per sample (the reference's grouped-conv form);
     avoids B separate weight tensors.  weight [O, I, kh, kw]; styles [B, I].  The two scalings and the FIR blur of the
     upsampling path are the native ops of ops.py (gf_ops.h).  The stride-1 3x3 convolution runs on the library's own wgmma
-    implicit-GEMM kernel (wt_packed, row f1) when TF32 convolutions are allowed and the shape is eligible, else on cuDNN; the
-    polyphase up-convolutions are cuDNN.
+    implicit-GEMM kernel (wt_packed, row f1) when TF32 convolutions are allowed and the shape is eligible, else on cuDNN; with
+    wt_packed the upsampling convolution, its blur and the demodulation are one kernel of the library, otherwise the polyphase
+    up-convolutions are cuDNN (the fp32 path).
     w_eff / wsq: optional cached equalised-LR weight (already transposed for up=2) and its squared sum over the taps.
     prescaled: x already carries the style scale (fused into the producer's store).  defer_demod (up == 1 only): return
     (conv output, d) and let the consumer (the attention kernel's load side) apply the demodulation."""
@@ -105,6 +110,8 @@ def modulated_conv2d(x: torch.Tensor, weight: torch.Tensor, styles: torch.Tensor
             return x, d
         if d is not None:
             x = ops.chan_scale(x, d)
+    elif wt_packed is not None and d is not None and ops._use_cuda(x, d):
+        x = ops.upconv_blur_native(x, wt_packed, scale=d, gain=4.0)    # row f1: convolution + blur + demodulation in one kernel (TF32)
     elif phases is not None and ops._use_cuda(x, d) and O % 4 == 0 and not os.environ.get("GF_NO_PHASES"):
         x = ops.upconv_blur_phases(x, phases, scale=d, gain=4.0)       # four polyphase stride-1 convolutions + blur
     else:
@@ -208,8 +215,8 @@ class SynthesisLayer(nn.Module):
         wsq = w.square().sum(dim=[2, 3])
         phases = ops.upconv_phase_weights(w) if self.up else None
         packed = None
-        if not self.up and w.is_cuda and kh == 3 and I % 32 == 0 and O % 64 == 0:
-            packed = ops.conv3x3_pack(w)                               # [9, O, I], TF32-rounded: operand of gf_conv3x3_nhwc_tf32
+        if w.is_cuda and kh == 3 and I % 32 == 0 and O % 64 == 0 and (not self.up or self.resolution >= UPCONV_FUSED_MIN_RES):
+            packed = ops.conv3x3_pack(w)      # [9, O, I], TF32-rounded: operand of gf_conv3x3_nhwc_tf32 / gf_upconv3x3_blur_nhwc_tf32
         if self.up:
             w = w.transpose(0, 1)
         return w.contiguous(memory_format=torch.channels_last), wsq.contiguous(), phases, packed
@@ -231,9 +238,11 @@ class SynthesisLayer(nn.Module):
         w_eff = wsq = phases = packed = None
         if _inference(self.weight) and x.is_cuda:
             w_eff, wsq, phases, packed = _cached(self, "conv", (self.weight,), self._conv_weights)
-            # own convolution kernel: TF32 only (the parity tests run true-fp32 convolutions), patches of 8 x 16 pixels
-            if packed is not None and not (torch.backends.cudnn.allow_tf32 and x.dtype == torch.float32 and x.shape[2] % 8 == 0
-                                           and x.shape[3] % 16 == 0 and not os.environ.get("GF_CUDNN_CONV")):
+            # own convolution kernels: TF32 only (the parity tests run true-fp32 convolutions); the stride-1 kernel takes patches of
+            # 8 x 16 pixels and can be switched to cuDNN (GF_CUDNN_CONV), the upsampling kernel any size (packed from 256^2 up)
+            if packed is not None and not (torch.backends.cudnn.allow_tf32 and x.dtype == torch.float32
+                                           and (self.up or (x.shape[2] % 8 == 0 and x.shape[3] % 16 == 0
+                                                            and not os.environ.get("GF_CUDNN_CONV")))):
                 packed = None
         fused = self.fusable(x)
         in_scale = None
@@ -246,7 +255,7 @@ class SynthesisLayer(nn.Module):
                                            wt_packed=packed)
         else:
             x = modulated_conv2d(x, self.weight, styles, up=2 if self.up else 1, f=self.fir, w_eff=w_eff, wsq=wsq,
-                                 prescaled=prescaled, phases=phases, wt_packed=None if self.up else packed, d=demod)
+                                 prescaled=prescaled, phases=phases, wt_packed=packed, d=demod)
         if noise_mode == "const":
             noise = self.noise_const
         elif noise_mode == "random":

@@ -341,3 +341,18 @@ def conv3x3_native(x: torch.Tensor, wt: torch.Tensor) -> torch.Tensor:
         _lib.check(_lib.load().gf_conv3x3_nhwc_tf32(xv.data_ptr(), wt.data_ptr(), y.data_ptr(), B, H, W, I, O, _stream(x.device)),
                    "gf_conv3x3_nhwc_tf32")
     return y.permute(0, 3, 1, 2)
+
+
+def upconv_blur_native(x: torch.Tensor, wt: torch.Tensor, scale: torch.Tensor, gain: float = 4.0) -> torch.Tensor:
+    """Stride-2 transposed 3x3 convolution + FIR blur + demodulation (scale [B, O]) of the upsampling layers in ONE wgmma kernel
+    (row f1, TF32): x [B, I, H, W] (channels-last storage), wt = conv3x3_pack of the un-transposed w [O, I, 3, 3] -> [B, O, 2H, 2W]
+    (channels-last storage).  Same result as upconv_blur_phases up to TF32 rounding.  CUDA fp32 inference only."""
+    xv = _nhwc_view(x)
+    B, H, W, I = xv.shape
+    O = wt.shape[1]
+    y = torch.empty((B, 2 * H, 2 * W, O), dtype=torch.float32, device=x.device)
+    sc = scale.contiguous()
+    with torch.cuda.device(x.device):
+        _lib.check(_lib.load().gf_upconv3x3_blur_nhwc_tf32(xv.data_ptr(), wt.data_ptr(), sc.data_ptr(), y.data_ptr(),
+                                                           B, H, W, I, O, ctypes.c_float(gain), _stream(x.device)), "gf_upconv3x3_blur_nhwc_tf32")
+    return y.permute(0, 3, 1, 2)

@@ -95,6 +95,14 @@ int gf_mapping_fwd(const float* z, const float* w, const float* b, const float* 
 int gf_conv3x3_pack_weights(const float* w, float* wt, int Cout, int Cin, float scale, void* stream);
 int gf_conv3x3_nhwc_tf32(const float* x, const float* wt, float* y, int B, int H, int W, int Cin, int Cout, void* stream);
 
+/* Row f1, the upsampling layers: stride-2 transposed 3x3 convolution + FIR blur (use (a) above) + demodulation in one wgmma kernel,
+ * TF32, channels-last.  x [B,H,W,Cin] -> y [B,2H,2W,Cout] =
+ *   gain * scale[b,o] * blur(conv_transpose2d(x, w^T, stride 2))
+ * with wt = gf_conv3x3_pack_weights of the UN-transposed w [Cout,Cin,3,3].  H, W are the input size (any positive value);
+ * Cin % 32 == 0, Cout % 64 == 0; 16-byte aligned pointers. */
+int gf_upconv3x3_blur_nhwc_tf32(const float* x, const float* wt, const float* scale, float* y, int B, int H, int W, int Cin, int Cout,
+                                float gain, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -1,34 +1,75 @@
-"""cuDNN stride-2 transposed 3x3 convolution vs its 4-phase decomposition into stride-1 convolutions (2x2, 2x1, 1x2, 1x1
-taps) on the low-resolution input: same flops, but the phases run cuDNN's fprop kernels instead of strided dgrad."""
-import torch, torch.nn.functional as F
-torch.backends.cudnn.allow_tf32 = True; torch.backends.cudnn.benchmark = True
-dev = torch.device("cuda:0")
+"""The six upsampling layers of the 256^2 generator (batch 32) on both inference paths: today's four cuDNN polyphase convolutions
+(TF32) + the polyphase blur (ops.upconv_blur_phases), and the fused wgmma kernel (ops.upconv_blur_native).  Per layer: ms (CUDA
+events over 10 calls after warm-up), algorithmic TFLOP/s (2 * B * (2H)^2 * Cin * Cout * 9 / 4, halo not counted) and the
+algorithmic bytes (x read once + y written once), plus the rel-RMS difference between the two paths.
+
+    python tools/upconv_probe.py [--paths phases,fused] [--batch 32]
+"""
+import argparse, math, os, sys, subprocess
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+import torch
+import gansformer_b200  # noqa: F401  (registers the package)
+from importlib import import_module
+ops = import_module("gansformer-reproducibility-challenge_b200.ops")
+
+# (input res, Cin, Cout) of the 256^2 generator's upsampling layers
+LAYERS = [(4, 512, 512), (8, 512, 512), (16, 512, 512), (32, 512, 512), (64, 512, 256), (128, 256, 128)]
+
+
 def timeit(fn, n=10):
-    for _ in range(3): fn()
+    for _ in range(3):
+        fn()
     torch.cuda.synchronize()
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     e0.record()
-    for _ in range(n): fn()
-    e1.record(); torch.cuda.synchronize()
+    for _ in range(n):
+        fn()
+    e1.record()
+    torch.cuda.synchronize()
     return e0.elapsed_time(e1) / n
-B = 32
-for (H, Cin, Cout) in [(32, 512, 512), (64, 512, 256), (128, 256, 128), (16, 512, 512)]:
-    x = torch.randn(B, Cin, H, H, device=dev).contiguous(memory_format=torch.channels_last)
-    w = torch.randn(Cout, Cin, 3, 3, device=dev) / (Cin * 9) ** 0.5
-    wT = w.transpose(0, 1).contiguous(memory_format=torch.channels_last)          # [Cin, Cout, 3, 3] for conv_transpose2d
-    ph = {}
-    for a in (0, 1):
-        for b in (0, 1):
-            ky = [2, 0] if a == 0 else [1]
-            kx = [2, 0] if b == 0 else [1]
-            ph[(a, b)] = (w[:, :, ky][:, :, :, kx].contiguous(memory_format=torch.channels_last), (1 if a == 0 else 0, 1 if b == 0 else 0))
-    def ref(): return F.conv_transpose2d(x, wT, stride=2)
-    def phases(): return [F.conv2d(x, wk, padding=pad) for (wk, pad) in ph.values()]
-    with torch.no_grad():
-        T = ref(); P = phases()
-        err = 0.0
-        for (a, b), p in zip(ph.keys(), P):
-            err = max(err, (T[:, :, a::2, b::2] - p).abs().max().item())
-        t_ref, t_ph = timeit(ref), timeit(phases)
-    gf = 2 * B * H * H * 9 * Cin * Cout / 1e9
-    print(f"H={H} {Cin}->{Cout}: conv_transpose {t_ref:.3f} ms ({gf / t_ref:.0f} TF/s)  4 phases {t_ph:.3f} ms ({gf / t_ph:.0f} TF/s)  max|diff|={err:.2e}")
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--paths", default="phases,fused")
+    ap.add_argument("--batch", type=int, default=32)
+    a = ap.parse_args()
+    paths = a.paths.split(",")
+    B = a.batch
+    dev = torch.device("cuda:0")
+    torch.backends.cudnn.allow_tf32 = True
+    torch.backends.cudnn.benchmark = True
+    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True)
+    print(f"card: {q.stdout.strip()}  batch {B}")
+    print(f"{'res':>4} {'Cin':>4} {'Cout':>4} {'GB':>6} {'TFLOP':>6}" + "".join(f" {p + ' ms':>11} {'TF/s':>6} {'GB/s':>6}" for p in paths)
+          + ("  rel-rms" if len(paths) == 2 else ""))
+    tot = {p: 0.0 for p in paths}
+    g = torch.Generator(device=dev).manual_seed(0)
+    for H, ci, co in LAYERS:
+        x = torch.randn(B, ci, H, H, device=dev, generator=g).contiguous(memory_format=torch.channels_last)
+        w = torch.randn(co, ci, 3, 3, device=dev, generator=g) / math.sqrt(ci * 9)
+        d = torch.rand(B, co, device=dev, generator=g) + 0.5
+        phases = ops.upconv_phase_weights(w)
+        wt = ops.conv3x3_pack(w)
+        fns = {"phases": lambda: ops.upconv_blur_phases(x, phases, scale=d, gain=4.0),
+               "fused": lambda: ops.upconv_blur_native(x, wt, d, gain=4.0)}
+        flops = 2.0 * B * (2 * H) ** 2 * ci * co * 9 / 4
+        nbytes = 4.0 * B * H * H * ci + 4.0 * B * (2 * H) ** 2 * co
+        line = f"{2 * H:4d} {ci:4d} {co:4d} {nbytes / 1e9:6.3f} {flops / 1e12:6.3f}"
+        outs = []
+        with torch.no_grad():
+            for p in paths:
+                t = timeit(fns[p])
+                tot[p] += t
+                outs.append(fns[p]())
+                line += f" {t:11.4f} {flops / t / 1e9:6.0f} {nbytes / t / 1e6:6.0f}"
+            if len(outs) == 2:
+                diff = (outs[0] - outs[1]).pow(2).mean().sqrt() / outs[0].pow(2).mean().sqrt()
+                line += f"  {diff.item():.2e}"
+        print(line, flush=True)
+        del x, w, d, phases, wt, outs
+    print("total " + "  ".join(f"{p}: {tot[p]:.3f} ms" for p in paths))
+
+
+if __name__ == "__main__":
+    main()
