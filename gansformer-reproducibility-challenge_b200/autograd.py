@@ -11,6 +11,7 @@ recomputation of the direct-form algebra with torch ops (``composite_forward``).
 """
 from __future__ import annotations
 
+import contextlib
 import math
 
 import torch
@@ -216,6 +217,20 @@ class _FusedAttention(torch.autograd.Function):
         return (None, None, None, None, *grads)
 
 
+@contextlib.contextmanager
+def _fp32_matmul():
+    """The tables, the token reductions (K = n, up to 65,536) and the autograd through the tables of the kernel backward run as
+    true fp32 GEMMs whatever torch.backends.cuda.matmul.allow_tf32 says: with TF32 the layer gradients are about 4e-4 to 9e-4
+    relative off the fp64 reference instead of 1e-6 (DESIGN.md section 5)."""
+    prev = torch.backends.cuda.matmul.allow_tf32
+    torch.backends.cuda.matmul.allow_tf32 = False
+    try:
+        yield
+    finally:
+        torch.backends.cuda.matmul.allow_tf32 = prev
+
+
+@_fp32_matmul()
 def _kernel_backward(m, names, x, y, params, g_out, dropout=None):
     """d(loss)/d(x, y, params) of a simplex layer through gf_attn_simplex_bwd (see the module docstring)."""
     B, H, W, C = x.shape
@@ -228,6 +243,7 @@ def _kernel_backward(m, names, x, y, params, g_out, dropout=None):
     return (dX, gy, *gp)
 
 
+@_fp32_matmul()
 def _duplex_kernel_backward(m, names, x, y, params, g_out, dropout=None, centroids=None):
     """d(loss)/d(x, y, params) of a duplex layer (one k-means iteration, norm layer / none):
       1. gf_attn_centroid_stats recomputes pass A in fp32 from the tables of ``centroid_tables``: Xbar [B,k,C], lse [B,KP];

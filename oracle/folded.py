@@ -116,13 +116,29 @@ def prologue(y: Tensor, f: Dict[str, Tensor], *, C: int, H: int, W: int, p: int,
 
 
 def per_token(X: Tensor, Kp: Tensor, Vt: Tensor, Rt: Tensor, Ct: Tensor, *, H: int, W: int,
-              integration: str, norm: Optional[str], return_att: bool = False, k: Optional[int] = None):
-    """Stage T.  X [B,n,C] channels-last tokens."""
+              integration: str, norm: Optional[str], return_att: bool = False, k: Optional[int] = None,
+              att_mult: Optional[Tensor] = None, cb: Optional[Tensor] = None, retain: Optional[dict] = None):
+    """Stage T.  X [B,n,C] channels-last tokens.
+
+    att_mult [B,n,KP] (or [B,n,k]) and cb [Cout] (attention dropout, the form the kernels use): q = p * mult weights the
+    values, and the constants cb (bo, +1 on the gain half) that dropout leaves unscaled are re-added,
+    ctl = sum_j q_j (Vt_j - cb) + cb.  retain (a dict) receives the logits "S", the probabilities "P", the dropped
+    probabilities "Q" and the control signal "ctl", so that a caller can take gradients with respect to them."""
     B, n, C = X.shape
     S = X @ Kp.transpose(1, 2)                                          # [B,n,KP]
     S = S + (Rt[:, :, None, :] + Ct[:, None, :, :]).reshape(B, n, -1)
     P = torch.softmax(S, dim=2)
-    GB = P @ Vt.transpose(1, 2)                                         # [B,n,Cout]
+    if att_mult is None:
+        Q = P
+        GB = P @ Vt.transpose(1, 2)                                     # [B,n,Cout]
+    else:
+        mult = att_mult.to(P.dtype)
+        if mult.shape[2] < P.shape[2]:                                  # the padded latents have p = 0: any multiplier
+            mult = torch.nn.functional.pad(mult, (0, P.shape[2] - mult.shape[2]), value=1.0)
+        Q = P * mult
+        GB = Q @ (Vt - cb[None, :, None]).transpose(1, 2) + cb
+    if retain is not None:
+        retain.update(S=S, P=P, Q=Q, ctl=GB)
     if norm == "layer":
         mu = X.mean(dim=2, keepdim=True)
         var = ((X - mu) ** 2).mean(dim=2, keepdim=True)
@@ -152,11 +168,25 @@ def centroid_pass(X: Tensor, y: Tensor, f: Dict[str, Tensor], *, H: int, W: int,
     m_all = y @ f["AM"] + f["CM"][None]                                 # [B,k,C+p+4]
     M = m_all[:, :, :C]
     Rt, Ct = _pos_tables(m_all, C, p, H, W, KP, use_pos)
-    L = X @ M.transpose(1, 2) + (Rt[:, :, None, :k] + Ct[:, None, :, :k]).reshape(B, n, k)  # [B,n,k]
-    A = torch.softmax(L, dim=1)                                         # over n
-    xbar = A.transpose(1, 2) @ X                                        # [B,k,C]
+    _, xbar, _ = centroid_softmax(X, M, Rt, Ct, k=k)
     cen = xbar @ f["WV2"] + f["BV2"]
     return cen, xbar
+
+
+def centroid_softmax(X: Tensor, M: Tensor, Rt2: Tensor, Ct2: Tensor, *, k: Optional[int] = None,
+                     retain: Optional[dict] = None):
+    """Pass A on its tables (the layout of gf_attn_centroid_stats): the logit of token (h, w) for latent j is
+    x.M_j + Rt2[h,j] + Ct2[w,j]; the softmax runs over the n tokens.  Only the first k latents are used (default: all rows
+    of M; the padded ones have Rt2 = -inf).  Returns A [B,n,k], Xbar = A^T X [B,k,C] and lse [B,k], the log of each
+    latent's softmax denominator.  retain (a dict) receives the logits "L"."""
+    B, n, C = X.shape
+    k = M.shape[1] if k is None else k
+    L = X @ M[:, :k].transpose(1, 2) + (Rt2[:, :, None, :k] + Ct2[:, None, :, :k]).reshape(B, n, k)   # [B,n,k]
+    A = torch.softmax(L, dim=1)                                         # over n
+    xbar = A.transpose(1, 2) @ X                                        # [B,k,C]
+    if retain is not None:
+        retain.update(L=L)
+    return A, xbar, torch.logsumexp(L, dim=1)
 
 
 def transformer_layer_folded(x_nhwc: Tensor, y: Tensor, w: Dict[str, Tensor], *, integration="mul", norm="layer",
