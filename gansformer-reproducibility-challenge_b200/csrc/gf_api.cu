@@ -109,8 +109,10 @@ int gf_attn_debug_layout(const gf_attn_desc* desc, long long* out, int n) {
   Layout L;
   int rc = make_layout(desc, &L);
   if (rc) return rc;
-  const long long v[8] = {(long long)L.w_PART, (long long)L.w_XBAR, L.nsplit_cen, L.KP, (long long)L.w_M, (long long)L.w_Rt2, (long long)L.w_Ct2, (long long)L.w_total};
-  for (int i = 0; i < n && i < 8; ++i) out[i] = v[i];
+  const long long v[15] = {(long long)L.w_PART, (long long)L.w_XBAR, L.nsplit_cen, L.KP, (long long)L.w_M, (long long)L.w_Rt2, (long long)L.w_Ct2,
+                           (long long)L.w_total, (long long)L.w_Kp, (long long)L.w_Vt, (long long)L.w_Rt, (long long)L.w_Ct, (long long)L.w_CB,
+                           (long long)L.w_NSCALE, (long long)L.w_NSHIFT};
+  for (int i = 0; i < n && i < 15; ++i) out[i] = v[i];
   return GF_OK;
 }
 

@@ -135,7 +135,11 @@ long long gf_attn_launch_count(void);
  * (GF_FLAG_FP32_EXACT, instance / batch norm, C not in {64,128,256,512}, ragged n); negative gf_status on a bad descriptor. */
 int gf_attn_tc_eligible(const gf_attn_desc* desc);
 
-/* Debug aid for the bring-up probes (tools/): float offsets {w_PART, w_XBAR, nsplit_cen, KP, w_M, w_Rt2, w_Ct2, w_total} of the workspace. */
+/* Debug aid for the bring-up probes (tools/) and the kernel tests: up to n of the values
+ *   {w_PART, w_XBAR, nsplit_cen, KP, w_M, w_Rt2, w_Ct2, w_total, w_Kp, w_Vt, w_Rt, w_Ct, w_CB, w_NSCALE, w_NSHIFT}
+ * (workspace offsets in floats; nsplit_cen and KP are counts).  The stage-T tables: K' [B,KP,C], V^T [B,Cout,KP], Rt [B,H,KP],
+ * Ct [B,W,KP] and the dropout constants CB [Cout]; w_NSCALE / w_NSHIFT are 0 when the layer has no instance / batch norm.  The
+ * five duplex offsets w_PART, w_XBAR, w_M, w_Rt2 and w_Ct2 are 0 for a simplex layer.  Values past the 15th are not written. */
 int gf_attn_debug_layout(const gf_attn_desc* desc, long long* out, int n);
 
 /* Size in floats of the folded-weight buffer (stage W output + its scratch). */

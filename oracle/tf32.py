@@ -6,6 +6,8 @@ relies on (DESIGN.md section 5):
     rounds toward zero.  The 3x3 convolution streams its activations this way.
   * ``tf32_rne``: round to nearest, ties to even, the same integer trick as ``round_tf32_rn`` in csrc/gf_tc_common.cuh.  The
     packed convolution weights and the attention tables are rounded this way before they reach the tensor core.
+  * ``tf32_rna``: round to nearest, ties away from zero: what ``cvt.rna.tf32.f32`` (``cvt_tf32`` in the attention kernels) does
+    to the probabilities before they become the second GEMM's operand.
 Both work on the raw bits, so they are exact whatever the value; infinities and NaNs are outside their use here.
 """
 from __future__ import annotations
@@ -32,6 +34,15 @@ def tf32_rne(x: torch.Tensor) -> torch.Tensor:
     of the mantissa moves into the exponent, which is the correct rounding.  The sum is formed in int64 so it cannot wrap."""
     b = _bits(x).to(torch.int64) & 0xFFFFFFFF
     b = (b + 0xFFF + ((b >> 13) & 1)) & 0xFFFFE000
+    b = torch.where(b >= 2 ** 31, b - 2 ** 32, b)
+    return b.to(torch.int32).view(torch.float32).reshape(x.shape)
+
+
+def tf32_rna(x: torch.Tensor) -> torch.Tensor:
+    """Round to the nearest TF32 value, ties away from zero: add half a TF32 ulp (0x1000) to the magnitude bits, then clear the low
+    13 bits.  The sign bit is untouched, so the rounding is symmetric about zero."""
+    b = _bits(x).to(torch.int64) & 0xFFFFFFFF
+    b = (b + 0x1000) & 0xFFFFE000
     b = torch.where(b >= 2 ** 31, b - 2 ** 32, b)
     return b.to(torch.int32).view(torch.float32).reshape(x.shape)
 

@@ -20,18 +20,16 @@ The reference is fp64 autograd through the folded oracle (``oracle/attn_bwd.py``
 * Determinism, batch independence and CUDA-graph replay, bit for bit.
 """
 import ctypes
-import math
 
 import pytest
 import torch
 
 from oracle import attn_bwd as ab
 from oracle.folded import pad_k
+from tests.guards import Guarded, assert_exact as _assert_exact
 
 pytestmark = pytest.mark.gpu
 
-GUARD = 64                       # floats of NaN guard before and after every output buffer (keeps the outputs 16-byte aligned)
-GUARD_BITS = 0x7FC0DEAD          # a quiet NaN no arithmetic produces
 # Per-element bounds of |kernel - fp64 reference| / companion, per output.  Measured worst cases over the tolerance cases below on
 # an H100 80GB HBM3 (700 W power limit), frozen at 1.5x or more (DESIGN.md section 5).
 BOUND = {"dX": 1.2e-7, "dS": 1.5e-8, "P": 8e-7, "dCtl": 3e-6, "Xbar": 8e-8, "lse": 6e-8, "cen_dX": 1.1e-6, "cen_dS": 1.3e-7}
@@ -103,28 +101,6 @@ def _f32(t, dev):
     return t.float().contiguous().to(dev)
 
 
-class Guarded:
-    """An fp32 output of the given shape in the middle of a NaN-filled buffer (or preloaded with `init`)."""
-
-    def __init__(self, shape, dev, init=None):
-        self.n = math.prod(shape)
-        self.buf = torch.full((self.n + 2 * GUARD,), GUARD_BITS, dtype=torch.int32, device=dev)
-        self.t = self.buf[GUARD:GUARD + self.n].view(torch.float32).view(shape)
-        assert self.t.data_ptr() % 16 == 0
-        if init is not None:
-            self.t.copy_(init)
-
-    def ptr(self):
-        return self.t.data_ptr()
-
-    def check(self, name, written=True):
-        assert (self.buf[:GUARD] == GUARD_BITS).all(), f"{name}: written before the output"
-        assert (self.buf[GUARD + self.n:] == GUARD_BITS).all(), f"{name}: written past the output"
-        if written:
-            assert not (self.buf[GUARD:GUARD + self.n] == GUARD_BITS).any(), f"{name}: elements left unwritten"
-        return self.t
-
-
 def stage_t(gf, dev, case, *, H, W, k, integration, norm):
     """gf_attn_simplex_bwd_ex on the case's tables; returns the checked outputs on the CPU as fp64."""
     X = _f32(case["X"], dev)
@@ -191,13 +167,6 @@ def place_winners(B, n, k, ranges, seed):
             lo, hi = picks[(b + j) % 3]
             w[b, j] = torch.randint(lo, hi, (1,), generator=g)
     return w
-
-
-def _assert_exact(got, want, name):
-    assert got.shape == want.shape, name
-    bad = got != want                                   # -inf == -inf; a NaN never equals
-    assert not bad.any(), (f"{name}: {int(bad.sum())} of {got.numel()} elements differ, first at {bad.nonzero()[0].tolist()}: "
-                           f"{got[bad][0].item()} vs {want[bad][0].item()}")
 
 
 def _worst(got, want, comp, name):

@@ -491,3 +491,42 @@ def test_weight_caches_follow_the_weights_epoch(gf):
                       g_img2ltnt=True)
     a = Gi.synthesis.layers[1].attention
     assert Gi.synthesis.iterative and a.iterative and a.kmeans_iters == 2 and a.img2ltnt and {"wcq", "wi2l", "bi2l"} <= set(a.param_dict())
+
+
+@pytest.mark.parametrize("B,H,W,C,k,integration,norm,duplex", [(3, 8, 16, 64, 5, "mul", "none", False),
+                                                                (2, 10, 13, 512, 20, "both", "layer", False),
+                                                                (4, 16, 16, 96, 16, "add", "instance", False),
+                                                                (2, 46, 91, 256, 32, "mul", "layer", 1),
+                                                                (1, 8, 8, 128, 3, "both", "batch", 1)])
+def test_debug_layout_reports_disjoint_stage_t_tables(gf, B, H, W, C, k, integration, norm, duplex):
+    """gf_attn_debug_layout: the first eight values are unchanged when a caller asks for eight, and nothing past n is written.  The
+    seven appended offsets (K', V^T, Rt, Ct, CB, and the instance / batch norm scale and shift, 0 without them) and the duplex
+    regions are disjoint, lie inside w_total, and the two TMA sources K' and V^T start 16-byte aligned."""
+    L = gf._lib
+    lib = L.load()
+    desc = L.make_desc(B, H, W, C, k, 16, norm=norm, integration=integration, duplex=duplex)
+    full = (ctypes.c_longlong * 16)(*([-7] * 16))
+    L.check(lib.gf_attn_debug_layout(ctypes.byref(desc), full, 16), "gf_attn_debug_layout")
+    assert full[15] == -7
+    eight = (ctypes.c_longlong * 9)(*([-7] * 9))
+    L.check(lib.gf_attn_debug_layout(ctypes.byref(desc), eight, 8), "gf_attn_debug_layout")
+    assert list(eight[:8]) == list(full[:8]) and eight[8] == -7
+    part, xbar, nsplit, KP, w_M, w_Rt2, w_Ct2, total, w_Kp, w_Vt, w_Rt, w_Ct, w_CB, w_nsc, w_nsh = full[:15]
+    assert KP == (16 if k <= 16 else 32) and total * 4 == L.workspace_bytes(desc)
+    Cout = 2 * C if integration == "both" else C
+    regions = {"Kp": (w_Kp, B * KP * C), "Vt": (w_Vt, B * Cout * KP), "Rt": (w_Rt, B * H * KP), "Ct": (w_Ct, B * W * KP),
+               "CB": (w_CB, Cout)}
+    if norm in ("instance", "batch"):
+        regions.update(NSCALE=(w_nsc, B * C), NSHIFT=(w_nsh, B * C))
+    else:
+        assert w_nsc == 0 and w_nsh == 0
+    if duplex:
+        regions.update(M=(w_M, B * KP * C), Rt2=(w_Rt2, B * H * KP), Ct2=(w_Ct2, B * W * KP), PART=(part, B * nsplit * KP * (C + 4)),
+                       XBAR=(xbar, B * k * C))
+    else:
+        assert (part, xbar, w_M, w_Rt2, w_Ct2) == (0, 0, 0, 0, 0)
+    spans = sorted((off, off + size, name) for name, (off, size) in regions.items())
+    for (a0, a1, an), (b0, b1, bn) in zip(spans, spans[1:]):
+        assert a1 <= b0, f"{an} [{a0}, {a1}) overlaps {bn} [{b0}, {b1})"
+    assert spans[0][0] >= 0 and spans[-1][1] <= total
+    assert (w_Kp * 4) % 16 == 0 and (w_Vt * 4) % 16 == 0

@@ -217,3 +217,33 @@ def test_tf32_helpers_match_an_arithmetic_definition():
         assert (tf32_low_bits(tf32_rne(v)) == 0).all() and (tf32_low_bits(tf32_trunc(v)) == 0).all()
     with pytest.raises(TypeError):
         tf32_rne(torch.ones(3, dtype=torch.float64))
+
+
+def test_tf32_rna_rounds_ties_away_from_zero():
+    """tf32_rna (what cvt.rna.tf32.f32 does to the attention probabilities): nearest, ties away from zero whatever the kept bit,
+    on hand-picked patterns and against the arithmetic definition; it differs from tf32_rne only on ties with an even kept bit."""
+    from oracle.tf32 import tf32_low_bits, tf32_rna, tf32_rne
+    cases = [  # bits in, rounded to nearest with ties away from zero
+        (0x3F800000, 0x3F800000),
+        (0x3F801000, 0x3F802000),   # exact tie, even kept bit: away from zero (rne stays)
+        (0x3F803000, 0x3F804000),   # exact tie, odd kept bit: away from zero (as rne)
+        (0x3F800FFF, 0x3F800000),
+        (0x3F801001, 0x3F802000),
+        (0xBF801000, 0xBF802000),   # negative tie: away from zero, i.e. more negative
+        (0x3FFFF000, 0x40000000),   # carry into the exponent
+        (0x00001000, 0x00002000),   # subnormal tie
+        (0x80000000, 0x80000000),
+    ]
+    x = _f32([c[0] for c in cases])
+    assert _u32(tf32_rna(x)) == [c[1] for c in cases]
+    g = torch.Generator().manual_seed(6)
+    v = torch.randn(4, 1000, generator=g) * torch.pow(2.0, torch.randint(-60, 60, (4, 1000), generator=g).float())
+    ties = ((v.view(torch.int32) & -0x2000) | 0x1000).view(torch.float32)
+    for t in (v, ties):
+        x64 = t.double().numpy()
+        ulp = np.exp2(np.floor(np.log2(np.abs(x64))) - 10)
+        want = np.sign(x64) * np.floor(np.abs(x64) / ulp + 0.5) * ulp
+        assert np.array_equal(tf32_rna(t).double().numpy(), want)
+        assert (tf32_low_bits(tf32_rna(t)) == 0).all()
+    differ = tf32_rna(ties) != tf32_rne(ties)
+    assert torch.equal(differ, ((ties.view(torch.int32) >> 13) & 1) == 0)
