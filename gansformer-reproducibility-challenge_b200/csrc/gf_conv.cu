@@ -189,43 +189,66 @@ conv3x3_tc_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant
 // needs phase positions i, i+1, i+2 for output pair i; TMA's zero fill makes T_odd[-1], T_odd[H] and T_even[H+1] zero, which is the
 // blur's padding of 1.  Work unit = (image, column strip of 16 phase columns = 14 output column pairs, N tile of 64 channels); it
 // walks down the strip 8 phase rows per step and keeps the last two phase rows in shared memory for the next step's vertical blur,
-// so only the two-column horizontal halo is recomputed.  Epilogue per 16-channel slice: the accumulators go to shared memory,
-// warp k blurs output row pair 8 step - 2 + k (horizontal then vertical, fixed order, see DESIGN §5) and scales once by
-// alpha * gain * d[b, c].
+// so only the two-column horizontal halo is recomputed.
+// MMA: the taps of one activation shift share their A operand, so they go into as few wgmmas as the accumulators allow.  Two
+// fragments of 64 floats per thread, X = [ee, eo] and Y = [oe, oo] (64 channels per phase), and per k8 step six instructions:
+//   shift (-1,-1) -> n128 into X (taps 8, 7) and n128 into Y (taps 5, 4);  (0,-1) -> n128 into X (taps 2, 1);
+//   (-1,0) -> n64 into X (tap 6) and n64 into Y (tap 3);  (0,0) -> n64 into X (tap 0).
+// Every wgmma writes a whole fragment or its first half: one n256 over [oe, ee, eo, oo] with n128 / n64 wgmmas on sub-ranges of it
+// makes ptxas serialise all of them (C7511, "insufficient register resources for the wgmma pipeline").  The B operand of an n128 is
+// its two taps' 64-row weight boxes placed next to each other (rows of one K-major SWIZZLE_128B matrix, no repacking).  Shift
+// (-1,-1) comes first in a chunk, so in the first chunk it initialises both fragments.  Per k8 and warpgroup that is 30 KB of
+// shared-memory reads (A 6 x 2 KB, B 9 x 2 KB) for 288 MMA clocks, against 36 KB for nine per-tap n64s.
+// Shared memory: the activation ring (4 boxes of 18 KB = two chunks), one weight stage of 72 KB holding a chunk's four shift groups
+// at fixed offsets, each group with its own full / empty barrier so its slot is refilled as soon as both warpgroups have finished
+// its MMAs, and the epilogue's carry (34 KB) and stage (34 KB): 213 KB of the 227 KB.
+// Warps 0-7 are the two consumer warpgroups (setmaxnreg 232), warps 8-11 the producer warpgroup (setmaxnreg 40, one thread issues
+// the TMA); ptxas -v: 168 registers at launch, no spill.
+// Epilogue per 16-channel slice: the accumulators go to shared memory, warp k blurs output row pair 8 step - 2 + k (horizontal then
+// vertical, fixed order, see DESIGN §5) and scales once by alpha * gain * d[b, c].  It does not overlap the next step's MMAs (the
+// tensor cores idle meanwhile); a full step's staging does not fit beside the rings, see DESIGN §4.4.
 constexpr int U_PC = 16, U_PR = 8;                     // phase columns of a strip, phase rows of a step
 constexpr int U_OC = U_PC - 2;                         // complete output column pairs per strip
 constexpr int U_BN = 64;                               // output channels per unit: 4 phases x 64 / 2 = 128 accumulators per thread
 constexpr int U_A_BYTES = (U_PR + 1) * U_PC * BK * 4;  // activation box {32 ch, 16 w, 9 h}: 18 KB
 constexpr int U_W_BYTES = U_BN * BK * 4;               // one tap's weight box: 8 KB
+constexpr int U_WS_BYTES = 9 * U_W_BYTES;              // weight stage: the nine taps of a chunk, grouped by shift: 72 KB
 constexpr int U_CS = 68;                               // floats per staged phase position: 4 phases x 16 channels + 4 (bank spread)
-constexpr int U_MAX_A = 4, U_MAX_W = 10;
+constexpr int U_NA = 4;                                // activation ring slots (two chunks)
+constexpr int U_THREADS = 384;                         // warps 0-7 consumers, warps 8-11 producer warpgroup
 
 struct UBars {
-  uint64_t full_a[U_MAX_A], empty_a[U_MAX_A], full_w[U_MAX_W], empty_w[U_MAX_W];
+  uint64_t full_a[U_NA], empty_a[U_NA], full_w[4], empty_w[4];
 };
 
 struct UParams {
   int B, H, W, Cin, Cout;                // H, W: input (low-resolution) size
   int strips, steps, tiles_n;
   int total_units;
-  int na, nw;
   float ag;                              // alpha * gain
   const float* scale;                    // d [B, Cout]
 };
 
-// tap order inside a 32-channel chunk: box (column shift 0, then -1), row shift, filter tap ky*3+kx, target phase (ee 0, eo 1, oe 2, oo 3)
-__device__ constexpr int U_TAP[9] = {0, 6, 3, 2, 1, 8, 7, 5, 4};
-__device__ constexpr int U_PH[9] = {0, 0, 2, 0, 1, 0, 1, 2, 3};
-__device__ constexpr int U_ROW0[9] = {1, 0, 0, 1, 1, 0, 0, 0, 0};      // 1: row shift 0 (view from box row 1), 0: row shift -1
-__device__ constexpr int U_FIRST[9] = {1, 0, 1, 0, 1, 0, 0, 0, 1};     // first tap of its phase: the accumulator starts there
+// shift groups in issue order: 0 = shift (-1,-1), 1 = (0,-1), 2 = (-1,0), 3 = (0,0).  Groups 0, 1 read the activation box of column
+// shift -1, groups 2, 3 the box of column shift 0; U_GROW 0: row shift -1 (view from box row 0), 1: row shift 0 (from box row 1).
+// A group's weight boxes: its U_GNX taps of fragment X (phase ee, then eo), then its taps of fragment Y (oe, then oo); one or two
+// taps per fragment make one n64 or n128 wgmma.  tests/test_host_cpu_upconv_v2.py reads these tables.
+__device__ constexpr int U_GTAPS[4] = {4, 2, 2, 1};
+__device__ constexpr int U_GNX[4] = {2, 2, 1, 1};
+__device__ constexpr int U_GTAP[4][4] = {{8, 7, 5, 4}, {2, 1, 0, 0}, {6, 3, 0, 0}, {0, 0, 0, 0}};
+__device__ constexpr int U_GOFF[4] = {0, 4, 6, 8};                    // first weight box of the group in the stage
+__device__ constexpr int U_GROW[4] = {0, 1, 0, 1};
 
-__global__ void __launch_bounds__(NUM_THREADS, 1)
+__device__ __forceinline__ void setmaxnreg_dec40() { asm volatile("setmaxnreg.dec.sync.aligned.u32 40;"); }
+__device__ __forceinline__ void setmaxnreg_inc232() { asm volatile("setmaxnreg.inc.sync.aligned.u32 232;"); }
+
+__global__ void __launch_bounds__(U_THREADS, 1)
 upconv_blur_tc_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmW, float* __restrict__ y, const UParams P) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   const uint32_t s_a = smem_u32(smem);
-  const uint32_t s_w = s_a + (uint32_t)P.na * U_A_BYTES;
-  float* carry = reinterpret_cast<float*>(smem + (size_t)P.na * U_A_BYTES + (size_t)P.nw * U_W_BYTES);   // [4 slices][2 rows][16][U_CS]
+  const uint32_t s_w = s_a + (uint32_t)U_NA * U_A_BYTES;
+  float* carry = reinterpret_cast<float*>(smem + (size_t)U_NA * U_A_BYTES + U_WS_BYTES);                  // [4 slices][2 rows][16][U_CS]
   float* stage = carry + 4 * 2 * U_PC * U_CS;                                                             // [8 rows][16][U_CS]
   UBars* bars = reinterpret_cast<UBars*>(stage + U_PR * U_PC * U_CS);
   const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);
@@ -233,8 +256,8 @@ upconv_blur_tc_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_cons
 
   if (warp == 8 && lane == 0) {
     prefetch_tmap(&tmX); prefetch_tmap(&tmW);
-    for (int i = 0; i < P.na; ++i) { mbar_init(smem_u32(&bars->full_a[i]), 1); mbar_init(smem_u32(&bars->empty_a[i]), 2); }
-    for (int i = 0; i < P.nw; ++i) { mbar_init(smem_u32(&bars->full_w[i]), 1); mbar_init(smem_u32(&bars->empty_w[i]), 2); }
+    for (int i = 0; i < U_NA; ++i) { mbar_init(smem_u32(&bars->full_a[i]), 1); mbar_init(smem_u32(&bars->empty_a[i]), 2); }
+    for (int i = 0; i < 4; ++i) { mbar_init(smem_u32(&bars->full_w[i]), 1); mbar_init(smem_u32(&bars->empty_w[i]), 2); }
     fence_barrier_init();
   }
   __syncthreads();
@@ -245,30 +268,32 @@ upconv_blur_tc_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_cons
     st = u % P.strips; b = u / P.strips;
   };
 
-  if (warp == 8) {
+  if (warp >= 8) {
     // =============================== TMA producer ===============================
-    if (lane == 0) {
-      int sa = 0, sw = 0; uint32_t pa = 0, pw_ = 0;
+    setmaxnreg_dec40();
+    if (warp == 8 && lane == 0) {
+      int sa = 0; uint32_t pa = 0, pw_ = 0;
       for (int u = blockIdx.x; u < P.total_units; u += gridDim.x) {
         int nt, st, b;
         decode(u, nt, st, b);
         const int j0 = st * U_OC, n0 = nt * U_BN;
         for (int s = 0; s < P.steps; ++s) {
           for (int c0 = 0; c0 < P.Cin; c0 += BK) {
-            for (int t = 0; t < 9; ++t) {
-              if (t == 0 || t == 3) {                      // box of column shift 0 (taps 0-2), then -1 (taps 3-8)
+            for (int g = 0; g < 4; ++g) {
+              if (g == 0 || g == 2) {                      // box of column shift -1 (groups 0, 1), then 0 (groups 2, 3)
                 mbar_wait(smem_u32(&bars->empty_a[sa]), pa ^ 1u);
                 const uint32_t fa = smem_u32(&bars->full_a[sa]);
                 mbar_expect_tx(fa, (uint32_t)U_A_BYTES);
-                tma_load_4d(s_a + (uint32_t)sa * U_A_BYTES, &tmX, fa, c0, j0 - (t == 3), s * U_PR - 1, b);   // zero fill = padding
-                if (++sa == P.na) { sa = 0; pa ^= 1u; }
+                tma_load_4d(s_a + (uint32_t)sa * U_A_BYTES, &tmX, fa, c0, j0 - (g == 0), s * U_PR - 1, b);   // zero fill = padding
+                if (++sa == U_NA) { sa = 0; pa ^= 1u; }
               }
-              mbar_wait(smem_u32(&bars->empty_w[sw]), pw_ ^ 1u);
-              const uint32_t fw = smem_u32(&bars->full_w[sw]);
-              mbar_expect_tx(fw, (uint32_t)U_W_BYTES);
-              tma_load_2d(s_w + (uint32_t)sw * U_W_BYTES, &tmW, fw, c0, U_TAP[t] * P.Cout + n0);
-              if (++sw == P.nw) { sw = 0; pw_ ^= 1u; }
+              mbar_wait(smem_u32(&bars->empty_w[g]), pw_ ^ 1u);
+              const uint32_t fw = smem_u32(&bars->full_w[g]);
+              mbar_expect_tx(fw, (uint32_t)(U_GTAPS[g] * U_W_BYTES));
+              for (int k = 0; k < U_GTAPS[g]; ++k)
+                tma_load_2d(s_w + (uint32_t)(U_GOFF[g] + k) * U_W_BYTES, &tmW, fw, c0, U_GTAP[g][k] * P.Cout + n0);
             }
+            pw_ ^= 1u;
           }
         }
       }
@@ -277,55 +302,63 @@ upconv_blur_tc_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_cons
   }
 
   // =============================== consumer warpgroups ===============================
+  setmaxnreg_inc232();
   const int wg = warp >> 2;                                    // warp k owns phase row k of the step (M rows 16k .. 16k+15)
   const int gid = lane >> 2, qd = lane & 3;
   const bool leader = (warp & 3) == 0 && lane == 0;
   const int cp = lane & 7, cg = lane >> 3;                     // epilogue: channels 2 cp, 2 cp + 1 of a slice; column pairs cg, cg + 4, ...
-  int sa = 0, sw = 0; uint32_t pa = 0, pw_ = 0;
+  int sa = 0; uint32_t pa = 0, pw_ = 0;
   for (int u = blockIdx.x; u < P.total_units; u += gridDim.x) {
     int nt, st, b;
     decode(u, nt, st, b);
     const int j0 = st * U_OC, n0 = nt * U_BN;
     for (int s = 0; s < P.steps; ++s) {
-      float acc[4][U_BN / 2];
-      int prev_w = -1, prev_a = -1;
+      float accx[U_BN], accy[U_BN];                            // [ee, eo] and [oe, oo] x 64 channels: two m64n128 fragments
+      int prev_a = -1;
       uint32_t a_view = 0;
 #pragma unroll 1
       for (int c0 = 0; c0 < P.Cin; c0 += BK) {
 #pragma unroll
-        for (int t = 0; t < 9; ++t) {
-          if (t == 0 || t == 3) {
+        for (int g = 0; g < 4; ++g) {
+          if (g == 0 || g == 2) {
             mbar_wait(smem_u32(&bars->full_a[sa]), pa);
             a_view = s_a + (uint32_t)sa * U_A_BYTES + wg * 4 * U_PC * 128;     // this warpgroup's 4 phase rows, row shift -1
           }
-          mbar_wait(smem_u32(&bars->full_w[sw]), pw_);
-          const uint64_t da = gmma_desc(a_view + U_ROW0[t] * U_PC * 128, 1024, LAYOUT_SW128);
-          const uint64_t db = gmma_desc(s_w + (uint32_t)sw * U_W_BYTES, 1024, LAYOUT_SW128);
-          const uint32_t acc0 = (c0 > 0 || !U_FIRST[t]) ? 1u : 0u;
+          mbar_wait(smem_u32(&bars->full_w[g]), pw_);
+          const uint64_t da = gmma_desc(a_view + U_GROW[g] * U_PC * 128, 1024, LAYOUT_SW128);
+          const uint64_t db = gmma_desc(s_w + (uint32_t)U_GOFF[g] * U_W_BYTES, 1024, LAYOUT_SW128);
+          const uint64_t dby = db + (uint64_t)(U_GNX[g] * U_W_BYTES >> 4);         // the group's Y taps follow its X taps
+          const int ny = U_GTAPS[g] - U_GNX[g];
+          const uint32_t acc0 = (c0 > 0 || g > 0) ? 1u : 0u;  // the first chunk's shift (-1,-1) initialises both fragments
           wgmma_fence();
 #pragma unroll
-          for (int kk = 0; kk < 4; ++kk) wgmma_ss<U_BN>(acc[U_PH[t]], da + kk * 2, db + kk * 2, (acc0 | kk) ? 1u : 0u);
+          for (int kk = 0; kk < 4; ++kk) {
+            const uint32_t ac = (acc0 | kk) ? 1u : 0u;
+            if (U_GNX[g] == 2) wgmma_ss<128>(accx, da + kk * 2, db + kk * 2, ac);
+            else wgmma_ss<64>(accx, da + kk * 2, db + kk * 2, ac);
+            if (ny == 2) wgmma_ss<128>(accy, da + kk * 2, dby + kk * 2, ac);
+            else if (ny == 1) wgmma_ss<64>(accy, da + kk * 2, dby + kk * 2, ac);
+          }
           wgmma_commit();
-          wgmma_wait<1>();                                     // the previous tap's MMAs are done: release its slots
-          if (prev_w >= 0) {
+          wgmma_wait<1>();                                     // the previous group's MMAs are done: release its slots
+          if (c0 > 0 || g > 0) {
             named_bar_sync(1 + wg, 128);
             if (leader) {
-              mbar_arrive(smem_u32(&bars->empty_w[prev_w]));
+              mbar_arrive(smem_u32(&bars->empty_w[(g + 3) & 3]));
               if (prev_a >= 0) mbar_arrive(smem_u32(&bars->empty_a[prev_a]));
             }
           }
-          prev_w = sw;
-          prev_a = (t == 2 || t == 8) ? sa : -1;               // last tap reading this box
-          if (++sw == P.nw) { sw = 0; pw_ ^= 1u; }
-          if (t == 2 || t == 8) { if (++sa == P.na) { sa = 0; pa ^= 1u; } }
+          prev_a = (g == 1 || g == 3) ? sa : -1;               // last group reading this box
+          if (g == 1 || g == 3) { if (++sa == U_NA) { sa = 0; pa ^= 1u; } }
         }
+        pw_ ^= 1u;
       }
       wgmma_wait<0>();
-#pragma unroll
-      for (int ph = 0; ph < 4; ++ph) fence_regs<U_BN / 2>(acc[ph]);
+      fence_regs<U_BN>(accx);
+      fence_regs<U_BN>(accy);
       named_bar_sync(1 + wg, 128);
       if (leader) {
-        mbar_arrive(smem_u32(&bars->empty_w[prev_w]));
+        mbar_arrive(smem_u32(&bars->empty_w[3]));
         mbar_arrive(smem_u32(&bars->empty_a[prev_a]));
       }
 
@@ -341,7 +374,7 @@ upconv_blur_tc_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_cons
 #pragma unroll
             for (int i = 0; i < 2; ++i)
               *reinterpret_cast<float2*>(my_row + (gid + 8 * i) * U_CS + ph * 16 + jj * 8 + 2 * qd) =
-                  make_float2(acc[ph][4 * (2 * sl + jj) + 2 * i], acc[ph][4 * (2 * sl + jj) + 2 * i + 1]);
+                  make_float2((ph < 2 ? accx : accy)[32 * (ph & 1) + 4 * (2 * sl + jj) + 2 * i], (ph < 2 ? accx : accy)[32 * (ph & 1) + 4 * (2 * sl + jj) + 2 * i + 1]);
         named_bar_sync(3, 256);
         if (io >= 0 && io < P.H) {
           // staged rows: 10-row index r = 0, 1 -> the previous step's last two phase rows (carry), r >= 2 -> this step's row r - 2
@@ -355,32 +388,42 @@ upconv_blur_tc_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_cons
 #pragma unroll 1
           for (int p = cg; p < U_OC && j0 + p < P.W; p += 4) {   // phase column p = output column pair j0 + p
             float* y0 = y + (((size_t)b * 2 * P.H + 2 * io) * Wo + 2 * (j0 + p)) * P.Cout + ch;
-#pragma unroll 1
-            for (int cb = 0; cb < 2; ++cb) {                   // output column 2 (j0 + p) + cb
-              // horizontal: h = A + 3 B + 3 C + D with column phases E[c] = T_even[p + c], O[c] = T_odd[p + c - 1]:
-              //   cb 0: O[0], E[0], O[1], E[1];  cb 1: E[0], O[1], E[1], O[2]
-              const int oA = cb ? 0 : 16, oB = cb ? U_CS + 16 : 0, oC = cb ? U_CS : U_CS + 16, oD = cb ? 2 * U_CS + 16 : U_CS;
-              float2 e, o;                                     // output rows 2 io, 2 io + 1
-              // five horizontally blurred rows, in the order that fixes the sums: Ho(io), He(io), Ho(io+1), He(io+1), Ho(io+2);
-              // vertical: y[2i] = Ho(i) + 3 He(i) + 3 Ho(i+1) + He(i+1),  y[2i+1] = He(i) + 3 Ho(i+1) + 3 He(i+1) + Ho(i+2)
+            // horizontal: h = A + 3 B + 3 C + D with column phases E[c] = T_even[p + c], O[c] = T_odd[p + c - 1]:
+            //   output column 2 (j0 + p):     O[0], E[0], O[1], E[1];  2 (j0 + p) + 1: E[0], O[1], E[1], O[2]
+            float2 e0, o0, e1, o1;                             // output rows 2 io (e), 2 io + 1 (o) of both columns
+            // five horizontally blurred rows, in the order that fixes the sums: Ho(io), He(io), Ho(io+1), He(io+1), Ho(io+2);
+            // vertical: y[2i] = Ho(i) + 3 He(i) + 3 Ho(i+1) + He(i+1),  y[2i+1] = He(i) + 3 Ho(i+1) + 3 He(i+1) + Ho(i+2)
 #pragma unroll
-              for (int v = 0; v < 5; ++v) {
-                // 10-row index of phase row io + v / 2; v = 0, 2, 4: row phase odd (oe, oo), v = 1, 3: even (ee, eo)
-                const float* base = row(warp + v / 2) + ((v & 1) ? 0 : 32) + p * U_CS;
-                const float2 A = *reinterpret_cast<const float2*>(base + oA), B_ = *reinterpret_cast<const float2*>(base + oB);
-                const float2 C = *reinterpret_cast<const float2*>(base + oC), D = *reinterpret_cast<const float2*>(base + oD);
-                float2 hv;
-                hv.x = ((A.x + 3.f * B_.x) + 3.f * C.x) + D.x;
-                hv.y = ((A.y + 3.f * B_.y) + 3.f * C.y) + D.y;
-                if (v == 0) { e = hv; }
-                else if (v == 1) { e.x += 3.f * hv.x; e.y += 3.f * hv.y; o = hv; }
-                else if (v == 2) { e.x += 3.f * hv.x; e.y += 3.f * hv.y; o.x += 3.f * hv.x; o.y += 3.f * hv.y; }
-                else if (v == 3) { e.x += hv.x; e.y += hv.y; o.x += 3.f * hv.x; o.y += 3.f * hv.y; }
-                else { o.x += hv.x; o.y += hv.y; }
+            for (int v = 0; v < 5; ++v) {
+              // 10-row index of phase row io + v / 2; v = 0, 2, 4: row phase odd (oe, oo), v = 1, 3: even (ee, eo)
+              const float* base = row(warp + v / 2) + ((v & 1) ? 0 : 32) + p * U_CS;
+              const float2 E0 = *reinterpret_cast<const float2*>(base), O0 = *reinterpret_cast<const float2*>(base + 16);
+              const float2 E1 = *reinterpret_cast<const float2*>(base + U_CS), O1 = *reinterpret_cast<const float2*>(base + U_CS + 16);
+              const float2 O2 = *reinterpret_cast<const float2*>(base + 2 * U_CS + 16);
+              float2 h0, h1;
+              h0.x = ((O0.x + 3.f * E0.x) + 3.f * O1.x) + E1.x;
+              h0.y = ((O0.y + 3.f * E0.y) + 3.f * O1.y) + E1.y;
+              h1.x = ((E0.x + 3.f * O1.x) + 3.f * E1.x) + O2.x;
+              h1.y = ((E0.y + 3.f * O1.y) + 3.f * E1.y) + O2.y;
+              if (v == 0) { e0 = h0; e1 = h1; }
+              else if (v == 1) {
+                e0.x += 3.f * h0.x; e0.y += 3.f * h0.y; o0 = h0;
+                e1.x += 3.f * h1.x; e1.y += 3.f * h1.y; o1 = h1;
+              } else if (v == 2) {
+                e0.x += 3.f * h0.x; e0.y += 3.f * h0.y; o0.x += 3.f * h0.x; o0.y += 3.f * h0.y;
+                e1.x += 3.f * h1.x; e1.y += 3.f * h1.y; o1.x += 3.f * h1.x; o1.y += 3.f * h1.y;
+              } else if (v == 3) {
+                e0.x += h0.x; e0.y += h0.y; o0.x += 3.f * h0.x; o0.y += 3.f * h0.y;
+                e1.x += h1.x; e1.y += h1.y; o1.x += 3.f * h1.x; o1.y += 3.f * h1.y;
+              } else {
+                o0.x += h0.x; o0.y += h0.y;
+                o1.x += h1.x; o1.y += h1.y;
               }
-              *reinterpret_cast<float2*>(y0 + cb * P.Cout) = make_float2(e.x * 0.015625f * f.x, e.y * 0.015625f * f.y);
-              *reinterpret_cast<float2*>(y0 + (size_t)Wo * P.Cout + cb * P.Cout) = make_float2(o.x * 0.015625f * f.x, o.y * 0.015625f * f.y);
             }
+            *reinterpret_cast<float2*>(y0) = make_float2(e0.x * 0.015625f * f.x, e0.y * 0.015625f * f.y);
+            *reinterpret_cast<float2*>(y0 + P.Cout) = make_float2(e1.x * 0.015625f * f.x, e1.y * 0.015625f * f.y);
+            *reinterpret_cast<float2*>(y0 + (size_t)Wo * P.Cout) = make_float2(o0.x * 0.015625f * f.x, o0.y * 0.015625f * f.y);
+            *reinterpret_cast<float2*>(y0 + (size_t)Wo * P.Cout + P.Cout) = make_float2(o1.x * 0.015625f * f.x, o1.y * 0.015625f * f.y);
           }
         }
         named_bar_sync(3, 256);                                // every read of this slice's carry and stage is done
@@ -393,7 +436,7 @@ upconv_blur_tc_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_cons
 #pragma unroll
               for (int i = 0; i < 2; ++i)
                 *reinterpret_cast<float2*>(crow + (gid + 8 * i) * U_CS + ph * 16 + jj * 8 + 2 * qd) =
-                    make_float2(acc[ph][4 * (2 * sl + jj) + 2 * i], acc[ph][4 * (2 * sl + jj) + 2 * i + 1]);
+                    make_float2((ph < 2 ? accx : accy)[32 * (ph & 1) + 4 * (2 * sl + jj) + 2 * i], (ph < 2 ? accx : accy)[32 * (ph & 1) + 4 * (2 * sl + jj) + 2 * i + 1]);
         }
       }
     }
@@ -465,16 +508,13 @@ static int launch_upconv(const float* x, const float* wt, const float* scale, fl
   P.total_units = (int)units;
   P.ag = 1.000352220f * gain;                      // alpha: the tensor core truncates x to TF32 (see launch_bn); the weights are pre-rounded
   P.scale = scale;
-  const int fixed = 8 * U_PC * U_CS * 4 + U_PR * U_PC * U_CS * 4 + (int)sizeof(UBars) + 1024;   // carry (4 slices x 2 rows), stage, barriers
-  P.na = U_MAX_A;
-  P.nw = (device_smem_optin() - fixed - P.na * U_A_BYTES) / U_W_BYTES;
-  if (P.nw > U_MAX_W) P.nw = U_MAX_W;
-  if (P.nw < 3) { set_error("upconv3x3_blur: shared memory too small"); return GF_ERR_UNSUPPORTED; }
-  const int smem_bytes = fixed + P.na * U_A_BYTES + P.nw * U_W_BYTES;
+  // activation ring, weight stage, carry (4 slices x 2 rows), stage, barriers, alignment slack
+  const int smem_bytes = U_NA * U_A_BYTES + U_WS_BYTES + 8 * U_PC * U_CS * 4 + U_PR * U_PC * U_CS * 4 + (int)sizeof(UBars) + 1024;
+  if (smem_bytes > device_smem_optin()) { set_error("upconv3x3_blur: shared memory too small"); return GF_ERR_UNSUPPORTED; }
   GF_CUDA_OK(cudaFuncSetAttribute(upconv_blur_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
   long long grid = device_sms();
   if (grid > P.total_units) grid = P.total_units;
-  upconv_blur_tc_kernel<<<(unsigned)grid, NUM_THREADS, smem_bytes, st>>>(tmX, tmW, y, P);
+  upconv_blur_tc_kernel<<<(unsigned)grid, U_THREADS, smem_bytes, st>>>(tmX, tmW, y, P);
   GF_LAUNCH_OK();
   return GF_OK;
 }

@@ -33,9 +33,12 @@ def _inference(*params) -> bool:
     return not (torch.is_grad_enabled() and any(p.requires_grad for p in params))
 
 
-# The fused upsampling kernel (gf_upconv3x3_blur_nhwc_tf32) beats the cuDNN polyphase path only from 256^2 outputs up (DESIGN §6:
-# 3.4 vs 4.7 ms at 256^2, 2.7 vs 1.7 ms at 128^2, batch 32; 512^2 not timed): below that the layers keep the cuDNN path.
-UPCONV_FUSED_MIN_RES = 256
+# Output resolutions whose upsampling layer runs on the fused kernel (gf_upconv3x3_blur_nhwc_tf32): those where tools/upconv_probe.py
+# measured it at least 20 % faster than the cuDNN polyphase path, judged against cuDNN's fastest run (DESIGN §6, batch 32, H100
+# 80GB HBM3 at 400 W: 0.058 vs 0.099-0.134 ms at 8^2, 2.14 vs 4.69 ms at 256^2); 512^2 is not timed and takes the kernel, whose lead
+# grows with the layer.  16^2 .. 128^2 keep cuDNN (0.126 vs 0.111-0.188 ms at 16^2, 1.86 vs 1.70 ms at 128^2).
+def upconv_fused(res: int) -> bool:
+    return res == 8 or res >= 256
 
 CACHE_BYPASS = False      # set by training.Trainer while it captures a CUDA graph: weight-derived tensors must be recomputed
                           # inside the graph on every replay (a replay runs no Python, so a version-keyed cache would go stale)
@@ -215,7 +218,7 @@ class SynthesisLayer(nn.Module):
         wsq = w.square().sum(dim=[2, 3])
         phases = ops.upconv_phase_weights(w) if self.up else None
         packed = None
-        if w.is_cuda and kh == 3 and I % 32 == 0 and O % 64 == 0 and (not self.up or self.resolution >= UPCONV_FUSED_MIN_RES):
+        if w.is_cuda and kh == 3 and I % 32 == 0 and O % 64 == 0 and (not self.up or upconv_fused(self.resolution)):
             packed = ops.conv3x3_pack(w)      # [9, O, I], TF32-rounded: operand of gf_conv3x3_nhwc_tf32 / gf_upconv3x3_blur_nhwc_tf32
         if self.up:
             w = w.transpose(0, 1)
@@ -239,7 +242,7 @@ class SynthesisLayer(nn.Module):
         if _inference(self.weight) and x.is_cuda:
             w_eff, wsq, phases, packed = _cached(self, "conv", (self.weight,), self._conv_weights)
             # own convolution kernels: TF32 only (the parity tests run true-fp32 convolutions); the stride-1 kernel takes patches of
-            # 8 x 16 pixels and can be switched to cuDNN (GF_CUDNN_CONV), the upsampling kernel any size (packed from 256^2 up)
+            # 8 x 16 pixels and can be switched to cuDNN (GF_CUDNN_CONV), the upsampling kernel any size (packed where upconv_fused)
             if packed is not None and not (torch.backends.cudnn.allow_tf32 and x.dtype == torch.float32
                                            and (self.up or (x.shape[2] % 8 == 0 and x.shape[3] % 16 == 0
                                                             and not os.environ.get("GF_CUDNN_CONV")))):

@@ -1,7 +1,8 @@
 """The six upsampling layers of the 256^2 generator (batch 32) on both inference paths: today's four cuDNN polyphase convolutions
 (TF32) + the polyphase blur (ops.upconv_blur_phases), and the fused wgmma kernel (ops.upconv_blur_native).  Per layer: ms (CUDA
 events over 10 calls after warm-up), algorithmic TFLOP/s (2 * B * (2H)^2 * Cin * Cout * 9 / 4, halo not counted) and the
-algorithmic bytes (x read once + y written once), plus the rel-RMS difference between the two paths.
+algorithmic bytes (x read once + y written once), the fused kernel's MMA work issued over the algorithmic work ("issued": strips of
+16 phase columns for 14 output column pairs, steps of 8 phase rows over H + 2), plus the rel-RMS difference between the two paths.
 
     python tools/upconv_probe.py [--paths phases,fused] [--batch 32]
 """
@@ -14,6 +15,12 @@ ops = import_module("gansformer-reproducibility-challenge_b200.ops")
 
 # (input res, Cin, Cout) of the 256^2 generator's upsampling layers
 LAYERS = [(4, 512, 512), (8, 512, 512), (16, 512, 512), (32, 512, 512), (64, 512, 256), (128, 256, 128)]
+
+
+def issued_over_algorithmic(H, W):
+    """MMA work upconv_blur_tc_kernel issues (16 x 8 phase positions per strip and step) over the H x W phase positions needed."""
+    strips, steps = (W + 13) // 14, (H + 2 + 7) // 8
+    return strips * 16 * steps * 8 / (H * W)
 
 
 def timeit(fn, n=10):
@@ -41,7 +48,7 @@ def main():
     torch.backends.cudnn.benchmark = True
     q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True)
     print(f"card: {q.stdout.strip()}  batch {B}")
-    print(f"{'res':>4} {'Cin':>4} {'Cout':>4} {'GB':>6} {'TFLOP':>6}" + "".join(f" {p + ' ms':>11} {'TF/s':>6} {'GB/s':>6}" for p in paths)
+    print(f"{'res':>4} {'Cin':>4} {'Cout':>4} {'GB':>6} {'TFLOP':>6} {'issued':>6}" + "".join(f" {p + ' ms':>11} {'TF/s':>6} {'GB/s':>6}" for p in paths)
           + ("  rel-rms" if len(paths) == 2 else ""))
     tot = {p: 0.0 for p in paths}
     g = torch.Generator(device=dev).manual_seed(0)
@@ -55,7 +62,7 @@ def main():
                "fused": lambda: ops.upconv_blur_native(x, wt, d, gain=4.0)}
         flops = 2.0 * B * (2 * H) ** 2 * ci * co * 9 / 4
         nbytes = 4.0 * B * H * H * ci + 4.0 * B * (2 * H) ** 2 * co
-        line = f"{2 * H:4d} {ci:4d} {co:4d} {nbytes / 1e9:6.3f} {flops / 1e12:6.3f}"
+        line = f"{2 * H:4d} {ci:4d} {co:4d} {nbytes / 1e9:6.3f} {flops / 1e12:6.3f} {issued_over_algorithmic(H, H):6.2f}"
         outs = []
         with torch.no_grad():
             for p in paths:
