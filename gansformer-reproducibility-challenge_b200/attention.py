@@ -365,6 +365,11 @@ class BipartiteAttention(nn.Module):
     'add' | 'both'), ``norm`` ('layer' | 'instance' | 'batch' | None), ``kmeans`` (duplex), ``kmeans_iters`` (1).
     """
 
+    # Opt-in (per module) for a duplex layer: the backward is always the duplex kernel backward (autograd._duplex_kernel_backward),
+    # with or without dropout, and the centroids output is differentiable.  That backward has no derivative of its own, so it
+    # raises when called with grad mode on (create_graph).  The discriminator sets it; generator layers keep their routes.
+    kernel_backward = False
+
     def __init__(self, dim: int, latent_dim: int, components_num: int, pos_dim: Optional[int] = None,
                  num_heads: int = 1, integration: str = "mul", norm: Optional[str] = "layer", kmeans: bool = False,
                  kmeans_iters: int = 1, use_pos: bool = True, att_dp: float = 0.0, exact_fp32: bool = False, img2ltnt: bool = False,

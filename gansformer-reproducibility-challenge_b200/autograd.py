@@ -6,6 +6,8 @@ batched GEMMs for the reductions over tokens, and torch autograd through the tin
 (``folded_tables``).  Backward of a duplex layer (one k-means iteration, layer norm / none) whose forward ran with attention
 dropout: the same stage-T kernel with keys from the centroids, plus the pass-A kernels ``gf_attn_centroid_stats`` /
 ``gf_attn_centroid_bwd`` and autograd through the pass-A tables (``centroid_tables``), see ``_duplex_kernel_backward``.
+A duplex module with ``kernel_backward = True`` (the discriminator's layers) takes that route without dropout too, and its
+centroids output is differentiable (the cotangent joins the same autograd call).
 Everything else (duplex without dropout, instance / batch norm, multi-head, CPU tensors): PyTorch autograd through a
 recomputation of the direct-form algebra with torch ops (``composite_forward``).
 """
@@ -192,13 +194,23 @@ class _FusedAttention(torch.autograd.Function):
         ctx.module, ctx.names, ctx.centroids = module, names, centroids
         ctx.dropout = module.dropout_postop(x.device)                  # the backward regenerates the same mask (same device state)
         ctx.save_for_backward(x, y, *params)
-        ctx.mark_non_differentiable(*[t for t in (att, cen) if t is not None])
+        ctx.cen_grad = module.kernel_backward and module.duplex and centroids is None     # computed centroids, differentiable
+        ctx.mark_non_differentiable(*[t for t in (att, cen) if t is not None and not (t is cen and ctx.cen_grad)])
         return out, att, cen
 
     @staticmethod
     def backward(ctx, g_out, g_att, g_cen):
         m = ctx.module
         x, y, *params = ctx.saved_tensors
+        if m.kernel_backward and m.duplex:
+            if torch.is_grad_enabled():
+                raise RuntimeError("the duplex kernel backward has no derivative of its own (create_graph=True): run the layer "
+                                   "through composite_forward for higher-order gradients, as Discriminator does in the R1 pass")
+            if not _duplex_kernel_backward_ok(m, x):
+                raise NotImplementedError("kernel_backward serves single-head duplex layers with kmeans_iters == 1, norm layer / none, "
+                                          "float32 CUDA tensors")
+            return (None, None, None, None, *_duplex_kernel_backward(m, ctx.names, x, y, params, g_out, ctx.dropout, ctx.centroids,
+                                                                     g_cen if ctx.cen_grad else None))
         if _kernel_backward_ok(m, x):
             return (None, None, None, None, *_kernel_backward(m, ctx.names, x, y, params, g_out, ctx.dropout))
         if ctx.dropout and _duplex_kernel_backward_ok(m, x):
@@ -244,12 +256,13 @@ def _kernel_backward(m, names, x, y, params, g_out, dropout=None):
 
 
 @_fp32_matmul()
-def _duplex_kernel_backward(m, names, x, y, params, g_out, dropout=None, centroids=None):
+def _duplex_kernel_backward(m, names, x, y, params, g_out, dropout=None, centroids=None, g_cen=None):
     """d(loss)/d(x, y, params) of a duplex layer (one k-means iteration, norm layer / none):
       1. gf_attn_centroid_stats recomputes pass A in fp32 from the tables of ``centroid_tables``: Xbar [B,k,C], lse [B,KP];
       2. Cen = Xbar Wv2_e + bv2 in torch (Xbar a leaf) and the stage-T tables from it (``folded_tables`` with centroids);
       3. stage T's backward (gf_attn_simplex_bwd_ex with a simplex descriptor of the same shape, same dropout), its token
-         reductions and autograd over the tables: dX, and the gradients of y, the parameters and Xbar;
+         reductions and autograd over the tables: dX, and the gradients of y, the parameters and Xbar; with ``g_cen`` (the
+         cotangent of the centroids output) Cen is one more (output, cotangent) pair of that autograd call;
       4. r = dXbar . Xbar, then gf_attn_centroid_bwd adds the pass-A part into dX and gives dS of the pass-A logits;
       5. dM = dS^T X, dRt2 / dCt2 = sums of dS, and autograd over the pass-A tables.
     With ``centroids`` given, pass A did not run in the forward: steps 1, 4 and 5 are skipped and the centroids get no gradient."""
@@ -269,6 +282,8 @@ def _duplex_kernel_backward(m, names, x, y, params, g_out, dropout=None, centroi
             cen = centroids.detach()
         tables = folded_tables(ys, pdict, H=H, W=W, C=C, integration=m.integration, use_pos=m.use_pos, centroids=cen, img2ltnt=m.img2ltnt)
     dX, outs, grads = _stage_t_backward(m, x, k, D, g_out, tables, dropout)
+    if g_cen is not None:
+        outs, grads = outs + [cen], grads + [g_cen.contiguous()]
     leaves = [ys, *ps] + ([xbar] if centroids is None else [])
     g1 = list(torch.autograd.grad(outs, leaves, grads, allow_unused=True))
     if centroids is None:

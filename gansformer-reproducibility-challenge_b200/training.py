@@ -9,8 +9,11 @@ gradient all-reduce.  Here: one process per GPU, gradients averaged through ONE 
 
 The attention layers run their CUDA forward.  Their backward (``autograd.py``) is the hand-written stage-T backward kernel for
 simplex layers, the same kernel plus the pass-A backward kernels for duplex layers with attention dropout, and the torch
-composite for the rest (duplex layers without dropout, instance / batch norm, multi-head).  The discriminator is plain PyTorch plumbing (cuDNN convolutions): it is not on
-the hot path.  Path-length regularisation and augmentation are out of scope.
+composite for the rest (duplex layers without dropout, instance / batch norm, multi-head).  The discriminator is PyTorch plumbing
+(cuDNN convolutions, the native FIR); with ``transformer=True`` it also has the paper's bipartite attention: duplex layers
+aggregating the image into learned latents that are carried from layer to layer and concatenated to the final features.  Those
+layers run the CUDA forward and the duplex kernel backward (``BipartiteAttention.kernel_backward``), and the torch composite in
+the R1 pass, which needs their second derivative.  Path-length regularisation and augmentation are out of scope.
 """
 from __future__ import annotations
 
@@ -23,7 +26,9 @@ import torch
 import torch.nn as nn
 import torch.nn.functional as F
 
-from . import dist as gdist
+from . import _lib, dist as gdist
+from .attention import BipartiteAttention
+from .autograd import _e, composite_forward
 from .networks import FullyConnected, nf
 from ._state import bump_weights_epoch
 from .ops import fir4, fir_filter, upfirdn2d_ref
@@ -58,45 +63,107 @@ class EqConv2d(nn.Module):
         return F.leaky_relu(x, 0.2) * SQRT2 if self.act == "lrelu" else x
 
 
+def _d_attention(C: int, resolution: int, att: dict) -> BipartiteAttention:
+    """One duplex attention layer of the discriminator (SURVEY A.4 item 11).  The shape is checked against the library here, so an
+    unsupported one raises at construction with the library's own message."""
+    if att["norm"] not in ("layer", None, "none"):
+        raise ValueError(f"discriminator attention runs the duplex kernel backward: norm 'layer' or None, got {att['norm']!r}")
+    k, D = att["components_num"], att["latent_dim"]
+    _lib.workspace_bytes(_lib.make_desc(1, resolution, resolution, C, k, D, norm=att["norm"], integration=att["integration"],
+                                        pos_dim=D if att["use_pos"] else 0, duplex=1, flags=_lib.FLAG_IMG2LTNT))
+    m = BipartiteAttention(C, D, k, integration=att["integration"], norm=att["norm"], kmeans=True, kmeans_iters=1, img2ltnt=True,
+                           use_pos=att["use_pos"], exact_fp32=att["exact_fp32"])
+    m.kernel_backward = True          # no generator gradients to preserve: the duplex kernel backward from the start
+    return m
+
+
+def _attend(att: BipartiteAttention, x: torch.Tensor, y: torch.Tensor, composite: bool):
+    """x [B,C,H,W] (channels-last memory), Y [B,k,D] -> (attended x, the Y carried to the next attention layer).
+
+    The carry is the layer's own value input, Y <- LN(Y) (1 + Cen Wi2l_e + bi2l), with Cen the layer's centroids.  ``composite``
+    runs the layer as torch ops (``composite_forward``), which can be differentiated twice (R1)."""
+    xt = x.permute(0, 2, 3, 1).contiguous()                            # [B,H,W,C]: a view of a channels-last activation
+    if composite:
+        out, cen = composite_forward(xt, y, att.param_dict(), integration=att.integration, norm=att.norm, duplex=True,
+                                     use_pos=att.use_pos, img2ltnt=True)
+    else:
+        out, _, cen = att(xt, y)
+    ym = y.mean(dim=2, keepdim=True)
+    yn = (y - ym) * torch.rsqrt(((y - ym) ** 2).mean(dim=2, keepdim=True) + 1e-8)
+    y = (yn * (1.0 + cen @ _e(att.wi2l) + att.bi2l)).contiguous()
+    return out.permute(0, 3, 1, 2), y
+
+
 class DiscriminatorBlock(nn.Module):
-    def __init__(self, in_ch: int, out_ch: int):
+    """Residual block; with ``attention`` (a dict of the discriminator's attention options) a duplex attention layer follows conv0
+    and another follows conv1, on the main path before the residual sum."""
+
+    def __init__(self, in_ch: int, out_ch: int, resolution: Optional[int] = None, attention: Optional[dict] = None):
         super().__init__()
         self.conv0 = EqConv2d(in_ch, in_ch, 3)
         self.conv1 = EqConv2d(in_ch, out_ch, 3, down=True)
         self.skip = EqConv2d(in_ch, out_ch, 1, down=True, bias=False, act="linear")
+        self.att0 = _d_attention(in_ch, resolution, attention) if attention else None
+        self.att1 = _d_attention(out_ch, resolution // 2, attention) if attention else None
 
-    def forward(self, x):
-        return (self.skip(x) + self.conv1(self.conv0(x))) * (1.0 / SQRT2)
+    def forward(self, x, y=None, composite: bool = False):
+        """x [B,C,H,W], Y [B,k,D] | None -> (x', Y')."""
+        if self.att0 is None:
+            return (self.skip(x) + self.conv1(self.conv0(x))) * (1.0 / SQRT2), y
+        h, y = _attend(self.att0, self.conv0(x), y, composite)
+        h, y = _attend(self.att1, self.conv1(h), y, composite)
+        return (self.skip(x) + h) * (1.0 / SQRT2), y
 
 
 class Discriminator(nn.Module):
-    """StyleGAN2 residual discriminator (config f channel schedule), images [B,3,R,R] -> logits [B]."""
+    """StyleGAN2 residual discriminator (config f channel schedule), images [B,3,R,R] -> logits [B].
 
-    def __init__(self, resolution: int = 256, fmap_base: int = 16384, fmap_max: int = 512, mbstd_group: int = 4):
+    ``transformer=True`` adds the GANsformer discriminator's bipartite attention (SURVEY A.4 item 11): learned aggregator latents
+    ``latents`` [k, D] are broadcast to Y [B,k,D]; every block whose input resolution lies in [d_start_res, d_end_res] runs a
+    duplex layer (one k-means iteration, g_img2ltnt) after conv0 and after conv1; Y is carried from layer to layer and fc0 takes
+    [flatten(x), flatten(Y)].  The layers run the CUDA forward and the duplex kernel backward; when the image and the parameters
+    both require grad under grad mode (the R1 pass), they run ``composite_forward`` instead, which has a second derivative."""
+
+    def __init__(self, resolution: int = 256, fmap_base: int = 16384, fmap_max: int = 512, mbstd_group: int = 4,
+                 transformer: bool = False, components_num: int = 16, latent_dim: int = 32, d_start_res: int = 8,
+                 d_end_res: Optional[int] = None, integration: str = "mul", norm: Optional[str] = "layer", use_pos: bool = True,
+                 exact_fp32: bool = False):
         super().__init__()
-        self.resolution, self.mbstd_group = resolution, mbstd_group
+        self.resolution, self.mbstd_group, self.transformer = resolution, mbstd_group, transformer
         log2 = int(math.log2(resolution))
+        d_end_res = resolution if d_end_res is None else d_end_res
+        att = dict(components_num=components_num, latent_dim=latent_dim, integration=integration, norm=norm, use_pos=use_pos,
+                   exact_fp32=exact_fp32) if transformer else None
         self.fromrgb = EqConv2d(3, nf(resolution, fmap_base, fmap_max), 1)
-        self.blocks = nn.ModuleList([DiscriminatorBlock(nf(2 ** i, fmap_base, fmap_max), nf(2 ** (i - 1), fmap_base, fmap_max))
+        self.blocks = nn.ModuleList([DiscriminatorBlock(nf(2 ** i, fmap_base, fmap_max), nf(2 ** (i - 1), fmap_base, fmap_max), 2 ** i,
+                                                        att if d_start_res <= 2 ** i <= d_end_res else None)
                                      for i in range(log2, 2, -1)])
         c4 = nf(4, fmap_base, fmap_max)
         self.conv4 = EqConv2d(c4 + 1, c4, 3)
-        self.fc0 = FullyConnected(c4 * 16, c4, act="lrelu")
+        self.fc0 = FullyConnected(c4 * 16 + (components_num * latent_dim if transformer else 0), c4, act="lrelu")
         self.fc1 = FullyConnected(c4, 1)
+        if transformer:
+            self.latents = nn.Parameter(torch.randn(components_num, latent_dim))
 
     def forward(self, img):
         x = self.fromrgb(img.contiguous(memory_format=torch.channels_last))
+        y, composite = None, False
+        if self.transformer:
+            y = self.latents[None].expand(img.shape[0], -1, -1).contiguous()
+            composite = torch.is_grad_enabled() and img.requires_grad and any(p.requires_grad for p in self.parameters())
         for blk in self.blocks:
-            x = blk(x)
+            x, y = blk(x, y, composite)
         B, C, H, W = x.shape                                            # minibatch standard deviation, one feature map
         G = min(self.mbstd_group, B)
         while B % G:
             G -= 1
-        y = x.reshape(G, B // G, C, H, W)
-        y = (y - y.mean(dim=0, keepdim=True)).square().mean(dim=0).add(1e-8).sqrt().mean(dim=[1, 2, 3])
-        y = y.reshape(1, B // G, 1, 1).expand(G, -1, H, W).reshape(B, 1, H, W)
-        x = self.conv4(torch.cat([x, y], dim=1))
-        return self.fc1(self.fc0(x.reshape(B, -1))).reshape(B)
+        s = x.reshape(G, B // G, C, H, W)
+        s = (s - s.mean(dim=0, keepdim=True)).square().mean(dim=0).add(1e-8).sqrt().mean(dim=[1, 2, 3])
+        s = s.reshape(1, B // G, 1, 1).expand(G, -1, H, W).reshape(B, 1, H, W)
+        x = self.conv4(torch.cat([x, s], dim=1)).reshape(B, -1)
+        if y is not None:
+            x = torch.cat([x, y.reshape(B, -1)], dim=1)
+        return self.fc1(self.fc0(x)).reshape(B)
 
 
 @dataclass
