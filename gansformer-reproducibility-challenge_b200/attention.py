@@ -369,6 +369,9 @@ class BipartiteAttention(nn.Module):
     # with or without dropout, and the centroids output is differentiable.  That backward has no derivative of its own, so it
     # raises when called with grad mode on (create_graph).  The discriminator sets it; generator layers keep their routes.
     kernel_backward = False
+    # Opt-in on top of kernel_backward: that backward, run with grad mode on, builds a graph the double-backward kernels
+    # differentiate (autograd._duplex_kernel_backward_graph) instead of raising.  Discriminator(r1_kernels=True) sets it.
+    kernel_double_backward = False
 
     def __init__(self, dim: int, latent_dim: int, components_num: int, pos_dim: Optional[int] = None,
                  num_heads: int = 1, integration: str = "mul", norm: Optional[str] = "layer", kmeans: bool = False,

@@ -7,7 +7,10 @@ batched GEMMs for the reductions over tokens, and torch autograd through the tin
 dropout: the same stage-T kernel with keys from the centroids, plus the pass-A kernels ``gf_attn_centroid_stats`` /
 ``gf_attn_centroid_bwd`` and autograd through the pass-A tables (``centroid_tables``), see ``_duplex_kernel_backward``.
 A duplex module with ``kernel_backward = True`` (the discriminator's layers) takes that route without dropout too, and its
-centroids output is differentiable (the cotangent joins the same autograd call).
+centroids output is differentiable (the cotangent joins the same autograd call).  With ``kernel_double_backward = True`` as well,
+that backward run with create_graph=True (the discriminator's R1 penalty) builds a graph of three Functions, each differentiable once more,
+whose own backward are the double-backward kernels ``gf_attn_simplex_bwd_vjp`` / ``gf_attn_centroid_bwd_vjp``, see
+``_duplex_kernel_backward_graph``.
 Everything else (duplex without dropout, instance / batch norm, multi-head, CPU tensors): PyTorch autograd through a
 recomputation of the direct-form algebra with torch ops (``composite_forward``).
 """
@@ -17,6 +20,7 @@ import contextlib
 import math
 
 import torch
+from torch.autograd.function import once_differentiable
 
 
 def _e(w):
@@ -204,8 +208,14 @@ class _FusedAttention(torch.autograd.Function):
         x, y, *params = ctx.saved_tensors
         if m.kernel_backward and m.duplex:
             if torch.is_grad_enabled():
-                raise RuntimeError("the duplex kernel backward has no derivative of its own (create_graph=True): run the layer "
-                                   "through composite_forward for higher-order gradients, as Discriminator does in the R1 pass")
+                if not m.kernel_double_backward:
+                    raise RuntimeError("the duplex kernel backward has no derivative of its own (create_graph=True): run the layer "
+                                       "through composite_forward for higher-order gradients, as Discriminator does in the R1 pass")
+                if ctx.dropout or ctx.centroids is not None or not _duplex_kernel_backward_ok(m, x):
+                    raise NotImplementedError("kernel_double_backward serves single-head duplex layers with kmeans_iters == 1, "
+                                              "norm layer / none, computed centroids, no attention dropout, float32 CUDA tensors")
+                return (None, None, None, None, *_duplex_kernel_backward_graph(m, ctx.names, x, y, params, g_out,
+                                                                               g_cen if ctx.cen_grad else None))
             if not _duplex_kernel_backward_ok(m, x):
                 raise NotImplementedError("kernel_backward serves single-head duplex layers with kmeans_iters == 1, norm layer / none, "
                                           "float32 CUDA tensors")
@@ -299,6 +309,180 @@ def _duplex_kernel_backward(m, names, x, y, params, g_out, dropout=None, centroi
         i = 1 + names.index("bk2")     # constant over the tokens, bk2 cancels in pass A's softmax: its gradient is exactly 0
         g1[i] = torch.zeros_like(params[i - 1])
     return (dX, *g1)
+
+
+def _alias(t):
+    """A differentiable alias of t: autograd.grad with respect to it does not follow the other paths that reach t."""
+    return t.view_as(t) if t.requires_grad else t.detach().requires_grad_(True)
+
+
+def _sum_grads(a, b):
+    return [u if v is None else (v if u is None else u + v) for u, v in zip(a, b)]
+
+
+@_fp32_matmul()
+def _duplex_kernel_backward_graph(m, names, x, y, params, g_out, g_cen=None):
+    """``_duplex_kernel_backward`` (no dropout, computed centroids) as a graph that can be differentiated once more, for a backward
+    run with create_graph=True (the R1 penalty).  The tables are built from the graph-connected y and parameters; the per-token
+    work runs in three once-differentiable Functions whose backward are the double-backward kernels:
+      _CentroidStats    X, pass-A tables -> Xbar, lse           (backward: gf_attn_centroid_bwd with r - lse cotangent)
+      _StageTBackward   X, dOut, tables -> dX, dKp, dVt, dRt, dCt (backward: gf_attn_simplex_bwd_vjp)
+      _CentroidBackward X, pass-A tables, lse, dXbar, r, dX -> dX + pass A, dM, dRt2, dCt2 (backward: gf_attn_centroid_bwd_vjp)
+    y and the parameters enter the stage-T tables and the pass-A tables through separate aliases, so that the gradient of the
+    stage-T tables stops at Xbar, as in the first-order route, while Xbar stays connected to X and the pass-A tables.  Saved for
+    the second pass: X, dOut and the per-image tables."""
+    B, H, W, C = x.shape
+    k, D = y.shape[1], y.shape[2]
+    xc = x.contiguous()
+    y1, y2 = _alias(y), _alias(y)
+    p1, p2 = [_alias(p) for p in params], [_alias(p) for p in params]
+    d1, d2 = dict(zip(names, p1)), dict(zip(names, p2))
+    cen_tabs = centroid_tables(y2, d2, H, W, C, m.use_pos)
+    xbar, lse = _CentroidStats.apply(m, k, D, xc, *cen_tabs)
+    if not xbar.requires_grad:
+        xbar.requires_grad_(True)
+    cen = xbar @ _e(d1["wv2"]) + d1["bv2"]
+    Kp, Vt, Rt, Ct, _ = folded_tables(y1, d1, H=H, W=W, C=C, integration=m.integration, use_pos=m.use_pos, centroids=cen,
+                                      img2ltnt=m.img2ltnt)
+    dX, *grads = _StageTBackward.apply(m, k, D, xc, g_out, Kp, Vt, Rt, Ct)
+    outs = [Kp, Vt, Rt, Ct]
+    if g_cen is not None:
+        outs, grads = outs + [cen], grads + [g_cen]
+    g1 = list(torch.autograd.grad(outs, [y1, *p1, xbar], grads, allow_unused=True, create_graph=True))
+    dxbar = g1.pop()
+    r = (dxbar * xbar).sum(dim=2)
+    dX, *g_tabs = _CentroidBackward.apply(m, k, D, xc, *cen_tabs, lse, dxbar, r, dX)
+    g2 = torch.autograd.grad(list(cen_tabs), [y2, *p2], g_tabs, allow_unused=True, create_graph=True)
+    g = _sum_grads(g1, g2)
+    i = 1 + names.index("bk2")         # constant over the tokens, bk2 cancels in pass A's softmax: its gradient is exactly 0
+    g[i] = torch.zeros_like(params[i - 1])
+    return (dX, *g)
+
+
+def _differentiable_twice(backward):
+    """once_differentiable, and refusing a third derivative at once: the error node once_differentiable leaves behind is not
+    visited by autograd.grad(..., inputs=...) when the inputs are reached by other paths, which would drop terms silently."""
+    inner = once_differentiable(backward)
+
+    def wrapper(ctx, *grads):
+        if torch.is_grad_enabled() and any(isinstance(g, torch.Tensor) and g.requires_grad for g in grads):
+            raise RuntimeError("the attention double-backward kernels have no derivative of their own: a third derivative "
+                               "(create_graph=True through the R1 penalty's backward) is not supported")
+        return inner(ctx, *grads)
+    return wrapper
+
+
+def _zeros_if_none(g, like):
+    return torch.zeros_like(like) if g is None else g.contiguous()
+
+
+class _StageTBackward(torch.autograd.Function):
+    """The stage-T backward with its token reductions, (X, dOut, Kp, Vt, Rt, Ct) -> (dX, dKp, dVt, dRt, dCt), without dropout.
+    Forward: gf_attn_simplex_bwd_ex and the reductions.  Backward: gf_attn_simplex_bwd_vjp and the reductions of its per-token
+    cotangents, Kp: Sg^T X + dS^T U, Vt: Ctlg^T P + dCtl^T dPg, Rt / Ct: sums of Sg."""
+
+    @staticmethod
+    def forward(ctx, m, k, D, x, g_out, Kp, Vt, Rt, Ct):
+        gc = g_out.contiguous()
+        dX, _, grads = _stage_t_backward(m, x, k, D, gc, (Kp, Vt, Rt, Ct, None), None)
+        ctx.m, ctx.k, ctx.D = m, k, D
+        ctx.save_for_backward(x, gc, Kp, Vt, Rt, Ct)
+        return (dX, *grads)
+
+    @staticmethod
+    @_differentiable_twice
+    @_fp32_matmul()
+    def backward(ctx, gdX, gKp, gVt, gRt, gCt):
+        import ctypes
+        from . import _lib
+        x, go, Kp, Vt, Rt, Ct = ctx.saved_tensors
+        m = ctx.m
+        B, H, W, C = x.shape
+        n, KP, Cout = H * W, Kp.shape[1], Vt.shape[1]
+        U = _zeros_if_none(gdX, x)
+        cots = [_zeros_if_none(g, t) for g, t in ((gKp, Kp), (gVt, Vt), (gRt, Rt), (gCt, Ct))]
+        Xg, dOg = torch.empty_like(x), torch.empty_like(x)
+        Sg, dPg, dS, P = (torch.empty((B, n, KP), dtype=torch.float32, device=x.device) for _ in range(4))
+        Ctlg, dCtl = (torch.empty((B, n, Cout), dtype=torch.float32, device=x.device) for _ in range(2))
+        desc = _lib.make_desc(B, H, W, C, ctx.k, ctx.D, heads=1, norm=m.norm, integration=m.integration,
+                              pos_dim=m.pos_dim if m.use_pos else 0, duplex=False, flags=0)
+        with torch.cuda.device(x.device):
+            _lib.check(_lib.load().gf_attn_simplex_bwd_vjp(
+                ctypes.byref(desc), *(t.data_ptr() for t in (x, go, Kp, Vt, Rt, Ct, U, *cots, Xg, dOg, Sg, dPg, Ctlg, dS, P, dCtl)),
+                ctypes.c_void_p(torch.cuda.current_stream(x.device).cuda_stream)), "gf_attn_simplex_bwd_vjp")
+        X2, U2 = x.reshape(B, n, C), U.reshape(B, n, C)
+        gKp_ = torch.bmm(Sg.transpose(1, 2), X2) + torch.bmm(dS.transpose(1, 2), U2)
+        gVt_ = torch.bmm(Ctlg.transpose(1, 2), P) + torch.bmm(dCtl.transpose(1, 2), dPg)
+        Sg4 = Sg.reshape(B, H, W, KP)
+        return None, None, None, Xg, dOg, gKp_, gVt_, Sg4.sum(dim=2), Sg4.sum(dim=1)
+
+
+class _CentroidStats(torch.autograd.Function):
+    """Pass A's statistics, (X, M, Rt2, Ct2) -> (Xbar, lse) (gf_attn_centroid_stats).  Backward: with cotangents dXbar and lseg,
+    d lse_j / d s[t,j] = A[t,j], so it is gf_attn_centroid_bwd with r = dXbar . Xbar - lseg and dX starting from zero."""
+
+    @staticmethod
+    def forward(ctx, m, k, D, x, Mt, Rt2, Ct2):
+        xbar, lse = _centroid_stats(m, x, k, D, Mt, Rt2, Ct2)
+        ctx.m, ctx.k, ctx.D = m, k, D
+        ctx.save_for_backward(x, Mt, Rt2, Ct2, xbar, lse)
+        return xbar, lse
+
+    @staticmethod
+    @_differentiable_twice
+    @_fp32_matmul()
+    def backward(ctx, gxbar, glse):
+        x, Mt, Rt2, Ct2, xbar, lse = ctx.saved_tensors
+        B, H, W, C = x.shape
+        gxbar = _zeros_if_none(gxbar, xbar)
+        r = (gxbar * xbar).sum(dim=2)
+        if glse is not None:
+            r = r - glse[:, :ctx.k]
+        dX = torch.zeros_like(x)
+        dS = _centroid_bwd(ctx.m, x, ctx.k, ctx.D, Mt, Rt2, Ct2, lse, gxbar, r.contiguous(), dX)
+        dS4 = dS.reshape(B, H, W, dS.shape[2])
+        return None, None, None, dX, torch.bmm(dS.transpose(1, 2), x.reshape(B, H * W, C)), dS4.sum(dim=2), dS4.sum(dim=1)
+
+
+class _CentroidBackward(torch.autograd.Function):
+    """The pass-A backward with its token reductions, (X, M, Rt2, Ct2, lse, dXbar, r, dX_in) -> (dX_out, dM, dRt2, dCt2).
+    Forward: gf_attn_centroid_bwd into a copy of dX_in (never into a tensor autograd tracks) and the reductions.  Backward:
+    gf_attn_centroid_bwd_vjp and the reductions dXbar: A^T U + Gg^T X, M: Sg^T X + dS^T U, r: -sum_t Gg, lse: -sum_t Sg."""
+
+    @staticmethod
+    def forward(ctx, m, k, D, x, Mt, Rt2, Ct2, lse, dxbar, r, dX_in):
+        B, H, W, C = x.shape
+        dxbar, r = dxbar.contiguous(), r.contiguous()
+        dX = dX_in.contiguous().clone()
+        dS = _centroid_bwd(m, x, k, D, Mt, Rt2, Ct2, lse, dxbar, r, dX)
+        ctx.m, ctx.k, ctx.D = m, k, D
+        ctx.save_for_backward(x, Mt, Rt2, Ct2, lse, dxbar, r)
+        dS4 = dS.reshape(B, H, W, dS.shape[2])
+        return dX, torch.bmm(dS.transpose(1, 2), x.reshape(B, H * W, C)), dS4.sum(dim=2), dS4.sum(dim=1)
+
+    @staticmethod
+    @_differentiable_twice
+    @_fp32_matmul()
+    def backward(ctx, gdX, gM, gRt2, gCt2):
+        import ctypes
+        from . import _lib
+        x, Mt, Rt2, Ct2, lse, dxbar, r = ctx.saved_tensors
+        B, H, W, C = x.shape
+        n, KP, k = H * W, Mt.shape[1], ctx.k
+        U = _zeros_if_none(gdX, x)
+        cots = [_zeros_if_none(g, t) for g, t in ((gM, Mt), (gRt2, Rt2), (gCt2, Ct2))]
+        Xg = torch.empty_like(x)
+        Sg, Gg, A, dS = (torch.empty((B, n, KP), dtype=torch.float32, device=x.device) for _ in range(4))
+        desc = _duplex_desc(ctx.m, x, k, ctx.D)
+        with torch.cuda.device(x.device):
+            _lib.check(_lib.load().gf_attn_centroid_bwd_vjp(
+                ctypes.byref(desc), *(t.data_ptr() for t in (x, Mt, Rt2, Ct2, lse, dxbar, r, U, *cots, Xg, Sg, Gg, A, dS)),
+                ctypes.c_void_p(torch.cuda.current_stream(x.device).cuda_stream)), "gf_attn_centroid_bwd_vjp")
+        X2, U2 = x.reshape(B, n, C), U.reshape(B, n, C)
+        gM_ = torch.bmm(Sg.transpose(1, 2), X2) + torch.bmm(dS.transpose(1, 2), U2)
+        gxbar = (torch.bmm(A.transpose(1, 2), U2) + torch.bmm(Gg.transpose(1, 2), X2))[:, :k]
+        Sg4 = Sg.reshape(B, H, W, KP)
+        return (None, None, None, Xg, gM_, Sg4.sum(dim=2), Sg4.sum(dim=1), -Sg.sum(dim=1), gxbar, -Gg.sum(dim=1)[:, :k], U)
 
 
 def _duplex_desc(m, x, k, D):

@@ -12,8 +12,9 @@ simplex layers, the same kernel plus the pass-A backward kernels for duplex laye
 composite for the rest (duplex layers without dropout, instance / batch norm, multi-head).  The discriminator is PyTorch plumbing
 (cuDNN convolutions, the native FIR); with ``transformer=True`` it also has the paper's bipartite attention: duplex layers
 aggregating the image into learned latents that are carried from layer to layer and concatenated to the final features.  Those
-layers run the CUDA forward and the duplex kernel backward (``BipartiteAttention.kernel_backward``), and the torch composite in
-the R1 pass, which needs their second derivative.  Path-length regularisation and augmentation are out of scope.
+layers run the CUDA forward and the duplex kernel backward (``BipartiteAttention.kernel_backward``), and by default the torch
+composite in the R1 pass, which needs their second derivative; with ``Discriminator(r1_kernels=True)`` the R1 pass runs them on the
+kernels too, differentiated twice through the double-backward kernels (``BipartiteAttention.kernel_double_backward``).  Path-length regularisation and augmentation are out of scope.
 """
 from __future__ import annotations
 
@@ -74,6 +75,7 @@ def _d_attention(C: int, resolution: int, att: dict) -> BipartiteAttention:
     m = BipartiteAttention(C, D, k, integration=att["integration"], norm=att["norm"], kmeans=True, kmeans_iters=1, img2ltnt=True,
                            use_pos=att["use_pos"], exact_fp32=att["exact_fp32"])
     m.kernel_backward = True          # no generator gradients to preserve: the duplex kernel backward from the start
+    m.kernel_double_backward = att.get("r1_kernels", False)
     return m
 
 
@@ -81,9 +83,10 @@ def _attend(att: BipartiteAttention, x: torch.Tensor, y: torch.Tensor, composite
     """x [B,C,H,W] (channels-last memory), Y [B,k,D] -> (attended x, the Y carried to the next attention layer).
 
     The carry is the layer's own value input, Y <- LN(Y) (1 + Cen Wi2l_e + bi2l), with Cen the layer's centroids.  ``composite``
-    runs the layer as torch ops (``composite_forward``), which can be differentiated twice (R1)."""
+    (the R1 pass) runs the layer as torch ops (``composite_forward``), which can be differentiated twice, unless the layer's
+    kernel backward has a derivative of its own (``kernel_double_backward``)."""
     xt = x.permute(0, 2, 3, 1).contiguous()                            # [B,H,W,C]: a view of a channels-last activation
-    if composite:
+    if composite and not att.kernel_double_backward:
         out, cen = composite_forward(xt, y, att.param_dict(), integration=att.integration, norm=att.norm, duplex=True,
                                      use_pos=att.use_pos, img2ltnt=True)
     else:
@@ -122,18 +125,21 @@ class Discriminator(nn.Module):
     ``latents`` [k, D] are broadcast to Y [B,k,D]; every block whose input resolution lies in [d_start_res, d_end_res] runs a
     duplex layer (one k-means iteration, g_img2ltnt) after conv0 and after conv1; Y is carried from layer to layer and fc0 takes
     [flatten(x), flatten(Y)].  The layers run the CUDA forward and the duplex kernel backward; when the image and the parameters
-    both require grad under grad mode (the R1 pass), they run ``composite_forward`` instead, which has a second derivative."""
+    both require grad under grad mode (the R1 pass), they run ``composite_forward`` instead, which has a second derivative.
+    ``r1_kernels=True`` keeps the R1 pass on the kernels: the kernel backward, run with create_graph=True, is differentiated by
+    the double-backward kernels, and only each layer's input and incoming gradient are kept for the second pass instead of the
+    composite's [B,n,C] projections.  The R1 gradients then differ from the default route by round-off."""
 
     def __init__(self, resolution: int = 256, fmap_base: int = 16384, fmap_max: int = 512, mbstd_group: int = 4,
                  transformer: bool = False, components_num: int = 16, latent_dim: int = 32, d_start_res: int = 8,
                  d_end_res: Optional[int] = None, integration: str = "mul", norm: Optional[str] = "layer", use_pos: bool = True,
-                 exact_fp32: bool = False):
+                 exact_fp32: bool = False, r1_kernels: bool = False):
         super().__init__()
         self.resolution, self.mbstd_group, self.transformer = resolution, mbstd_group, transformer
         log2 = int(math.log2(resolution))
         d_end_res = resolution if d_end_res is None else d_end_res
         att = dict(components_num=components_num, latent_dim=latent_dim, integration=integration, norm=norm, use_pos=use_pos,
-                   exact_fp32=exact_fp32) if transformer else None
+                   exact_fp32=exact_fp32, r1_kernels=r1_kernels) if transformer else None
         self.fromrgb = EqConv2d(3, nf(resolution, fmap_base, fmap_max), 1)
         self.blocks = nn.ModuleList([DiscriminatorBlock(nf(2 ** i, fmap_base, fmap_max), nf(2 ** (i - 1), fmap_base, fmap_max), 2 ** i,
                                                         att if d_start_res <= 2 ** i <= d_end_res else None)

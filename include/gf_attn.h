@@ -227,6 +227,30 @@ int gf_attn_centroid_stats(const gf_attn_desc* desc, const float* X, const float
 int gf_attn_centroid_bwd(const gf_attn_desc* desc, const float* X, const float* M, const float* Rt2, const float* Ct2,
                          const float* lse, const float* dXbar, const float* r, float* dX, float* dS, void* stream);
 
+/* The backward of gf_attn_centroid_stats itself, with cotangents dXbar of Xbar and lseg of lse, is gf_attn_centroid_bwd with
+ * r_j = dXbar_j . Xbar_j - lseg_j and dX preloaded with zeros: d lse_j / d s[t,j] = A[t,j], so lseg only shifts r. */
+
+/* Double backward (the discriminator's R1 penalty).  Both entries are the vector-Jacobian products of a first-order backward
+ * taken together with its token reductions; fp32, one thread per token, no atomics, no workspace, the caller's stream.
+ *
+ * gf_attn_simplex_bwd_vjp: the VJP of (X, dOut, Kp, Vt, Rt, Ct) -> (dX, dS^T X, dCtl^T P, sum_w dS, sum_h dS) of
+ * gf_attn_simplex_bwd (no dropout; simplex descriptor, norm layer / none, one head).  Cotangents in: U [B,n,C] of dX, Kpg
+ * [B,KP,C], Vtg [B,Cout,KP], Rtg [B,H,KP], Ctg [B,W,KP] of the reductions.  Out: Xg, dOutg [B,n,C] (the cotangents of X and
+ * dOut), Sg [B,n,KP] (of the logits), dPg [B,n,KP] (of dp = Vt^T dCtl), Ctlg [B,n,Cout] (of the control signal), and the
+ * first-order dS, P, dCtl.  The caller reduces  Kp: Sg^T X + dS^T U,  Vt: Ctlg^T P + dCtl^T dPg,  Rt / Ct: sums of Sg. */
+int gf_attn_simplex_bwd_vjp(const gf_attn_desc* desc, const float* X, const float* dOut, const float* Kp, const float* Vt,
+                            const float* Rt, const float* Ct, const float* U, const float* Kpg, const float* Vtg, const float* Rtg,
+                            const float* Ctg, float* Xg, float* dOutg, float* Sg, float* dPg, float* Ctlg, float* dS, float* P,
+                            float* dCtl, void* stream);
+
+/* gf_attn_centroid_bwd_vjp: the VJP of (X, M, Rt2, Ct2, lse, dXbar, r, dX_in) -> (dX_out, dS^T X, sum_w dS, sum_h dS) of
+ * gf_attn_centroid_bwd.  Cotangents in: U [B,n,C] of dX_out, Mg [B,KP,C], Rt2g [B,H,KP], Ct2g [B,W,KP].  Out: Xg [B,n,C] (the
+ * cotangent of X), Sg [B,n,KP] (of the logits), Gg [B,n,KP] (of g = x.dXbar), A [B,n,KP] and dS [B,n,KP].  The caller reduces
+ *   dXbar: A^T U + Gg^T X,  M: Sg^T X + dS^T U,  r: -sum_t Gg,  lse: -sum_t Sg,  Rt2 / Ct2: sums of Sg,  dX_in: U. */
+int gf_attn_centroid_bwd_vjp(const gf_attn_desc* desc, const float* X, const float* M, const float* Rt2, const float* Ct2,
+                             const float* lse, const float* dXbar, const float* r, const float* U, const float* Mg,
+                             const float* Rt2g, const float* Ct2g, float* Xg, float* Sg, float* Gg, float* A, float* dS, void* stream);
+
 /* The dropout multipliers themselves, mask [B, H*W, KP] (0 or 1 / (1 - att_dp); KP = 16 for k <= 16, else 32; columns of a
  * multi-head layer: head * seg + j): what the fused kernels apply.  For the composite training path and for tests. */
 int gf_attn_dropout_mask(const gf_attn_desc* desc, float att_dp, uint32_t dp_salt, const unsigned long long* dp_state, float* mask, void* stream);

@@ -1,7 +1,8 @@
 """The discriminator's attention at 256x256, batch 32: discriminator forward + backward (the D step's route: parameters require grad,
 the image does not), the R1 pass (image and parameters require grad: the attention layers run the torch composite, double
-backward), and Trainer.step_graphed images/s with the 256x256 K = 16 generator of bench.py's train_step, for the plain
-discriminator and for transformer=True with d_end_res in {32, 64, 256} (K = 16, D = 32).  CUDA events, mean over --reps calls
+backward, or with r1_kernels=True the kernel backward differentiated by the double-backward kernels), and Trainer.step_graphed
+images/s with the 256x256 K = 16 generator of bench.py's train_step, for the plain discriminator and for transformer=True with
+d_end_res in {32, 64, 256} (K = 16, D = 32), each on both R1 routes, one after the other.  CUDA events, mean over --reps calls
 after --warmup; peak = the allocator's peak above what was allocated before the calls.  When the R1 graph does not fit, the
 plain steps are timed with a trainer without the penalty (r1_gamma = 0).  One JSON line per configuration.
 
@@ -24,8 +25,11 @@ import gansformer_b200 as gf  # noqa: E402
 tr = import_module("gansformer-reproducibility-challenge_b200.training")
 
 RES, B, K = 256, 32, 16
-CONFIGS = [("plain", dict())] + [(f"transformer d_end_res={r}", dict(transformer=True, components_num=K, latent_dim=32, d_end_res=r))
-                                 for r in (32, 64, 256)]
+# each transformer configuration twice in a row, the R1 pass on the double-backward kernels and on the composite (the default):
+# the kernels first, because a graph capture that runs out of memory (the composite at d_end_res=256) keeps memory in its pool
+CONFIGS = [("plain", dict())] + [(f"transformer d_end_res={r}{' r1_kernels' if rk else ''}",
+                                  dict(transformer=True, components_num=K, latent_dim=32, d_end_res=r, r1_kernels=rk))
+                                 for r in (32, 64, 256) for rk in (True, False)]
 
 
 def timed(fn, reps, warmup):
