@@ -11,6 +11,9 @@ centroids output is differentiable (the cotangent joins the same autograd call).
 that backward run with create_graph=True (the discriminator's R1 penalty) builds a graph of three Functions, each differentiable once more,
 whose own backward are the double-backward kernels ``gf_attn_simplex_bwd_vjp`` / ``gf_attn_centroid_bwd_vjp``, see
 ``_duplex_kernel_backward_graph``.
+A generator layer's backward run with create_graph=True (the path-length penalty) builds a graph on every route: the simplex kernel
+route through ``_simplex_kernel_backward_graph``, the duplex route with dropout through ``_duplex_kernel_backward_graph``, both
+with the forward's dropout mask in ``gf_attn_simplex_bwd_vjp_ex``, and the composite route through autograd with create_graph=True.
 Everything else (duplex without dropout, instance / batch norm, multi-head, CPU tensors): PyTorch autograd through a
 recomputation of the direct-form algebra with torch ops (``composite_forward``).
 """
@@ -221,13 +224,30 @@ class _FusedAttention(torch.autograd.Function):
                                           "float32 CUDA tensors")
             return (None, None, None, None, *_duplex_kernel_backward(m, ctx.names, x, y, params, g_out, ctx.dropout, ctx.centroids,
                                                                      g_cen if ctx.cen_grad else None))
+        # grad mode on: the backward runs with create_graph=True (the generator's path-length penalty) and must itself be
+        # differentiable; the first-order calls below are the same with it off
+        graph = torch.is_grad_enabled()
         if _kernel_backward_ok(m, x):
+            if graph:
+                return (None, None, None, None, *_simplex_kernel_backward_graph(m, ctx.names, x, y, params, g_out, ctx.dropout))
             return (None, None, None, None, *_kernel_backward(m, ctx.names, x, y, params, g_out, ctx.dropout))
         if ctx.dropout and _duplex_kernel_backward_ok(m, x):
+            if graph:
+                if ctx.centroids is not None:
+                    raise NotImplementedError("a duplex layer with attention dropout and given centroids has no second derivative "
+                                              "on the kernels")
+                return (None, None, None, None, *_duplex_kernel_backward_graph(m, ctx.names, x, y, params, g_out, dropout=ctx.dropout))
             return (None, None, None, None, *_duplex_kernel_backward(m, ctx.names, x, y, params, g_out, ctx.dropout, ctx.centroids))
         if ctx.dropout:
             raise NotImplementedError("attention dropout needs the backward kernels: single-head layers with norm layer / none, "
                                       "simplex or duplex with kmeans_iters == 1")
+        if graph:                          # composite route, differentiable again: autograd on the saved tensors themselves
+            xs, ys, ps = _alias(x), _alias(y), [_alias(p) for p in params]
+            out, _ = composite_forward(xs, ys, dict(zip(ctx.names, ps)), integration=m.integration, norm=m.norm,
+                                       duplex=m.duplex, use_pos=m.use_pos, centroids=ctx.centroids, kmeans_iters=m.kmeans_iters,
+                                       img2ltnt=m.img2ltnt, num_heads=m.num_heads)
+            grads = torch.autograd.grad(out, [xs, ys, *ps], g_out, allow_unused=True, create_graph=True)
+            return (None, None, None, None, *grads)
         with torch.enable_grad():
             xs = x.detach().requires_grad_(True)
             ys = y.detach().requires_grad_(True)
@@ -321,12 +341,30 @@ def _sum_grads(a, b):
 
 
 @_fp32_matmul()
-def _duplex_kernel_backward_graph(m, names, x, y, params, g_out, g_cen=None):
-    """``_duplex_kernel_backward`` (no dropout, computed centroids) as a graph that can be differentiated once more, for a backward
-    run with create_graph=True (the R1 penalty).  The tables are built from the graph-connected y and parameters; the per-token
-    work runs in three once-differentiable Functions whose backward are the double-backward kernels:
+def _simplex_kernel_backward_graph(m, names, x, y, params, g_out, dropout=None):
+    """``_kernel_backward`` as a graph that can be differentiated once more, for a backward run with create_graph=True (the
+    generator's path-length penalty): the tables (with cb under dropout) are built from the graph-connected y and parameters, the
+    per-token work is ``_StageTBackward`` (backward: gf_attn_simplex_bwd_vjp_ex, the same dropout mask), and autograd takes the
+    table gradients back through stages W and I with create_graph=True."""
+    B, H, W, C = x.shape
+    ys, ps = _alias(y), [_alias(p) for p in params]
+    Kp, Vt, Rt, Ct, cb = folded_tables(ys, dict(zip(names, ps)), H=H, W=W, C=C, integration=m.integration, use_pos=m.use_pos)
+    dX, *grads = _StageTBackward.apply(m, y.shape[1], y.shape[2], dropout or None, x.contiguous(), g_out, Kp, Vt, Rt, Ct,
+                                       cb if dropout else None)
+    outs = [Kp, Vt, Rt, Ct] + ([cb] if dropout else [])
+    g = torch.autograd.grad(outs, [ys, *ps], grads, allow_unused=True, create_graph=True)
+    return (dX, *g)
+
+
+@_fp32_matmul()
+def _duplex_kernel_backward_graph(m, names, x, y, params, g_out, g_cen=None, dropout=None):
+    """``_duplex_kernel_backward`` (computed centroids) as a graph that can be differentiated once more, for a backward run with
+    create_graph=True (the discriminator's R1 penalty, the generator's path-length penalty).  The tables are built from the
+    graph-connected y and parameters; the per-token work runs in three once-differentiable Functions whose backward are the
+    double-backward kernels:
       _CentroidStats    X, pass-A tables -> Xbar, lse           (backward: gf_attn_centroid_bwd with r - lse cotangent)
-      _StageTBackward   X, dOut, tables -> dX, dKp, dVt, dRt, dCt (backward: gf_attn_simplex_bwd_vjp)
+      _StageTBackward   X, dOut, tables (+ cb) -> dX, dKp, dVt, dRt, dCt (+ dcb) (backward: gf_attn_simplex_bwd_vjp_ex; with
+                        ``dropout``, the mask of the forward, which only stage T has)
       _CentroidBackward X, pass-A tables, lse, dXbar, r, dX -> dX + pass A, dM, dRt2, dCt2 (backward: gf_attn_centroid_bwd_vjp)
     y and the parameters enter the stage-T tables and the pass-A tables through separate aliases, so that the gradient of the
     stage-T tables stops at Xbar, as in the first-order route, while Xbar stays connected to X and the pass-A tables.  Saved for
@@ -342,10 +380,10 @@ def _duplex_kernel_backward_graph(m, names, x, y, params, g_out, g_cen=None):
     if not xbar.requires_grad:
         xbar.requires_grad_(True)
     cen = xbar @ _e(d1["wv2"]) + d1["bv2"]
-    Kp, Vt, Rt, Ct, _ = folded_tables(y1, d1, H=H, W=W, C=C, integration=m.integration, use_pos=m.use_pos, centroids=cen,
-                                      img2ltnt=m.img2ltnt)
-    dX, *grads = _StageTBackward.apply(m, k, D, xc, g_out, Kp, Vt, Rt, Ct)
-    outs = [Kp, Vt, Rt, Ct]
+    Kp, Vt, Rt, Ct, cb = folded_tables(y1, d1, H=H, W=W, C=C, integration=m.integration, use_pos=m.use_pos, centroids=cen,
+                                       img2ltnt=m.img2ltnt)
+    dX, *grads = _StageTBackward.apply(m, k, D, dropout or None, xc, g_out, Kp, Vt, Rt, Ct, cb if dropout else None)
+    outs = [Kp, Vt, Rt, Ct] + ([cb] if dropout else [])
     if g_cen is not None:
         outs, grads = outs + [cen], grads + [g_cen]
     g1 = list(torch.autograd.grad(outs, [y1, *p1, xbar], grads, allow_unused=True, create_graph=True))
@@ -377,26 +415,28 @@ def _zeros_if_none(g, like):
 
 
 class _StageTBackward(torch.autograd.Function):
-    """The stage-T backward with its token reductions, (X, dOut, Kp, Vt, Rt, Ct) -> (dX, dKp, dVt, dRt, dCt), without dropout.
-    Forward: gf_attn_simplex_bwd_ex and the reductions.  Backward: gf_attn_simplex_bwd_vjp and the reductions of its per-token
-    cotangents, Kp: Sg^T X + dS^T U, Vt: Ctlg^T P + dCtl^T dPg, Rt / Ct: sums of Sg."""
+    """The stage-T backward with its token reductions, (X, dOut, Kp, Vt, Rt, Ct) -> (dX, dKp, dVt, dRt, dCt); with attention
+    dropout (the forward's mask, regenerated) cb is one more table and dcb = sum_tokens (1 - sum q) dCtl one more output.
+    Forward: gf_attn_simplex_bwd_ex and the reductions.  Backward: gf_attn_simplex_bwd_vjp_ex (without dropout its att_dp = 0 form,
+    gf_attn_simplex_bwd_vjp) and the reductions of its per-token cotangents, Kp: Sg^T X + dS^T U, Vt: Ctlg^T P + dCtl^T dPg,
+    Rt / Ct: sums of Sg, cb: (1 - sum P) Ctlg - (sum dPg) dCtl."""
 
     @staticmethod
-    def forward(ctx, m, k, D, x, g_out, Kp, Vt, Rt, Ct):
+    def forward(ctx, m, k, D, dropout, x, g_out, Kp, Vt, Rt, Ct, cb):
         gc = g_out.contiguous()
-        dX, _, grads = _stage_t_backward(m, x, k, D, gc, (Kp, Vt, Rt, Ct, None), None)
-        ctx.m, ctx.k, ctx.D = m, k, D
-        ctx.save_for_backward(x, gc, Kp, Vt, Rt, Ct)
+        dX, _, grads = _stage_t_backward(m, x, k, D, gc, (Kp, Vt, Rt, Ct, cb), dropout)
+        ctx.m, ctx.k, ctx.D, ctx.dropout = m, k, D, dropout or {}
+        ctx.save_for_backward(x, gc, Kp, Vt, Rt, Ct, cb)
         return (dX, *grads)
 
     @staticmethod
     @_differentiable_twice
     @_fp32_matmul()
-    def backward(ctx, gdX, gKp, gVt, gRt, gCt):
+    def backward(ctx, gdX, gKp, gVt, gRt, gCt, *gcb):
         import ctypes
         from . import _lib
-        x, go, Kp, Vt, Rt, Ct = ctx.saved_tensors
-        m = ctx.m
+        x, go, Kp, Vt, Rt, Ct, cb = ctx.saved_tensors
+        m, dpo = ctx.m, ctx.dropout
         B, H, W, C = x.shape
         n, KP, Cout = H * W, Kp.shape[1], Vt.shape[1]
         U = _zeros_if_none(gdX, x)
@@ -406,15 +446,24 @@ class _StageTBackward(torch.autograd.Function):
         Ctlg, dCtl = (torch.empty((B, n, Cout), dtype=torch.float32, device=x.device) for _ in range(2))
         desc = _lib.make_desc(B, H, W, C, ctx.k, ctx.D, heads=1, norm=m.norm, integration=m.integration,
                               pos_dim=m.pos_dim if m.use_pos else 0, duplex=False, flags=0)
+        ptrs = [t.data_ptr() for t in (x, go, Kp, Vt, Rt, Ct, U, *cots, Xg, dOg, Sg, dPg, Ctlg, dS, P, dCtl)]
+        stream = ctypes.c_void_p(torch.cuda.current_stream(x.device).cuda_stream)
         with torch.cuda.device(x.device):
-            _lib.check(_lib.load().gf_attn_simplex_bwd_vjp(
-                ctypes.byref(desc), *(t.data_ptr() for t in (x, go, Kp, Vt, Rt, Ct, U, *cots, Xg, dOg, Sg, dPg, Ctlg, dS, P, dCtl)),
-                ctypes.c_void_p(torch.cuda.current_stream(x.device).cuda_stream)), "gf_attn_simplex_bwd_vjp")
+            if dpo:                              # the mask of the forward, regenerated from the same device state
+                cbg = _zeros_if_none(gcb[0], cb)
+                _lib.check(_lib.load().gf_attn_simplex_bwd_vjp_ex(
+                    ctypes.byref(desc), *ptrs, ctypes.c_float(dpo["att_dp"]), int(dpo.get("dp_salt", 0)), dpo["dp_state"].data_ptr(),
+                    cb.data_ptr(), cbg.data_ptr(), stream), "gf_attn_simplex_bwd_vjp_ex")
+            else:                                # the same kernel: the dropout-free entry is _ex at att_dp = 0
+                _lib.check(_lib.load().gf_attn_simplex_bwd_vjp(ctypes.byref(desc), *ptrs, stream), "gf_attn_simplex_bwd_vjp")
         X2, U2 = x.reshape(B, n, C), U.reshape(B, n, C)
         gKp_ = torch.bmm(Sg.transpose(1, 2), X2) + torch.bmm(dS.transpose(1, 2), U2)
         gVt_ = torch.bmm(Ctlg.transpose(1, 2), P) + torch.bmm(dCtl.transpose(1, 2), dPg)
         Sg4 = Sg.reshape(B, H, W, KP)
-        return None, None, None, Xg, dOg, gKp_, gVt_, Sg4.sum(dim=2), Sg4.sum(dim=1)
+        gcb_ = None
+        if dpo:                                  # cb: sum_tokens qdef gbar - F dCtl, qdef = 1 - sum q, F = sum_j fq_j
+            gcb_ = ((1.0 - P.sum(dim=2, keepdim=True)) * Ctlg - dPg.sum(dim=2, keepdim=True) * dCtl).sum(dim=(0, 1))
+        return None, None, None, None, Xg, dOg, gKp_, gVt_, Sg4.sum(dim=2), Sg4.sum(dim=1), gcb_
 
 
 class _CentroidStats(torch.autograd.Function):

@@ -390,11 +390,27 @@ __global__ void __launch_bounds__(BTM) centroid_bwd_kernel(const CenBwdParams P)
 // and the first-order dS, P, dCtl again.  The caller reduces Kpg = Sg^T X + dS^T U, Vtg = Ctlg^T P + dCtl^T dPg, Rtg / Ctg = sums of Sg.
 // Four sweeps over the 32-channel chunks; Xg doubles as the staging buffer of the cotangent of xn between sweeps 3 and 4 (each
 // element is stored and reloaded by the same thread).
+//
+// With attention dropout (gf_attn_simplex_bwd_vjp_ex, the generator's path-length penalty) the first-order backward is the one of
+// token_bwd_kernel: mask mk (0 or 1/(1-p)) from the same Philox draw, q = p mk, qdef = 1 - sum q, the gain of ctl
+// g = sum_j q_j Vt_j + qdef cb, dp = Vt^T dCtl, dcbt = dCtl.cb, dS = p (dpp - <p,dpp>) with dpp = mk (dp - dcbt), and P = q; the
+// function gains one reduction, dcb = sum_tokens qdef dCtl, whose cotangent cbg [Cout] comes in.  Reversed:
+//     f = p (e - <p,e>) as above, fq = mk f = cotangent of dp (dPg),  F = sum_j fq_j = -(cotangent of dcbt)
+//     cotangent of dCtl = Vt fq + Vg q - F cb + qdef cbg                (each half with its own rows of Vt, Vg, cb, cbg)
+//     cotangent of q    = Vg^T dCtl - dCtl.cbg + Vt_gain^T gbar - gbar.cb   (gbar = cotangent of the gain, as above)
+//     cotangent of p    = mk (cotangent of q) + e (dpp - <p,dpp>) - <p,e> dpp,   then Sg = p (pbar - <p,pbar>) as above
+//     cotangent of cb   = sum_tokens qdef gbar - F dCtl: the caller forms it from the outputs, (1 - sum P) Ctlg - (sum dPg) dCtl.
+// The LayerNorm terms are unchanged.  dS, the direct softmax term of pbar (staged in Sg) and q (in P) leave the registers after
+// sweep 2 and dS is reloaded for sweep 4, so the dropout variant holds as many [KP] arrays as the plain one; the mask is one word.
+// Without dropout the cotangent cbg is ignored: dcb is 0 for every input (sum p = 1).
 struct VjpParams {
   const float* X; const float* dOut; const float* Kp; const float* Vt; const float* Rt; const float* Ct;
   const float* U; const float* Kg; const float* Vg; const float* Rg; const float* Cg;
   float* Xg; float* dOutg; float* Sg; float* dPg; float* Ctlg; float* dS; float* P; float* dCtl;
   int n, H, W, C, Cout, norm, integration;
+  DropoutArgs dp;            // attention dropout of the forward call (thr = 0: off)
+  const float* cb;           // [Cout] bo (+1 on the gain half), read when dropout is on
+  const float* cbg;          // [Cout] cotangent of dcb, read when dropout is on
 };
 
 __device__ __forceinline__ void bwd_zero_chunk(float* __restrict__ dst, int t0, int n, int ld, int c0) {
@@ -426,7 +442,7 @@ __device__ __forceinline__ void vjp_load_cols(float (*dst)[KP], const float* __r
     reinterpret_cast<float4*>(&dst[0][0])[i] = __ldg(reinterpret_cast<const float4*>(src + (size_t)c0 * KP) + i);
 }
 
-template <int KP>
+template <int KP, bool DROP>
 __global__ void __launch_bounds__(BTM) token_bwd_vjp_kernel(const VjpParams P) {
   extern __shared__ __align__(16) uint8_t vsm_raw[];
   float (*xs)[BXS] = reinterpret_cast<float (*)[BXS]>(vsm_raw);
@@ -439,6 +455,7 @@ __global__ void __launch_bounds__(BTM) token_bwd_vjp_kernel(const VjpParams P) {
   float (*vb)[KP] = reinterpret_cast<float (*)[KP]>(tab + KP * BCH);                  // V^T bias chunk
   float (*wa)[KP] = reinterpret_cast<float (*)[KP]>(tab + 2 * KP * BCH);              // Vg gain chunk
   float (*wb)[KP] = reinterpret_cast<float (*)[KP]>(tab + 3 * KP * BCH);              // Vg bias chunk
+  float (*cbs)[BCH] = reinterpret_cast<float (*)[BCH]>(tab + 4 * KP * BCH);           // with dropout: cb, cbg chunks (gain, bias)
 
   const int b = blockIdx.y, t0 = blockIdx.x * BTM, tid = threadIdx.x, t = t0 + tid;
   const int n = P.n, C = P.C, Cout = P.Cout, integ = P.integration;
@@ -455,6 +472,7 @@ __global__ void __launch_bounds__(BTM) token_bwd_vjp_kernel(const VjpParams P) {
   float* dOgb = P.dOutg + (size_t)b * n * C;
   float* dCb = P.dCtl + (size_t)b * n * Cout;
   float* Cgb = P.Ctlg + (size_t)b * n * Cout;
+  const size_t orow = ((size_t)b * n + t) * KP;                   // this token's row of the [B,n,KP] outputs
 
   float s[KP], e[KP];
   {
@@ -502,6 +520,30 @@ __global__ void __launch_bounds__(BTM) token_bwd_vjp_kernel(const VjpParams P) {
   const float inv = 1.f / den;
 #pragma unroll
   for (int j = 0; j < KP; ++j) s[j] *= inv;                       // s = p from here on
+  // attention dropout: the mask of token_bwd_kernel as one bit per latent (multiplier 1/(1-p) where set), q = p mk
+  uint32_t keep = 0;
+  float q[KP], qdef = 0.f;                                       // q (without dropout: p itself, s is read instead)
+  if constexpr (DROP) {
+    const unsigned long long seed = P.dp.state[0], step = P.dp.state[1];
+#pragma unroll 1                                                 // unrolled, the Philox rounds push s and e out of the registers
+    for (int g4 = 0; g4 < KP / 4; ++g4) {
+      float m4[4];
+      dropout_mult4(P.dp, seed, step, (uint32_t)((size_t)b * n + (valid ? t : 0)), g4, m4);
+#pragma unroll
+      for (int i = 0; i < 4; ++i) keep |= (m4[i] != 0.f ? 1u : 0u) << (g4 * 4 + i);
+    }
+    float qs = 0.f;
+#pragma unroll
+    for (int j = 0; j < KP; ++j) { q[j] = s[j] * (((keep >> j) & 1u) ? P.dp.scale : 0.f); qs += q[j]; }
+    qdef = 1.f - qs;
+  }
+  if constexpr (DROP) {                                          // e is not read in sweep 2: parked in Sg (same thread) meanwhile
+    if (valid) {
+#pragma unroll
+      for (int j4 = 0; j4 < KP; j4 += 4)
+        *reinterpret_cast<float4*>(P.Sg + orow + j4) = make_float4(e[j4], e[j4 + 1], e[j4 + 2], e[j4 + 3]);
+    }
+  }
   float mean = 0.f, rstd = 1.f;
   if (ln) {
     const float md = sum * invC;
@@ -510,11 +552,12 @@ __global__ void __launch_bounds__(BTM) token_bwd_vjp_kernel(const VjpParams P) {
     rstd = rsqrtf(var + 1e-8f);
   }
 
-  // ---- sweep 2: dCtl (stored), dp, the LayerNorm-backward sums, pbar = Vg^T dCtl, and the sums of U against 1, xn and dxn
+  // ---- sweep 2: dCtl (stored), dp, the LayerNorm-backward sums, pbar = Vg^T dCtl (with dropout: the cotangent of q, from the
+  //      reduction dVt = dCtl^T q), the sums of U against 1, xn and dxn; with dropout also dCtl.cb and dCtl.cbg
   float dp[KP], pb[KP];
 #pragma unroll
   for (int j = 0; j < KP; ++j) { dp[j] = 0.f; pb[j] = 0.f; }
-  float a1 = 0.f, a2 = 0.f, su = 0.f, sux = 0.f, sud = 0.f;
+  float a1 = 0.f, a2 = 0.f, su = 0.f, sux = 0.f, sud = 0.f, dcbt = 0.f, dcg = 0.f;
   for (int c0 = 0; c0 < C; c0 += BCH) {
     __syncthreads();
     bwd_load_chunk(xs, Xb, t0, n, C, c0);
@@ -523,6 +566,12 @@ __global__ void __launch_bounds__(BTM) token_bwd_vjp_kernel(const VjpParams P) {
     vjp_load_cols<KP>(va, Vtb, c0);
     vjp_load_cols<KP>(wa, Vgb, c0);
     if (both) { vjp_load_cols<KP>(vb, Vtb, C + c0); vjp_load_cols<KP>(wb, Vgb, C + c0); }
+    if constexpr (DROP) {
+      if (tid < 4 * BCH) {                                       // rows: cb gain, cb bias, cbg gain, cbg bias
+        const int r = tid / BCH, c = tid % BCH;
+        cbs[r][c] = (r & 1) && !both ? 0.f : __ldg((r < 2 ? P.cb : P.cbg) + ((r & 1) ? C : 0) + c0 + c);
+      }
+    }
     __syncthreads();
     if (both) bwd_store_chunk(dCb, gs, t0, n, Cout, C + c0);      // bias half of dCtl = dOut (before gs is reused)
     __syncthreads();
@@ -535,8 +584,13 @@ __global__ void __launch_bounds__(BTM) token_bwd_vjp_kernel(const VjpParams P) {
       else {
         float g = 0.f;
 #pragma unroll
-        for (int j = 0; j < KP; ++j) g = fmaf(s[j], va[cc][j], g);
+        for (int j = 0; j < KP; ++j) g = fmaf(DROP ? q[j] : s[j], va[cc][j], g);
+        if constexpr (DROP) g = fmaf(qdef, cbs[0][cc], g);
         dxn = go * g; dc = go * xn;
+      }
+      if constexpr (DROP) {
+        dcbt = fmaf(dc, cbs[0][cc], dcbt); dcg = fmaf(dc, cbs[2][cc], dcg);
+        if (both) { dcbt = fmaf(go, cbs[1][cc], dcbt); dcg = fmaf(go, cbs[3][cc], dcg); }
       }
       a1 += dxn; a2 = fmaf(dxn, xn, a2);
       su += u; sux = fmaf(u, xn, sux); sud = fmaf(u, dxn, sud);
@@ -552,31 +606,68 @@ __global__ void __launch_bounds__(BTM) token_bwd_vjp_kernel(const VjpParams P) {
     bwd_store_chunk(dCb, gs, t0, n, Cout, c0);                    // gain half (or the only half) of dCtl
   }
   // ---- the softmax backward and its reverse: dS (kept in dp), f = cotangent of dp (kept in e), pbar += e (dp - pd) - pe dp
-  float pd = 0.f, pe = 0.f;
+  float fsum = 0.f;                                              // with dropout: F = sum_j fq_j
+  if constexpr (!DROP) {
+    float pd = 0.f, pe = 0.f;
 #pragma unroll
-  for (int j = 0; j < KP; ++j) { pd = fmaf(s[j], dp[j], pd); pe = fmaf(s[j], e[j], pe); }
+    for (int j = 0; j < KP; ++j) { pd = fmaf(s[j], dp[j], pd); pe = fmaf(s[j], e[j], pe); }
 #pragma unroll
-  for (int j = 0; j < KP; ++j) {
-    const float d = dp[j] - pd;
-    pb[j] = fmaf(e[j], d, fmaf(-pe, dp[j], pb[j]));
-    dp[j] = s[j] * d;                                            // dp = dS from here on
-    e[j] = s[j] * (e[j] - pe);                                   // e = f from here on
-  }
-  if (valid) {
-    const size_t o = ((size_t)b * n + t) * KP;
+    for (int j = 0; j < KP; ++j) {
+      const float d = dp[j] - pd;
+      pb[j] = fmaf(e[j], d, fmaf(-pe, dp[j], pb[j]));
+      dp[j] = s[j] * d;                                          // dp = dS from here on
+      e[j] = s[j] * (e[j] - pe);                                 // e = f from here on
+    }
+    if (valid) {
 #pragma unroll
-    for (int j4 = 0; j4 < KP / 4; ++j4) {
-      reinterpret_cast<float4*>(P.dS + o)[j4] = make_float4(dp[j4 * 4], dp[j4 * 4 + 1], dp[j4 * 4 + 2], dp[j4 * 4 + 3]);
-      reinterpret_cast<float4*>(P.P + o)[j4] = make_float4(s[j4 * 4], s[j4 * 4 + 1], s[j4 * 4 + 2], s[j4 * 4 + 3]);
-      reinterpret_cast<float4*>(P.dPg + o)[j4] = make_float4(e[j4 * 4], e[j4 * 4 + 1], e[j4 * 4 + 2], e[j4 * 4 + 3]);
+      for (int j4 = 0; j4 < KP / 4; ++j4) {
+        reinterpret_cast<float4*>(P.dS + orow)[j4] = make_float4(dp[j4 * 4], dp[j4 * 4 + 1], dp[j4 * 4 + 2], dp[j4 * 4 + 3]);
+        reinterpret_cast<float4*>(P.P + orow)[j4] = make_float4(s[j4 * 4], s[j4 * 4 + 1], s[j4 * 4 + 2], s[j4 * 4 + 3]);
+        reinterpret_cast<float4*>(P.dPg + orow)[j4] = make_float4(e[j4 * 4], e[j4 * 4 + 1], e[j4 * 4 + 2], e[j4 * 4 + 3]);
+      }
+    }
+  } else {
+    // dpp = mk (dp - dcbt) is what the softmax backward saw; its direct term of pbar is staged in Sg (same thread, reloaded after
+    // sweep 3), dS goes out and is reloaded for sweep 4, e becomes fq = mk f; pb keeps the cotangent of q
+    float pd = 0.f, pe = 0.f;
+#pragma unroll
+    for (int j4 = 0; j4 < KP; j4 += 4) {
+      float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+      if (valid) v = *reinterpret_cast<const float4*>(P.Sg + orow + j4);
+      e[j4] = v.x; e[j4 + 1] = v.y; e[j4 + 2] = v.z; e[j4 + 3] = v.w;
+    }
+#pragma unroll
+    for (int j = 0; j < KP; ++j) {
+      dp[j] = (dp[j] - dcbt) * (((keep >> j) & 1u) ? P.dp.scale : 0.f);
+      pd = fmaf(s[j], dp[j], pd); pe = fmaf(s[j], e[j], pe);
+    }
+#pragma unroll
+    for (int j4 = 0; j4 < KP; j4 += 4) {
+      float dr[4];
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        const int j = j4 + i;
+        const float d = dp[j] - pd;
+        dr[i] = fmaf(e[j], d, -pe * dp[j]);
+        dp[j] = s[j] * d;
+        e[j] = (((keep >> j) & 1u) ? P.dp.scale : 0.f) * (s[j] * (e[j] - pe));
+        fsum += e[j];
+      }
+      if (valid) {
+        *reinterpret_cast<float4*>(P.Sg + orow + j4) = make_float4(dr[0], dr[1], dr[2], dr[3]);
+        *reinterpret_cast<float4*>(P.dS + orow + j4) = make_float4(dp[j4], dp[j4 + 1], dp[j4 + 2], dp[j4 + 3]);
+        *reinterpret_cast<float4*>(P.P + orow + j4) = make_float4(q[j4], q[j4 + 1], q[j4 + 2], q[j4 + 3]);
+        *reinterpret_cast<float4*>(P.dPg + orow + j4) = make_float4(e[j4], e[j4 + 1], e[j4 + 2], e[j4 + 3]);
+      }
     }
   }
   const float m2 = a2 * invC;
   const float hb = ln ? sud - su * (a1 * invC) - sux * m2 : 0.f;     // derivative of U.J dxn in rstd
   const float su_c = su * invC, sux_c = sux * invC;
 
-  // ---- sweep 3: cotangents of dCtl, dxn, ctl, dOut and xn; pbar += Vt_gain ctlbar
+  // ---- sweep 3: cotangents of dCtl, dxn, ctl, dOut and xn; pbar += Vt_gain ctlbar (with dropout: the cotangent of q, and gcb)
   float t1 = 0.f, t2 = 0.f;                                      // sum_c xnbar, sum_c xnbar * xn
+  float gcb = 0.f;                                               // with dropout: gbar.cb
   for (int c0 = 0; c0 < C; c0 += BCH) {
     __syncthreads();
     bwd_load_chunk(xs, Xb, t0, n, C, c0);
@@ -585,6 +676,12 @@ __global__ void __launch_bounds__(BTM) token_bwd_vjp_kernel(const VjpParams P) {
     vjp_load_cols<KP>(va, Vtb, c0);
     vjp_load_cols<KP>(wa, Vgb, c0);
     if (both) { vjp_load_cols<KP>(vb, Vtb, C + c0); vjp_load_cols<KP>(wb, Vgb, C + c0); }
+    if constexpr (DROP) {
+      if (tid < 4 * BCH) {                                       // rows: cb gain, cb bias, cbg gain, cbg bias
+        const int r = tid / BCH, c = tid % BCH;
+        cbs[r][c] = (r & 1) && !both ? 0.f : __ldg((r < 2 ? P.cb : P.cbg) + ((r & 1) ? C : 0) + c0 + c);
+      }
+    }
     __syncthreads();
 #pragma unroll 2
     for (int cc = 0; cc < BCH; ++cc) {
@@ -594,12 +691,20 @@ __global__ void __launch_bounds__(BTM) token_bwd_vjp_kernel(const VjpParams P) {
       float g = 0.f, cg = 0.f, cbias = 0.f;
 #pragma unroll
       for (int j = 0; j < KP; ++j) {
-        if (!add) g = fmaf(s[j], va[cc][j], g);
-        cg = fmaf(wa[cc][j], s[j], fmaf(va[cc][j], e[j], cg));       // cotangent of dCtl (gain half, or the only half)
+        const float qj = DROP ? q[j] : s[j];
+        if (!add) g = fmaf(qj, va[cc][j], g);
+        cg = fmaf(wa[cc][j], qj, fmaf(va[cc][j], e[j], cg));         // cotangent of dCtl (gain half, or the only half)
       }
       if (both) {
 #pragma unroll
-        for (int j = 0; j < KP; ++j) cbias = fmaf(wb[cc][j], s[j], fmaf(vb[cc][j], e[j], cbias));
+        for (int j = 0; j < KP; ++j) cbias = fmaf(wb[cc][j], DROP ? q[j] : s[j], fmaf(vb[cc][j], e[j], cbias));
+      }
+      float cbc = 0.f;
+      if constexpr (DROP) {
+        cbc = cbs[0][cc];
+        if (!add) g = fmaf(qdef, cbc, g);
+        cg = fmaf(qdef, cbs[2][cc], fmaf(-fsum, cbc, cg));
+        if (both) cbias = fmaf(qdef, cbs[3][cc], fmaf(-fsum, cbs[1][cc], cbias));
       }
       const float dxn = add ? go : go * g;
       float gbar = 0.f, dog, xnb;
@@ -608,6 +713,7 @@ __global__ void __launch_bounds__(BTM) token_bwd_vjp_kernel(const VjpParams P) {
         gbar = dxnb * go;                                        // cotangent of ctl (gain half)
 #pragma unroll
         for (int j = 0; j < KP; ++j) pb[j] = fmaf(gbar, va[cc][j], pb[j]);
+        if constexpr (DROP) gcb = fmaf(gbar, cbc, gcb);
         dog = fmaf(dxnb, g, cg * xn) + cbias;
         xnb = cg * go;
       }
@@ -623,6 +729,22 @@ __global__ void __launch_bounds__(BTM) token_bwd_vjp_kernel(const VjpParams P) {
     bwd_store_chunk(Cgb, us, t0, n, Cout, c0);
     if (both) bwd_zero_chunk(Cgb, t0, n, Cout, C + c0);
   }
+  if constexpr (DROP) {
+    // pbar = mk (cotangent of q) + the staged direct term; dS back for sweep 4
+    const float sh = dcg + gcb;
+#pragma unroll
+    for (int j4 = 0; j4 < KP; j4 += 4) {
+      float4 dr = make_float4(0.f, 0.f, 0.f, 0.f), ds = dr;
+      if (valid) { dr = *reinterpret_cast<const float4*>(P.Sg + orow + j4); ds = *reinterpret_cast<const float4*>(P.dS + orow + j4); }
+      const float drv[4] = {dr.x, dr.y, dr.z, dr.w}, dsv[4] = {ds.x, ds.y, ds.z, ds.w};
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        const int j = j4 + i;
+        pb[j] = fmaf(((keep >> j) & 1u) ? P.dp.scale : 0.f, pb[j] - sh, drv[i]);
+        dp[j] = dsv[i];
+      }
+    }
+  }
   // ---- Sg = p (pbar - <p, pbar>)
   float pp = 0.f;
 #pragma unroll
@@ -630,7 +752,7 @@ __global__ void __launch_bounds__(BTM) token_bwd_vjp_kernel(const VjpParams P) {
 #pragma unroll
   for (int j = 0; j < KP; ++j) pb[j] = s[j] * (pb[j] - pp);      // pb = Sg from here on
   if (valid) {
-    float4* sg4 = reinterpret_cast<float4*>(P.Sg + ((size_t)b * n + t) * KP);
+    float4* sg4 = reinterpret_cast<float4*>(P.Sg + orow);
 #pragma unroll
     for (int j4 = 0; j4 < KP / 4; ++j4) sg4[j4] = make_float4(pb[j4 * 4], pb[j4 * 4 + 1], pb[j4 * 4 + 2], pb[j4 * 4 + 3]);
   }
@@ -881,6 +1003,22 @@ extern "C" int gf_attn_simplex_bwd_vjp(const gf_attn_desc* desc, const float* X,
                                        const float* Rt, const float* Ct, const float* U, const float* Kpg, const float* Vtg,
                                        const float* Rtg, const float* Ctg, float* Xg, float* dOutg, float* Sg, float* dPg, float* Ctlg,
                                        float* dS, float* Pout, float* dCtl, void* stream) {
+  return gf_attn_simplex_bwd_vjp_ex(desc, X, dOut, Kp, Vt, Rt, Ct, U, Kpg, Vtg, Rtg, Ctg, Xg, dOutg, Sg, dPg, Ctlg, dS, Pout, dCtl,
+                                    0.f, 0, nullptr, nullptr, nullptr, stream);
+}
+
+template <int KP, bool DROP>
+static int launch_token_bwd_vjp(const VjpParams& P, dim3 grid, int smem, cudaStream_t st) {
+  GF_CUDA_OK(cudaFuncSetAttribute(token_bwd_vjp_kernel<KP, DROP>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+  token_bwd_vjp_kernel<KP, DROP><<<grid, BTM, smem, st>>>(P);
+  return GF_OK;
+}
+
+extern "C" int gf_attn_simplex_bwd_vjp_ex(const gf_attn_desc* desc, const float* X, const float* dOut, const float* Kp, const float* Vt,
+                                          const float* Rt, const float* Ct, const float* U, const float* Kpg, const float* Vtg,
+                                          const float* Rtg, const float* Ctg, float* Xg, float* dOutg, float* Sg, float* dPg, float* Ctlg,
+                                          float* dS, float* Pout, float* dCtl, float att_dp, uint32_t dp_salt,
+                                          const unsigned long long* dp_state, const float* cb, const float* cbg, void* stream) {
   Layout L;
   int rc = make_layout(desc, &L);
   if (rc) return rc;
@@ -890,21 +1028,27 @@ extern "C" int gf_attn_simplex_bwd_vjp(const gf_attn_desc* desc, const float* X,
   if (desc->norm != GF_NORM_LAYER && desc->norm != GF_NORM_NONE) { set_error("gf_attn_simplex_bwd_vjp: norm must be layer or none"); return GF_ERR_UNSUPPORTED; }
   if (L.heads != 1) { set_error("gf_attn_simplex_bwd_vjp: one head"); return GF_ERR_UNSUPPORTED; }
   if (L.B > 65535) { set_error("gf_attn_simplex_bwd_vjp: B > 65535"); return GF_ERR_UNSUPPORTED; }
-  if ((rc = check_device())) return rc;
   VjpParams P;
+  {
+    gf_attn_postop post;
+    memset(&post, 0, sizeof(post));
+    post.att_dp = att_dp; post.dp_salt = dp_salt; post.dp_state = dp_state;
+    if ((rc = dropout_args(&post, &P.dp))) return rc;
+    if (P.dp.thr && (!cb || !cbg)) {
+      set_error("gf_attn_simplex_bwd_vjp_ex: attention dropout needs cb (bo, +1 on the gain half) and its cotangent cbg"); return GF_ERR_INVALID;
+    }
+    P.cb = cb; P.cbg = cbg;
+  }
+  if ((rc = check_device())) return rc;
   P.X = X; P.dOut = dOut; P.Kp = Kp; P.Vt = Vt; P.Rt = Rt; P.Ct = Ct; P.U = U; P.Kg = Kpg; P.Vg = Vtg; P.Rg = Rtg; P.Cg = Ctg;
   P.Xg = Xg; P.dOutg = dOutg; P.Sg = Sg; P.dPg = dPg; P.Ctlg = Ctlg; P.dS = dS; P.P = Pout; P.dCtl = dCtl;
   P.n = L.n; P.H = L.H; P.W = L.W; P.C = L.C; P.Cout = L.Cout; P.norm = desc->norm; P.integration = desc->integration;
   dim3 grid((L.n + BTM - 1) / BTM, L.B);
-  const int smem = (int)(3 * sizeof(float) * BTM * BXS + 4 * sizeof(float) * L.KP * BCH);
+  const int smem = (int)(3 * sizeof(float) * BTM * BXS + 4 * sizeof(float) * L.KP * BCH + (P.dp.thr ? 4 * sizeof(float) * BCH : 0));
   cudaStream_t st = (cudaStream_t)stream;
-  if (L.KP == 16) {
-    GF_CUDA_OK(cudaFuncSetAttribute(token_bwd_vjp_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    token_bwd_vjp_kernel<16><<<grid, BTM, smem, st>>>(P);
-  } else {
-    GF_CUDA_OK(cudaFuncSetAttribute(token_bwd_vjp_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    token_bwd_vjp_kernel<32><<<grid, BTM, smem, st>>>(P);
-  }
+  if (L.KP == 16) rc = P.dp.thr ? launch_token_bwd_vjp<16, true>(P, grid, smem, st) : launch_token_bwd_vjp<16, false>(P, grid, smem, st);
+  else rc = P.dp.thr ? launch_token_bwd_vjp<32, true>(P, grid, smem, st) : launch_token_bwd_vjp<32, false>(P, grid, smem, st);
+  if (rc) return rc;
   GF_LAUNCH_OK();
   return GF_OK;
 }

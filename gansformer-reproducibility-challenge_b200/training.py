@@ -14,7 +14,14 @@ composite for the rest (duplex layers without dropout, instance / batch norm, mu
 aggregating the image into learned latents that are carried from layer to layer and concatenated to the final features.  Those
 layers run the CUDA forward and the duplex kernel backward (``BipartiteAttention.kernel_backward``), and by default the torch
 composite in the R1 pass, which needs their second derivative; with ``Discriminator(r1_kernels=True)`` the R1 pass runs them on the
-kernels too, differentiated twice through the double-backward kernels (``BipartiteAttention.kernel_double_backward``).  Path-length regularisation and augmentation are out of scope.
+kernels too, differentiated twice through the double-backward kernels (``BipartiteAttention.kernel_double_backward``).
+
+``TrainConfig.pl_weight > 0`` adds StyleGAN2's path-length regularisation of the generator, lazily, every ``g_reg_interval``-th
+step after the G update: on the first B // pl_batch_shrink latents, the gradient of <G.synthesis(ws), noise / sqrt(H W)> with respect
+to the dlatents ws [B, k+1, D], its length over the k+1 latent components (SURVEY A.4 item 12), and the squared distance of that
+length to its running mean.  The backward of that gradient needs the generator's second derivative: the attention layers give it
+through the double-backward kernels (``gf_attn_simplex_bwd_vjp_ex``, with the forward's dropout mask) or, on the composite route, torch
+autograd.  Off by default.  Augmentation is out of scope.
 """
 from __future__ import annotations
 
@@ -181,6 +188,10 @@ class TrainConfig:
     noise_mode: str = "random"
     bucket_mb: float = 32.0             # gradient all-reduce bucket size (MB of fp32 gradients)
     w_avg_beta: float = 0.995           # decay of the running mean of the mapping outputs (truncation trick)
+    pl_weight: float = 0.0              # path-length regularisation of G (StyleGAN2: 2); 0 = off
+    g_reg_interval: int = 4             # lazy path-length regularisation: every 4th generator step
+    pl_batch_shrink: int = 2            # the path-length phase runs on the first B // 2 latents
+    pl_decay: float = 0.01              # decay of the running mean of the path lengths
 
 
 @dataclass
@@ -191,6 +202,8 @@ class StepStats:
     allreduce_bytes: float = 0.0
     allreduce_ms: float = 0.0
     extra: Dict[str, float] = field(default_factory=dict)
+    pl_penalty: float = 0.0             # mean squared deviation of the path lengths from their running mean (a path-length step)
+    pl_mean: float = 0.0                # the running mean of the path lengths (this rank's)
 
 
 class Trainer:
@@ -201,7 +214,10 @@ class Trainer:
         self.G_ema = copy.deepcopy(G).eval().requires_grad_(False)
         c = self.cfg.d_reg_interval / (self.cfg.d_reg_interval + 1.0)  # lazy regularisation: rescale lr and betas
         cap = next(G.parameters()).is_cuda                              # capturable: the step can be replayed from a CUDA graph
-        self.opt_g = torch.optim.Adam(G.parameters(), lr=self.cfg.lr, betas=(0.0, 0.99), eps=1e-8, capturable=cap)
+        cg = self.cfg.g_reg_interval / (self.cfg.g_reg_interval + 1.0) if self.cfg.pl_weight > 0 else 1.0
+        self.opt_g = torch.optim.Adam(G.parameters(), lr=self.cfg.lr * cg, betas=(0.0 ** cg, 0.99 ** cg), eps=1e-8, capturable=cap)
+        # running mean of the path lengths: a device tensor updated in place (capturable), per rank as upstream
+        self.pl_mean = torch.zeros((), device=next(G.parameters()).device) if self.cfg.pl_weight > 0 else None
         self.opt_d = torch.optim.Adam(D.parameters(), lr=self.cfg.lr * c, betas=(0.0 ** c, 0.99 ** c), eps=1e-8, capturable=cap)
         self.it = 0
         # data parallel: gradients live in one flat buffer per network, reduced bucket by bucket while backward still runs
@@ -218,8 +234,10 @@ class Trainer:
         if buckets is not None:
             stats.allreduce_bytes += buckets.finish()      # joins the communication stream (the buckets overlapped backward)
 
-    def _step_tensors(self, z: torch.Tensor, reals: torch.Tensor, do_r1: bool, stats: Optional[StepStats] = None):
-        """One D update + one G update; returns (loss_d, loss_g, r1) as device tensors without synchronising (capturable)."""
+    def _step_tensors(self, z: torch.Tensor, reals: torch.Tensor, do_r1: bool, stats: Optional[StepStats] = None,
+                      do_pl: bool = False):
+        """One D update + one G update (+ the path-length update with ``do_pl``); returns (loss_d, loss_g, r1, pl_penalty) as device
+        tensors without synchronising (capturable); pl_penalty is None without ``do_pl``."""
         G, D, cfg = self.G, self.D, self.cfg
         stats = stats if stats is not None else StepStats()
         # ---- discriminator: logistic loss (+ lazy R1 on the reals)
@@ -250,6 +268,7 @@ class Trainer:
         self.opt_g.step()
         if z.is_cuda:
             advance_dropout(z.device)                 # ... and for the next step
+        pl_penalty = self._pl_phase(z, stats) if do_pl else None
         # ---- moving average of the generator (and of the mapping outputs: the truncation trick's w_avg)
         with torch.no_grad():
             if hasattr(G, "mapping") and hasattr(G.mapping, "w_avg"):
@@ -262,31 +281,66 @@ class Trainer:
                 pe.lerp_(p.detach(), 1.0 - beta)
             for be, b in zip(self.G_ema.buffers(), G.buffers()):
                 be.copy_(b)
-        return loss_d.detach(), loss_g.detach(), r1.detach()
+        return loss_d.detach(), loss_g.detach(), r1.detach(), pl_penalty
+
+    def _pl_phase(self, z: torch.Tensor, stats: StepStats) -> torch.Tensor:
+        """The lazy path-length update of G (StyleGAN2): returns the penalty as a device tensor (capturable: no host sync, the
+        noise is drawn on the device)."""
+        G, cfg = self.G, self.cfg
+        if z.is_cuda:
+            from .attention import advance_dropout
+            advance_dropout(z.device)                 # fresh attention-dropout masks; the backward regenerates the same ones
+        self._zero(self.opt_g, self.buckets_g)
+        ws = G.mapping(z[:max(1, z.shape[0] // cfg.pl_batch_shrink)])
+        img = G.synthesis(ws, noise_mode=cfg.noise_mode)
+        pl_noise = torch.randn_like(img) / math.sqrt(img.shape[2] * img.shape[3])
+        (pl_grads,) = torch.autograd.grad((img * pl_noise).sum(), ws, create_graph=True)
+        pl_lengths = pl_grads.square().sum(dim=2).mean(dim=1).sqrt()          # [B']: over D, then over the k+1 latent components
+        with torch.no_grad():
+            self.pl_mean.lerp_(pl_lengths.mean(), cfg.pl_decay)
+        pl_penalty = (pl_lengths - self.pl_mean).square().mean()
+        (pl_penalty * (cfg.pl_weight * cfg.g_reg_interval)).backward()
+        self._allreduce(self.buckets_g, stats)
+        self.opt_g.step()
+        if z.is_cuda:
+            advance_dropout(z.device)
+        return pl_penalty.detach()
+
+    def _do_pl(self) -> bool:
+        return self.cfg.pl_weight > 0 and self.it % self.cfg.g_reg_interval == 0
+
+    def _finish_stats(self, stats: StepStats, loss_d, loss_g, r1, pl_penalty) -> StepStats:
+        stats.loss_d, stats.loss_g, stats.r1 = float(loss_d), float(loss_g), float(r1)
+        if pl_penalty is not None:
+            stats.pl_penalty = float(pl_penalty)
+        if self.pl_mean is not None:
+            stats.pl_mean = float(self.pl_mean)
+        return stats
 
     def step(self, z: torch.Tensor, reals: torch.Tensor) -> StepStats:
         stats = StepStats()
         do_r1 = self.cfg.r1_gamma > 0 and self.it % self.cfg.d_reg_interval == 0
-        loss_d, loss_g, r1 = self._step_tensors(z, reals, do_r1, stats)
-        stats.loss_d, stats.loss_g, stats.r1 = float(loss_d), float(loss_g), float(r1)
+        outs = self._step_tensors(z, reals, do_r1, stats, self._do_pl())
+        self._finish_stats(stats, *outs)
         bump_weights_epoch()
         self.it += 1
         return stats
 
     def step_graphed(self, z: torch.Tensor, reals: torch.Tensor) -> StepStats:
-        """The same step replayed from a CUDA graph (one graph with the lazy R1 term, one without): the eager step is bound by
-        the host launching ~5000 small kernels.  Shapes are fixed by the first call; the first calls warm up eagerly."""
+        """The same step replayed from a CUDA graph (one graph per combination of the lazy R1 term and the lazy path-length
+        phase that occurs, at most three with the default intervals): the eager step is bound by the host launching ~5000 small
+        kernels.  Shapes are fixed by the first call; the first calls warm up eagerly."""
         from . import attention as _att, networks as _nets
         cfg = self.cfg
         do_r1 = cfg.r1_gamma > 0 and self.it % cfg.d_reg_interval == 0
         st = self.__dict__.setdefault("_graphs", {})
         _nets.CACHE_BYPASS = _att.FORCE_REFOLD = True                  # weight-derived tensors are recomputed inside the graph
         try:
-            return self._step_graphed(z, reals, do_r1, st)
+            return self._step_graphed(z, reals, (do_r1, self._do_pl()), st)
         finally:
             _nets.CACHE_BYPASS = _att.FORCE_REFOLD = False
 
-    def _step_graphed(self, z, reals, do_r1, st) -> StepStats:
+    def _step_graphed(self, z, reals, key, st) -> StepStats:
         cfg = self.cfg
         if "z" not in st:
             st["z"], st["reals"] = torch.empty_like(z), torch.empty_like(reals)
@@ -296,17 +350,19 @@ class Trainer:
             with torch.cuda.stream(side):
                 for r in ([True, False] if cfg.r1_gamma > 0 else [False]):
                     self._step_tensors(st["z"], st["reals"], r)
+                if cfg.pl_weight > 0:
+                    self._step_tensors(st["z"], st["reals"], False, do_pl=True)
             torch.cuda.current_stream(z.device).wait_stream(side)
             torch.cuda.synchronize(z.device)
         st["z"].copy_(z); st["reals"].copy_(reals)
-        if do_r1 not in st:
+        if key not in st:
             graph = torch.cuda.CUDAGraph()
             with torch.cuda.graph(graph):
-                outs = self._step_tensors(st["z"], st["reals"], do_r1)
-            st[do_r1] = (graph, outs)
+                outs = self._step_tensors(st["z"], st["reals"], key[0], do_pl=key[1])
+            st[key] = (graph, outs)
             # (capture does not execute: fall through to the replay below)
-        graph, (loss_d, loss_g, r1) = st[do_r1]
+        graph, outs = st[key]
         graph.replay()
         bump_weights_epoch()          # the replay moved G / D / G_ema weights without touching their version counters
         self.it += 1
-        return StepStats(loss_g=float(loss_g), loss_d=float(loss_d), r1=float(r1))
+        return self._finish_stats(StepStats(), *outs)

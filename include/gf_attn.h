@@ -243,6 +243,18 @@ int gf_attn_simplex_bwd_vjp(const gf_attn_desc* desc, const float* X, const floa
                             const float* Ctg, float* Xg, float* dOutg, float* Sg, float* dPg, float* Ctlg, float* dS, float* P,
                             float* dCtl, void* stream);
 
+/* gf_attn_simplex_bwd_vjp with attention dropout (the generator's path-length penalty): the VJP of gf_attn_simplex_bwd_ex.  The
+ * same (att_dp, dp_salt, dp_state) as the forward call regenerate the mask; cb [Cout] as there.  The function differentiated gains
+ * the reduction dcb = sum_tokens (1 - sum_j q_j) dCtl, whose cotangent is cbg [Cout].  P then receives q (the probabilities after
+ * dropout), dPg the cotangent of dp = Vt^T dCtl before the mask; the caller's reductions are those above (with P = q) plus
+ *   cb: sum_tokens (1 - sum_j P_j) Ctlg - (sum_j dPg_j) dCtl.
+ * With att_dp == 0 this is gf_attn_simplex_bwd_vjp bit for bit, and cb, cbg may be NULL (cbg is ignored: dcb is then 0). */
+int gf_attn_simplex_bwd_vjp_ex(const gf_attn_desc* desc, const float* X, const float* dOut, const float* Kp, const float* Vt,
+                               const float* Rt, const float* Ct, const float* U, const float* Kpg, const float* Vtg, const float* Rtg,
+                               const float* Ctg, float* Xg, float* dOutg, float* Sg, float* dPg, float* Ctlg, float* dS, float* P,
+                               float* dCtl, float att_dp, uint32_t dp_salt, const unsigned long long* dp_state, const float* cb,
+                               const float* cbg, void* stream);
+
 /* gf_attn_centroid_bwd_vjp: the VJP of (X, M, Rt2, Ct2, lse, dXbar, r, dX_in) -> (dX_out, dS^T X, sum_w dS, sum_h dS) of
  * gf_attn_centroid_bwd.  Cotangents in: U [B,n,C] of dX_out, Mg [B,KP,C], Rt2g [B,H,KP], Ct2g [B,W,KP].  Out: Xg [B,n,C] (the
  * cotangent of X), Sg [B,n,KP] (of the logits), Gg [B,n,KP] (of g = x.dXbar), A [B,n,KP] and dS [B,n,KP].  The caller reduces
