@@ -15,6 +15,10 @@ static inline int grid_for(size_t work_items, int threads) {
   return (int)(b > cap ? cap : (b < 1 ? 1 : b));
 }
 
+// the streaming kernels move float4s: every operand they access that way must start on a 16-byte boundary (NULL passes:
+// the optional operands are checked for presence elsewhere)
+static inline bool misaligned16(const void* p) { return ((uintptr_t)p & 15) != 0; }
+
 __global__ void __launch_bounds__(256) chan_scale_kernel(const float4* __restrict__ x, const float4* __restrict__ s,
                                                          float4* __restrict__ y, size_t total4, int hw_c4, int c4n, int s_ld4) {
   for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < total4; i += (size_t)gridDim.x * blockDim.x) {
@@ -405,8 +409,9 @@ extern "C" {
 
 int gf_chan_scale_nhwc(const float* x, const float* s, int s_ld, float* y, int B, int HW, int C, void* stream) {
   if (!x || !s || !y) { set_error("gf_chan_scale_nhwc: null pointer"); return GF_ERR_INVALID; }
-  if (B <= 0 || HW <= 0 || C <= 0 || (C & 3) || s_ld < C || (s_ld & 3) || ((uintptr_t)s & 15)) {
-    set_error("gf_chan_scale_nhwc: need B,HW,C > 0, C %% 4 == 0, s_ld >= C, s_ld %% 4 == 0, s 16-byte aligned (C=%d s_ld=%d)", C, s_ld);
+  if (misaligned16(x) || misaligned16(s) || misaligned16(y)) { set_error("gf_chan_scale_nhwc: x, s and y must be 16-byte aligned"); return GF_ERR_INVALID; }
+  if (B <= 0 || HW <= 0 || C <= 0 || (C & 3) || s_ld < C || (s_ld & 3)) {
+    set_error("gf_chan_scale_nhwc: need B,HW,C > 0, C %% 4 == 0, s_ld >= C, s_ld %% 4 == 0 (C=%d s_ld=%d)", C, s_ld);
     return GF_ERR_UNSUPPORTED;
   }
   const size_t total4 = (size_t)B * HW * (C >> 2);
@@ -418,6 +423,7 @@ int gf_chan_scale_nhwc(const float* x, const float* s, int s_ld, float* y, int B
 
 int gf_blur_up_nhwc(const float* x, float* y, const float* scale, int B, int Hout, int Wout, int C, float gain, void* stream) {
   if (!x || !y) { set_error("gf_blur_up_nhwc: null pointer"); return GF_ERR_INVALID; }
+  if (misaligned16(x) || misaligned16(y) || misaligned16(scale)) { set_error("gf_blur_up_nhwc: x, y and scale must be 16-byte aligned"); return GF_ERR_INVALID; }
   if (B <= 0 || Hout <= 0 || Wout <= 0 || C <= 0 || (C & 3) || B > 65535) { set_error("gf_blur_up_nhwc: bad shape (B=%d Hout=%d Wout=%d C=%d)", B, Hout, Wout, C); return GF_ERR_UNSUPPORTED; }
   constexpr int ROWS = 8;
   dim3 grid((Wout * (C >> 2) + 255) / 256, (Hout + ROWS - 1) / ROWS, B);
@@ -429,6 +435,9 @@ int gf_blur_up_nhwc(const float* x, float* y, const float* scale, int B, int Hou
 int gf_blur_up_phases_nhwc(const float* p00, const float* p01, const float* p10, const float* p11, float* y, const float* scale,
                            int B, int Hout, int Wout, int C, float gain, void* stream) {
   if (!p00 || !p01 || !p10 || !p11 || !y) { set_error("gf_blur_up_phases_nhwc: null pointer"); return GF_ERR_INVALID; }
+  if (misaligned16(p00) || misaligned16(p01) || misaligned16(p10) || misaligned16(p11) || misaligned16(y) || misaligned16(scale)) {
+    set_error("gf_blur_up_phases_nhwc: the four phases, y and scale must be 16-byte aligned"); return GF_ERR_INVALID;
+  }
   if (B <= 0 || Hout <= 0 || Wout <= 0 || (Hout & 1) || (Wout & 1) || C <= 0 || (C & 3) || B > 65535) {
     set_error("gf_blur_up_phases_nhwc: bad shape (B=%d Hout=%d Wout=%d C=%d)", B, Hout, Wout, C); return GF_ERR_UNSUPPORTED;
   }
@@ -443,6 +452,7 @@ int gf_blur_up_phases_nhwc(const float* p00, const float* p01, const float* p10,
 
 int gf_fir4_nhwc(const float* x, float* y, int B, int Hin, int Win, int C, int pad, float gain, void* stream) {
   if (!x || !y) { set_error("gf_fir4_nhwc: null pointer"); return GF_ERR_INVALID; }
+  if (misaligned16(x) || misaligned16(y)) { set_error("gf_fir4_nhwc: x and y must be 16-byte aligned"); return GF_ERR_INVALID; }
   const int Hout = Hin + 2 * pad - 3, Wout = Win + 2 * pad - 3;
   if (B <= 0 || Hout <= 0 || Wout <= 0 || C <= 0 || (C & 3) || B > 65535 || pad < 0 || pad > 3) {
     set_error("gf_fir4_nhwc: bad arguments (B=%d Hin=%d Win=%d C=%d pad=%d)", B, Hin, Win, C, pad); return GF_ERR_UNSUPPORTED;
@@ -467,6 +477,7 @@ int gf_upsample2x_nchw(const float* x, const float* add, float* y, int B, int C,
 int gf_bias_act_nhwc(const float* x, float* y, const float* bias, const float* noise, const float* strength,
                      long long noise_bstride, int B, int HW, int C, int act, float gain, void* stream) {
   if (!x || !y) { set_error("gf_bias_act_nhwc: null pointer"); return GF_ERR_INVALID; }
+  if (misaligned16(x) || misaligned16(y) || misaligned16(bias)) { set_error("gf_bias_act_nhwc: x, y and bias must be 16-byte aligned"); return GF_ERR_INVALID; }
   if (B <= 0 || HW <= 0 || C <= 0 || (C & 3) || act < 0 || act > 1) { set_error("gf_bias_act_nhwc: bad arguments (C=%d act=%d)", C, act); return GF_ERR_UNSUPPORTED; }
   const size_t total4 = (size_t)B * HW * (C >> 2);
   bias_act_kernel<<<grid_for(total4, 256 * 4), 256, 0, (cudaStream_t)stream>>>(
@@ -508,6 +519,7 @@ int gf_torgb_nhwc(const float* x, const float* w, const float* styles, int s_ld,
 int gf_torgb_scale_nhwc(const float* x, const float* w, const float* styles, int s_ld, const float* bias, float wscale, float* y,
                         const float* s2, int s2_ld, float* xs_out, int B, int HW, int C, void* stream) {
   if (!x || !w || !styles || !y) { set_error("gf_torgb_nhwc: null pointer"); return GF_ERR_INVALID; }
+  if (misaligned16(x) || misaligned16(w) || misaligned16(styles)) { set_error("gf_torgb_nhwc: x, w and styles must be 16-byte aligned"); return GF_ERR_INVALID; }
   if ((xs_out != nullptr) != (s2 != nullptr) || (xs_out && (s2_ld < C || (s2_ld & 3) || ((uintptr_t)s2 & 15) || ((uintptr_t)xs_out & 15)))) {
     set_error("gf_torgb_scale_nhwc: s2 / xs_out must both be given, 16-byte aligned, s2_ld >= C and %% 4 == 0"); return GF_ERR_INVALID;
   }

@@ -55,18 +55,25 @@ def _nhwc_view(x: torch.Tensor) -> torch.Tensor:
     return v if v.is_contiguous() else v.contiguous()
 
 
+def _aligned(t: torch.Tensor) -> torch.Tensor:
+    """t as a contiguous tensor starting on a 16-byte boundary, as the float4 kernels of gf_ops.h require: a contiguous view
+    that starts inside its storage (e.g. b[1:1 + C]) is copied."""
+    t = t.contiguous()
+    return t if t.data_ptr() % 16 == 0 else t.clone()
+
+
 def _rows(s: torch.Tensor):
     """(tensor, row stride in floats) of a [B, C] matrix that may be a column slice of a wider contiguous matrix."""
     if s.dim() == 2 and s.stride(1) == 1 and s.stride(0) % 4 == 0 and s.data_ptr() % 16 == 0 and s.stride(0) >= s.shape[1]:
         return s, s.stride(0)
-    s = s.contiguous()
+    s = _aligned(s)
     return s, s.shape[1]
 
 
 def chan_scale(x: torch.Tensor, s: torch.Tensor) -> torch.Tensor:
     """x [B,C,H,W] * s [B,C] (style modulation / demodulation as activation scaling)."""
     if _use_cuda(x, s) and x.shape[1] % 4 == 0:
-        xv = _nhwc_view(x)
+        xv = _aligned(_nhwc_view(x))
         B, H, W, C = xv.shape
         y = torch.empty_like(xv)
         sr, ld = _rows(s)
@@ -84,7 +91,7 @@ class _Fir4(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, pad, gain):
         ctx.pad, ctx.gain = pad, gain
-        xv = _nhwc_view(x.detach())
+        xv = _aligned(_nhwc_view(x.detach()))
         B, H, W, C = xv.shape
         y = torch.empty((B, H + 2 * pad - 3, W + 2 * pad - 3, C), dtype=torch.float32, device=x.device)
         with torch.cuda.device(x.device):
@@ -108,11 +115,11 @@ def fir4(x: torch.Tensor, f: torch.Tensor, pad: int, gain: float = 1.0) -> torch
 def blur_up(x: torch.Tensor, f: torch.Tensor, scale: Optional[torch.Tensor] = None, gain: float = 4.0) -> torch.Tensor:
     """FIR blur after a stride-2 transposed conv: x [B,C,2H+1,2W+1] -> [B,C,2H,2W] (pad 1), optional * scale [B,C]."""
     if _use_cuda(x, scale) and x.shape[1] % 4 == 0:
-        xv = _nhwc_view(x)
+        xv = _aligned(_nhwc_view(x))
         B, Hin, Win, C = xv.shape
         y = torch.empty((B, Hin - 1, Win - 1, C), dtype=torch.float32, device=x.device)
         with torch.cuda.device(x.device):
-            _lib.check(_lib.load().gf_blur_up_nhwc(xv.data_ptr(), y.data_ptr(), None if scale is None else scale.contiguous().data_ptr(),
+            _lib.check(_lib.load().gf_blur_up_nhwc(xv.data_ptr(), y.data_ptr(), None if scale is None else _aligned(scale).data_ptr(),
                                                    B, Hin - 1, Win - 1, C, float(gain), _stream(x.device)), "gf_blur_up_nhwc")
         return y.permute(0, 3, 1, 2)
     y = fir4(x, f, 1, gain=gain)                                        # training: native FIR both ways, scale in torch
@@ -139,7 +146,7 @@ def upconv_blur_phases(x: torch.Tensor, phases, scale: Optional[torch.Tensor] = 
     y = torch.empty((B, 2 * H, 2 * W, C), dtype=torch.float32, device=x.device)
     with torch.cuda.device(x.device):
         _lib.check(_lib.load().gf_blur_up_phases_nhwc(ps[0].data_ptr(), ps[1].data_ptr(), ps[2].data_ptr(), ps[3].data_ptr(), y.data_ptr(),
-                                                      None if scale is None else scale.contiguous().data_ptr(), B, 2 * H, 2 * W, C,
+                                                      None if scale is None else _aligned(scale).data_ptr(), B, 2 * H, 2 * W, C,
                                                       float(gain), _stream(x.device)), "gf_blur_up_phases_nhwc")
     return y.permute(0, 3, 1, 2)
 
@@ -160,13 +167,13 @@ def upsample2x(x: torch.Tensor, f: torch.Tensor, add: Optional[torch.Tensor] = N
 
 
 def _bias_act_native(x, bias, act, noise, strength, gain):
-    xv = _nhwc_view(x)
+    xv = _aligned(_nhwc_view(x))
     B, H, W, C = xv.shape
     y = torch.empty_like(xv)
     nz = None if noise is None else noise.contiguous()
     bstride = H * W if (nz is not None and nz.numel() == B * H * W and B > 1) else 0
     with torch.cuda.device(x.device):
-        _lib.check(_lib.load().gf_bias_act_nhwc(xv.data_ptr(), y.data_ptr(), None if bias is None else bias.contiguous().data_ptr(),
+        _lib.check(_lib.load().gf_bias_act_nhwc(xv.data_ptr(), y.data_ptr(), None if bias is None else _aligned(bias).data_ptr(),
                                                 None if nz is None else nz.data_ptr(),
                                                 None if strength is None else strength.data_ptr(), bstride, B, H * W, C,
                                                 1 if act == "lrelu" else 0, float(gain), _stream(x.device)), "gf_bias_act_nhwc")
@@ -207,13 +214,13 @@ def bias_act(x: torch.Tensor, bias: Optional[torch.Tensor], act: str = "lrelu", 
             and any(t is not None and t.requires_grad for t in (x, bias, strength)):
         return _BiasAct.apply(x, bias, noise, strength, act, gain)
     if _use_cuda(x, bias, noise, strength) and x.shape[1] % 4 == 0:
-        xv = _nhwc_view(x)
+        xv = _aligned(_nhwc_view(x))
         B, H, W, C = xv.shape
         y = torch.empty_like(xv)
         nz = None if noise is None else noise.contiguous()
         bstride = H * W if (nz is not None and nz.numel() == B * H * W and B > 1) else 0
         with torch.cuda.device(x.device):
-            _lib.check(_lib.load().gf_bias_act_nhwc(xv.data_ptr(), y.data_ptr(), None if bias is None else bias.contiguous().data_ptr(),
+            _lib.check(_lib.load().gf_bias_act_nhwc(xv.data_ptr(), y.data_ptr(), None if bias is None else _aligned(bias).data_ptr(),
                                                     None if nz is None else nz.data_ptr(),
                                                     None if strength is None else strength.data_ptr(), bstride, B, H * W, C,
                                                     1 if act == "lrelu" else 0, float(gain), _stream(x.device)), "gf_bias_act_nhwc")
@@ -280,11 +287,11 @@ def torgb(x: torch.Tensor, weight: torch.Tensor, styles: torch.Tensor, bias: Opt
     O, I = weight.shape[:2]
     wscale = 1.0 / math.sqrt(I)
     if _use_cuda(x, weight, styles, bias, next_styles) and O == 3 and I % 4 == 0 and I <= 512:
-        xv = _nhwc_view(x)
+        xv = _aligned(_nhwc_view(x))
         B, H, W, C = xv.shape
         y = torch.empty((B, O, H, W), device=x.device, dtype=torch.float32)
         sr, ld = _rows(styles)
-        wv = weight.reshape(O, I).contiguous()
+        wv = _aligned(weight.reshape(O, I))
         xs = s2 = None
         ld2 = 0
         if next_styles is not None:

@@ -6,6 +6,10 @@
  * /root/reference/.SUBMODULES.json:2) -- restricted to the uses the generator makes of them, plus the
  * activation-scaling form of StyleGAN2's weight (de)modulation.  Channels-last fp32, raw device pointers,
  * enqueue-only on `stream` (a cudaStream_t passed as void*), same error convention as gf_attn.h.
+ *
+ * Alignment: the channels-last kernels move float4s.  Every operand listed as "16-byte aligned" below must start on a 16-byte
+ * boundary (a contiguous view that starts 4 bytes into its storage does not); otherwise the call returns GF_ERR_INVALID
+ * before it touches the device.
  */
 #ifndef GF_OPS_H_
 #define GF_OPS_H_
@@ -19,25 +23,29 @@ extern "C" {
 
 /* y[b,t,c] = x[b,t,c] * s[b*s_ld + c].   Style modulation of a conv input / demodulation of a conv output
  * (modulated_conv2d_layer in the reference, activation-scaling form).  y may alias x.  C % 4 == 0; s_ld (row stride
- * of s in floats) % 4 == 0 so that rows of a column slice of a wider [B, sum C] style matrix can be passed directly. */
+ * of s in floats) % 4 == 0 so that rows of a column slice of a wider [B, sum C] style matrix can be passed directly.
+ * x, s and y 16-byte aligned. */
 int gf_chan_scale_nhwc(const float* x, const float* s, int s_ld, float* y, int B, int HW, int C, void* stream);
 
 /* upfirdn_2d, use (a): the FIR blur that follows a stride-2 transposed convolution.
  * x [B, Hout+1, Wout+1, C] -> y [B, Hout, Wout, C]; separable filter [1,3,3,1]/8 per axis, total gain `gain`
- * (4 after an upsampling conv), zero padding 1 on every side; optional per-(b,c) scale (demodulation). C % 4 == 0. */
+ * (4 after an upsampling conv), zero padding 1 on every side; optional per-(b,c) scale (demodulation). C % 4 == 0.
+ * x, y and scale 16-byte aligned. */
 int gf_blur_up_nhwc(const float* x, float* y, const float* scale, int B, int Hout, int Wout, int C, float gain, void* stream);
 
 /* Use (a) again, with the transposed convolution's output T [B, Hout+1, Wout+1, C] given as its four polyphase components
  * pab[b, i, j, c] = T[b, 2i+a, 2j+b', c] (p00 [B,H+1,W+1,C], p01 [B,H+1,W,C], p10 [B,H,W+1,C], p11 [B,H,W,C]; H = Hout/2,
  * W = Wout/2): the stride-2 transposed 3x3 convolution equals four stride-1 convolutions of the low-resolution input
- * (2x2, 2x1, 1x2 and 1x1 taps), which cuDNN runs 1.3-1.7x faster than its strided dgrad; they are never interleaved. */
+ * (2x2, 2x1, 1x2 and 1x1 taps), which cuDNN runs 1.3-1.7x faster than its strided dgrad; they are never interleaved.
+ * The four phases, y and scale 16-byte aligned. */
 int gf_blur_up_phases_nhwc(const float* p00, const float* p01, const float* p10, const float* p11, float* y, const float* scale,
                            int B, int Hout, int Wout, int C, float gain, void* stream);
 
 /* upfirdn_2d, general stride-1 form with the [1,3,3,1]^2/64 filter and symmetric zero padding `pad` in 0..3:
  * x [B,Hin,Win,C] -> y [B,Hin+2*pad-3,Win+2*pad-3,C] times `gain`.  pad 1 = use (a); pad 2 = its adjoint (the backward pass:
  * the filter is symmetric, so d/dx of a pad-p blur is a pad-(3-p) blur of the incoming gradient) and the blur in front of the
- * discriminator's stride-2 3x3 convolutions; pad 1 also serves the discriminator's 1x1 skip path.  C % 4 == 0. */
+ * discriminator's stride-2 3x3 convolutions; pad 1 also serves the discriminator's 1x1 skip path.  C % 4 == 0.
+ * x and y 16-byte aligned. */
 int gf_fir4_nhwc(const float* x, float* y, int B, int Hin, int Win, int C, int pad, float gain, void* stream);
 
 /* upfirdn_2d, use (b): 2x upsampling of an NCHW image (skip connection of the tRGB outputs):
@@ -46,7 +54,8 @@ int gf_upsample2x_nchw(const float* x, const float* add, float* y, int B, int C,
 
 /* fused_bias_act (+ the noise input of the synthesis layer):
  *   y = act(x + noise[b*noise_bstride + t] * (*strength) + bias[c]) * gain
- * act: 0 linear, 1 leaky-ReLU(0.2).  noise / strength / bias nullable.  y may alias x.  C % 4 == 0. */
+ * act: 0 linear, 1 leaky-ReLU(0.2).  noise / strength / bias nullable.  y may alias x.  C % 4 == 0.
+ * x, y and bias 16-byte aligned. */
 int gf_bias_act_nhwc(const float* x, float* y, const float* bias, const float* noise, const float* strength,
                      long long noise_bstride, int B, int HW, int C, int act, float gain, void* stream);
 
@@ -68,13 +77,13 @@ int gf_demod_coef_batch(const gf_demod_job* jobs, int n, int B, float eps, void*
 /* tRGB (SURVEY row f4): 1x1 modulated convolution WITHOUT demodulation from channels-last activations to a planar image,
  *   y[b,o,t] = sum_c x[b,t,c] * w[o*C + c] * styles[b*s_ld + c] * wscale + bias[o],   o < 3
  * (modulated_conv2d_layer(..., demodulate=False, kernel=1) + bias of the reference's torgb); x is read once.
- * C % 4 == 0, C <= 512; s_ld % 4 == 0; bias nullable. */
+ * C % 4 == 0, C <= 512; s_ld % 4 == 0; bias nullable; x, w and styles 16-byte aligned. */
 int gf_torgb_nhwc(const float* x, const float* w, const float* styles, int s_ld, const float* bias, float wscale, float* y,
                   int B, int HW, int C, void* stream);
 
 /* gf_torgb_nhwc with a second output from the same read of x: xs_out[b,t,c] = x[b,t,c] * s2[b*s2_ld + c] -- the style modulation
  * of the NEXT block's first convolution (replaces a gf_chan_scale_nhwc pass over the same tensor).  s2 / xs_out both NULL or both
- * given. */
+ * given, both 16-byte aligned. */
 int gf_torgb_scale_nhwc(const float* x, const float* w, const float* styles, int s_ld, const float* bias, float wscale, float* y,
                         const float* s2, int s2_ld, float* xs_out, int B, int HW, int C, void* stream);
 
