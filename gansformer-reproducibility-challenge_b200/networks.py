@@ -338,18 +338,40 @@ class SynthesisNetwork(nn.Module):
             self.torgbs.append(ToRGB(out_ch, latent_dim))
         self.register_buffer("fir", fir_filter())
         self.num_attention_layers = sum(1 for l in self.layers if l.attention is not None)
+        # index into per-layer latents [B, num_ws, k+1, D] of every style affine (conv layers, then tRGBs): conv layer i reads
+        # index i, the tRGB of a block reads the index after its block's last conv layer (SURVEY A.4 item 13)
+        ends = list(np.cumsum([1 if res == 4 else 2 for res in self.block_resolutions]))
+        self.ws_index: List[int] = list(range(len(self.layers))) + [int(e) for e in ends]
+
+    @property
+    def num_ws(self) -> int:
+        """Number of per-layer latent sets ``forward`` accepts: one per conv layer, plus one for the last tRGB."""
+        return len(self.layers) + 1
 
     def forward(self, ws: torch.Tensor, noise_mode: str = "const", return_att: bool = False, return_features: bool = False):
-        """return_features: also return, per attention layer, the layer's activation after noise + bias + leaky-ReLU and
+        """ws: [B, k+1, D] (every layer reads the same latents) or per-layer [B, num_ws, k+1, D] (style mixing: conv layer i
+        takes its attention latents ws[:, i, :k] and its style from ws[:, i, k]; a block's tRGB takes the index after its last
+        conv layer).  return_features: also return, per attention layer, the layer's activation after noise + bias + leaky-ReLU and
         before the next convolution's style scale, as NCHW views (parity checks against oracle.generator, which returns the
         same quantity).  The store-side fusion of the NEXT layer's style scale is switched off for such a call, so that the
         captured activations are exactly the layer outputs; everything else takes the same kernels."""
         k = self.components_num
         B = ws.shape[0]
-        y = ws[:, :k].contiguous()
-        w_glob = ws[:, k]
+        per_layer = ws.dim() == 4
+        if per_layer:
+            if ws.shape[1] != self.num_ws or ws.shape[2] != k + 1:
+                raise ValueError(f"per-layer ws must be [B, {self.num_ws}, {k + 1}, D], got {tuple(ws.shape)}")
+            wsl = ws.transpose(0, 1)                                    # [L, B, k+1, D]
+            ys = list(wsl[:, :, :k].contiguous().unbind(0))             # one copy for all layers; each [B, k, D] contiguous
+            wgs = wsl[:, :, k]                                          # [L, B, D]
+        else:
+            y = ws[:, :k].contiguous()
+            w_glob = ws[:, k]
+            ys, wgs = [y] * self.num_ws, [w_glob] * self.num_ws
         x = self.const[None].expand(B, -1, -1, -1).contiguous(memory_format=torch.channels_last)
-        # all style affines (one per conv layer and per tRGB) read the same global latent: one batched GEMM at inference
+        # all style affines (one per conv layer and per tRGB) read the same global latent: one batched GEMM at inference; with
+        # per-layer latents, the same GEMM once per latent set, of which each affine keeps its own columns (the same operand shapes
+        # as the shared-latent GEMM, so equal latent sets give its result bit for bit)
         mods = list(self.layers) + list(self.torgbs)
         aff = [m.affine for m in mods]
         aff_params = [t for a in aff for t in (a.weight, a.bias)]
@@ -359,7 +381,12 @@ class SynthesisNetwork(nn.Module):
                 ws_, bs_ = zip(*[a.effective() for a in aff])
                 return torch.cat(ws_, dim=1).contiguous(), torch.cat(bs_)
             wt_cat, b_cat = _cached(self, "affines", aff_params, cat_affines)
-            styles_all = torch.addmm(b_cat, w_glob, wt_cat).split([a.weight.shape[0] for a in aff], dim=1)
+            widths = [a.weight.shape[0] for a in aff]
+            if per_layer:
+                per_set = [torch.addmm(b_cat, wgs[i], wt_cat).split(widths, dim=1) for i in range(self.num_ws)]
+                styles_all = [per_set[i][m] for m, i in enumerate(self.ws_index)]
+            else:
+                styles_all = torch.addmm(b_cat, w_glob, wt_cat).split(widths, dim=1)
         # Stage I of every attention layer (keys / V^T / positional tables of a simplex layer, pass-A query tables + V^T of a
         # duplex layer) depends only on the latents and the styles: ONE batched launch for the whole network
         # (gf_attn_prologue_batch) instead of two small launches in front of every layer's token pass.
@@ -381,7 +408,7 @@ class SynthesisNetwork(nn.Module):
                         _, wsq_, _, _ = _cached(layer, "conv", (layer.weight,), layer._conv_weights)
                         d_ = ops.demod_coef(styles_all[li_], wsq_)
                 C_ = layer.weight.shape[0]
-                items.append((layer.attention, y, (B, layer.resolution, layer.resolution, C_), d_))
+                items.append((layer.attention, ys[li_], (B, layer.resolution, layer.resolution, C_), d_))
                 prepared[li_] = (None, d_)
             prologue_batch(items)
         img = None
@@ -420,7 +447,7 @@ class SynthesisNetwork(nn.Module):
                         rgb = torch.empty((B, 3, res, res), device=x.device, dtype=torch.float32)
                         rgb_args = dict(rgb_w=rgb_w, rgb_bias=tg.bias, rgb_out=rgb)
                         post_scale = nxt
-                x, att, cen_out = layer(x, w_glob, y, noise_mode=noise_mode, return_att=return_att, styles=styles_all[li],
+                x, att, cen_out = layer(x, wgs[li], ys[li], noise_mode=noise_mode, return_att=return_att, styles=styles_all[li],
                                         prescaled=prescaled, post_scale=post_scale, prepared=prepared[li], rgb=rgb_args,
                                         centroids_init=cen_init, demod=demods[li])
                 if layer.attention is not None:
@@ -434,7 +461,7 @@ class SynthesisNetwork(nn.Module):
             if rgb is not None:
                 block_prescaled = nxt is not None
             else:
-                rgb = self.torgbs[bi](x, w_glob, styles=styles_all[len(self.layers) + bi], next_styles=nxt)
+                rgb = self.torgbs[bi](x, wgs[self.ws_index[len(self.layers) + bi]], styles=styles_all[len(self.layers) + bi], next_styles=nxt)
                 block_prescaled = nxt is not None
                 if block_prescaled:
                     rgb, x = rgb

@@ -22,6 +22,11 @@ to the dlatents ws [B, k+1, D], its length over the k+1 latent components (SURVE
 length to its running mean.  The backward of that gradient needs the generator's second derivative: the attention layers give it
 through the double-backward kernels (``gf_attn_simplex_bwd_vjp_ex``, with the forward's dropout mask) or, on the composite route, torch
 autograd.  Off by default.  Augmentation is out of scope.
+
+``TrainConfig.style_mixing > 0`` adds StyleGAN2's style mixing (SURVEY A.4 item 13): each generator forward of the D and G phases
+maps z and a second draw z2, and feeds the synthesis per-layer latents that switch from the first to the second at a cutoff drawn
+per minibatch on the device (``mixing_cutoff``, ``mix_latents``).  The path-length phase, the w_avg update and inference do not
+mix.  Off by default: with 0 the step makes the same calls and draws the same random numbers as without the option.
 """
 from __future__ import annotations
 
@@ -192,6 +197,22 @@ class TrainConfig:
     g_reg_interval: int = 4             # lazy path-length regularisation: every 4th generator step
     pl_batch_shrink: int = 2            # the path-length phase runs on the first B // 2 latents
     pl_decay: float = 0.01              # decay of the running mean of the path lengths
+    style_mixing: float = 0.0           # probability of style mixing per generator forward (StyleGAN2 / GANsformer: 0.9); 0 = off
+
+
+def mixing_cutoff(p: float, num_ws: int, device) -> torch.Tensor:
+    """The style-mixing cutoff of one minibatch as a 0-d int64 tensor on ``device``, drawn without a host sync: with probability
+    ``p`` uniform in [1, num_ws - 1], else num_ws (no mixing).  ``p == 0`` draws no random number and returns num_ws."""
+    no_mix = torch.full((), num_ws, dtype=torch.int64, device=device)
+    if p <= 0.0:
+        return no_mix
+    return torch.where(torch.rand((), device=device) < p, torch.randint(1, num_ws, (), device=device), no_mix)
+
+
+def mix_latents(ws1: torch.Tensor, ws2: torch.Tensor, cutoff: torch.Tensor, num_ws: int) -> torch.Tensor:
+    """Per-layer latents [B, num_ws, k+1, D] from two mapping outputs [B, k+1, D]: index i takes ws1 where i < cutoff, else ws2."""
+    first = torch.arange(num_ws, device=ws1.device) < cutoff
+    return torch.where(first[None, :, None, None], ws1[:, None], ws2[:, None])
 
 
 @dataclass
@@ -211,6 +232,10 @@ class Trainer:
 
     def __init__(self, G: nn.Module, D: nn.Module, cfg: Optional[TrainConfig] = None, world: int = 1):
         self.G, self.D, self.cfg, self.world = G, D, cfg or TrainConfig(), world
+        if not 0.0 <= self.cfg.style_mixing <= 1.0:
+            raise ValueError(f"style_mixing must be in [0, 1], got {self.cfg.style_mixing}")
+        if self.cfg.style_mixing > 0 and not (hasattr(G, "mapping") and hasattr(G, "synthesis")):
+            raise ValueError("style_mixing needs a generator with `mapping` and `synthesis`")
         self.G_ema = copy.deepcopy(G).eval().requires_grad_(False)
         c = self.cfg.d_reg_interval / (self.cfg.d_reg_interval + 1.0)  # lazy regularisation: rescale lr and betas
         cap = next(G.parameters()).is_cuda                              # capturable: the step can be replayed from a CUDA graph
@@ -236,15 +261,17 @@ class Trainer:
 
     def _step_tensors(self, z: torch.Tensor, reals: torch.Tensor, do_r1: bool, stats: Optional[StepStats] = None,
                       do_pl: bool = False):
-        """One D update + one G update (+ the path-length update with ``do_pl``); returns (loss_d, loss_g, r1, pl_penalty) as device
-        tensors without synchronising (capturable); pl_penalty is None without ``do_pl``."""
+        """One D update + one G update (+ the path-length update with ``do_pl``); returns (loss_d, loss_g, r1, pl_penalty, cutoffs) as
+        device tensors without synchronising (capturable); pl_penalty is None without ``do_pl``; cutoffs maps the StepStats.extra
+        names of the style-mixing cutoffs of the D and G phases to them (empty without style mixing)."""
         G, D, cfg = self.G, self.D, self.cfg
         stats = stats if stats is not None else StepStats()
+        cutoffs: Dict[str, torch.Tensor] = {}
         # ---- discriminator: logistic loss (+ lazy R1 on the reals)
         G.requires_grad_(False); D.requires_grad_(True)
         self._zero(self.opt_d, self.buckets_d)
         with torch.no_grad():
-            fakes = G(z, noise_mode=cfg.noise_mode)
+            fakes = self._generate(z, cutoffs, "d")
         reals_in = reals.detach().requires_grad_(do_r1)
         logit_real, logit_fake = D(reals_in), D(fakes)
         loss_d = F.softplus(logit_fake).mean() + F.softplus(-logit_real).mean()
@@ -262,7 +289,7 @@ class Trainer:
             advance_dropout(z.device)                 # attention dropout: fresh masks for the G phase (device-side, capturable)
         G.requires_grad_(True); D.requires_grad_(False)
         self._zero(self.opt_g, self.buckets_g)
-        loss_g = F.softplus(-D(G(z, noise_mode=cfg.noise_mode))).mean()
+        loss_g = F.softplus(-D(self._generate(z, cutoffs, "g"))).mean()
         loss_g.backward()
         self._allreduce(self.buckets_g, stats)
         self.opt_g.step()
@@ -281,7 +308,20 @@ class Trainer:
                 pe.lerp_(p.detach(), 1.0 - beta)
             for be, b in zip(self.G_ema.buffers(), G.buffers()):
                 be.copy_(b)
-        return loss_d.detach(), loss_g.detach(), r1.detach(), pl_penalty
+        return loss_d.detach(), loss_g.detach(), r1.detach(), pl_penalty, cutoffs
+
+    def _generate(self, z: torch.Tensor, cutoffs: Dict[str, torch.Tensor], phase: str) -> torch.Tensor:
+        """The fakes of one phase: G(z), or with style mixing (SURVEY A.4 item 13) the synthesis of per-layer latents that switch
+        from G.mapping(z) to the mapping of a second draw at a cutoff of their own.  Device-side throughout (capturable)."""
+        G, cfg = self.G, self.cfg
+        if cfg.style_mixing <= 0.0:
+            return G(z, noise_mode=cfg.noise_mode)
+        num_ws = G.synthesis.num_ws
+        z2 = torch.randn_like(z)
+        ws1, ws2 = G.mapping(z), G.mapping(z2)
+        cutoff = mixing_cutoff(cfg.style_mixing, num_ws, z.device)
+        cutoffs["style_mixing_cutoff_" + phase] = cutoff
+        return G.synthesis(mix_latents(ws1, ws2, cutoff, num_ws), noise_mode=cfg.noise_mode)
 
     def _pl_phase(self, z: torch.Tensor, stats: StepStats) -> torch.Tensor:
         """The lazy path-length update of G (StyleGAN2): returns the penalty as a device tensor (capturable: no host sync, the
@@ -309,8 +349,10 @@ class Trainer:
     def _do_pl(self) -> bool:
         return self.cfg.pl_weight > 0 and self.it % self.cfg.g_reg_interval == 0
 
-    def _finish_stats(self, stats: StepStats, loss_d, loss_g, r1, pl_penalty) -> StepStats:
+    def _finish_stats(self, stats: StepStats, loss_d, loss_g, r1, pl_penalty, cutoffs) -> StepStats:
         stats.loss_d, stats.loss_g, stats.r1 = float(loss_d), float(loss_g), float(r1)
+        for name, cutoff in cutoffs.items():
+            stats.extra[name] = float(cutoff)
         if pl_penalty is not None:
             stats.pl_penalty = float(pl_penalty)
         if self.pl_mean is not None:
