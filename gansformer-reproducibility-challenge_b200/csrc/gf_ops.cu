@@ -405,6 +405,107 @@ __global__ void __launch_bounds__(MAP_WARPS * 32) mapping_kernel(const float* __
   }
 }
 
+// Class-conditional G_mapping (SURVEY A.4 item 14): mapping_kernel with the label embedding e_b = c_b E concatenated to every
+// latent of image b = row / (k+1) before the pixel norm, so layer 0 has fan-in 2D.  A warp computes e_b itself: its lanes load 32
+// labels at a time, and the nonzero ones (a warp-uniform ballot) add their row of E in ascending order, read through L2.  Layer 0
+// reads its latent half [D][D] from shared memory and its label half from L2; layers 1..L-1 are staged as in mapping_kernel.
+__global__ void __launch_bounds__(MAP_WARPS * 32) mapping_cond_kernel(const float* __restrict__ z, const float* __restrict__ c, int c_dim,
+                                                                      const float* __restrict__ E, const float* __restrict__ W0,
+                                                                      const float* __restrict__ Wt, const float* __restrict__ bias,
+                                                                      const float* __restrict__ w_avg, float psi, float* __restrict__ out,
+                                                                      int rows, int k, int D, int L) {
+  extern __shared__ float msm[];
+  const int DD = D * D;
+  float* W0s = msm;                                  // [2][D][D]: rows 0..D-1 (the latent half) of each path's [2D][D]
+  float* Ws = W0s + (size_t)2 * DD;                  // [2][L-1][D][D]
+  float* bs = Ws + (size_t)2 * (L - 1) * DD;         // [2][L][D]
+  float* xs = bs + (size_t)2 * L * D;                // [MAP_WARPS][2D]
+  for (int i = threadIdx.x; i < 2 * DD; i += blockDim.x) W0s[i] = W0[(size_t)(i / DD) * 2 * DD + i % DD];
+  for (int i = threadIdx.x; i < 2 * (L - 1) * DD; i += blockDim.x) Ws[i] = Wt[i];
+  for (int i = threadIdx.x; i < 2 * L * D; i += blockDim.x) bs[i] = bias[i];
+  __syncthreads();
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  float* x = xs + warp * 2 * D;
+  const int nm = (D + 31) >> 5;
+  for (int row = blockIdx.x * MAP_WARPS + warp; row < rows; row += gridDim.x * MAP_WARPS) {
+    const int b = row / (k + 1), comp = row % (k + 1);
+    const int path = comp == k ? 1 : 0;              // the last latent of every sample is the global one
+    // e_b = c_b . E
+    float e[MAP_MAXM];
+#pragma unroll
+    for (int m = 0; m < MAP_MAXM; ++m) e[m] = 0.f;
+    const float* cb = c + (size_t)b * c_dim;
+    for (int j0 = 0; j0 < c_dim; j0 += 32) {
+      const float cv = j0 + lane < c_dim ? cb[j0 + lane] : 0.f;
+      unsigned nz = __ballot_sync(0xffffffffu, cv != 0.f);
+      while (nz) {
+        const int s = __ffs(nz) - 1;
+        nz &= nz - 1;
+        const float cj = __shfl_sync(0xffffffffu, cv, s);
+        const float* Er = E + (size_t)(j0 + s) * D;
+#pragma unroll
+        for (int m = 0; m < MAP_MAXM; ++m) if (m < nm && lane + 32 * m < D) e[m] = fmaf(cj, __ldg(Er + lane + 32 * m), e[m]);
+      }
+    }
+    // pixel norm of [z || e]: x * rsqrt(mean over the 2D entries of x^2 + 1e-8)
+    float v[MAP_MAXM], ss = 0.f;
+#pragma unroll
+    for (int m = 0; m < MAP_MAXM; ++m) {
+      const int o = lane + 32 * m;
+      v[m] = (m < nm && o < D) ? z[(size_t)row * D + o] : 0.f;
+      ss = fmaf(v[m], v[m], ss);
+      ss = fmaf(e[m], e[m], ss);
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) ss += __shfl_xor_sync(0xffffffffu, ss, o);
+    const float rn = rsqrtf(ss / (float)(2 * D) + 1e-8f);
+#pragma unroll
+    for (int m = 0; m < MAP_MAXM; ++m) if (m < nm && lane + 32 * m < D) { x[lane + 32 * m] = v[m] * rn; x[D + lane + 32 * m] = e[m] * rn; }
+    __syncwarp();
+    for (int l = 0; l < L; ++l) {
+      const float* bb = bs + ((size_t)path * L + l) * D;
+      float acc[MAP_MAXM];
+#pragma unroll
+      for (int m = 0; m < MAP_MAXM; ++m) acc[m] = (m < nm && lane + 32 * m < D) ? bb[lane + 32 * m] : 0.f;
+      if (l == 0) {
+        const float* W = W0s + (size_t)path * DD;
+        const float* We = W0 + ((size_t)path * 2 + 1) * DD;     // the label half of layer 0
+        for (int i = 0; i < D; ++i) {
+          const float xi = x[i];
+#pragma unroll
+          for (int m = 0; m < MAP_MAXM; ++m) if (m < nm && lane + 32 * m < D) acc[m] = fmaf(xi, W[(size_t)i * D + lane + 32 * m], acc[m]);
+        }
+        for (int i = 0; i < D; ++i) {
+          const float xi = x[D + i];
+#pragma unroll
+          for (int m = 0; m < MAP_MAXM; ++m) if (m < nm && lane + 32 * m < D) acc[m] = fmaf(xi, __ldg(We + (size_t)i * D + lane + 32 * m), acc[m]);
+        }
+      } else {
+        const float* W = Ws + ((size_t)path * (L - 1) + (l - 1)) * DD;
+        for (int i = 0; i < D; ++i) {
+          const float xi = x[i];
+#pragma unroll
+          for (int m = 0; m < MAP_MAXM; ++m) if (m < nm && lane + 32 * m < D) acc[m] = fmaf(xi, W[(size_t)i * D + lane + 32 * m], acc[m]);
+        }
+      }
+      __syncwarp();
+#pragma unroll
+      for (int m = 0; m < MAP_MAXM; ++m) if (m < nm && lane + 32 * m < D) x[lane + 32 * m] = fmaxf(acc[m], 0.2f * acc[m]);
+      __syncwarp();
+    }
+#pragma unroll
+    for (int m = 0; m < MAP_MAXM; ++m) {
+      const int o = lane + 32 * m;
+      if (m < nm && o < D) {
+        float r = x[o];
+        if (w_avg) { const float a = w_avg[path * D + o]; r = a + psi * (r - a); }      // one label-agnostic w_avg
+        out[(size_t)row * D + o] = r;
+      }
+    }
+    __syncwarp();
+  }
+}
+
 extern "C" {
 
 int gf_chan_scale_nhwc(const float* x, const float* s, int s_ld, float* y, int B, int HW, int C, void* stream) {
@@ -559,6 +660,27 @@ int gf_mapping_fwd(const float* z, const float* w, const float* b, const float* 
   int grid = (rows + MAP_WARPS - 1) / MAP_WARPS;
   if (grid > num_sms()) grid = num_sms();
   mapping_kernel<<<grid, MAP_WARPS * 32, smem, (cudaStream_t)stream>>>(z, w, b, w_avg, psi, out, rows, k, D, L);
+  GF_LAUNCH_OK();
+  return GF_OK;
+}
+
+int gf_mapping_fwd_cond(const float* z, const float* c, int c_dim, const float* E, const float* w0, const float* w, const float* b,
+                        const float* w_avg, float psi, float* out, int B, int k, int D, int L, void* stream) {
+  if (!z || !c || !E || !w0 || !b || !out || (L > 1 && !w)) { set_error("gf_mapping_fwd_cond: null pointer"); return GF_ERR_INVALID; }
+  if (B <= 0 || k < 0 || D <= 0 || L <= 0 || c_dim < 1) {
+    set_error("gf_mapping_fwd_cond: bad sizes B=%d k=%d D=%d L=%d c_dim=%d", B, k, D, L, c_dim); return GF_ERR_INVALID;
+  }
+  if (D > 32 * MAP_MAXM) { set_error("gf_mapping_fwd_cond: latent width D=%d > %d is not served by the fused kernel", D, 32 * MAP_MAXM); return GF_ERR_UNSUPPORTED; }
+  const size_t smem = ((size_t)2 * L * D * D + (size_t)2 * L * D + (size_t)MAP_WARPS * 2 * D) * sizeof(float);
+  int dev = 0, optin = 0;
+  GF_CUDA_OK(cudaGetDevice(&dev));
+  GF_CUDA_OK(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
+  if (smem > (size_t)optin) { set_error("gf_mapping_fwd_cond: 2*L*D*D weights (%zu bytes) do not fit shared memory", smem); return GF_ERR_UNSUPPORTED; }
+  GF_CUDA_OK(cudaFuncSetAttribute(mapping_cond_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  const int rows = B * (k + 1);
+  int grid = (rows + MAP_WARPS - 1) / MAP_WARPS;
+  if (grid > num_sms()) grid = num_sms();
+  mapping_cond_kernel<<<grid, MAP_WARPS * 32, smem, (cudaStream_t)stream>>>(z, c, c_dim, E, w0, w, b, w_avg, psi, out, rows, k, D, L);
   GF_LAUNCH_OK();
   return GF_OK;
 }

@@ -152,27 +152,65 @@ class MappingNetwork(nn.Module):
     ``ltnt2ltnt=True`` (upstream's latent-to-latent option, SURVEY 2.2 / row f4): after every fully connected layer the k local
     latents attend to each other -- the same bipartite block as in the synthesis network (``BipartiteAttention`` with the
     latents as both the "grid" [B, k, 1, D] and the attended set, no positional encoding, integration / norm as given), so it runs
-    on the same C-ABI kernels (C = D = 32: the CUDA-core kernel).  Off by default, as in the benchmarked configurations."""
+    on the same C-ABI kernels (C = D = 32: the CUDA-core kernel).  Off by default, as in the benchmarked configurations.
+
+    ``c_dim > 0`` makes the mapping class-conditional (SURVEY A.4 item 14, StyleGAN2's label concatenation): a label embedding
+    ``embed`` [c_dim, D] (N(0, 1), no equalised-LR gain), e_b = c_b embed concatenated to every latent of image b before the pixel
+    norm, and layer 0 of both MLPs with fan-in 2D.  Truncation keeps the one label-agnostic w_avg.  ``c_dim = 0`` (the default)
+    builds exactly the unconditional network and ignores ``c``."""
 
     def __init__(self, latent_dim: int, components_num: int, num_layers: int = 8, lr_mul: float = 0.01, ltnt2ltnt: bool = False,
-                 integration: str = "mul", norm: Optional[str] = "layer", exact_fp32: bool = False):
+                 integration: str = "mul", norm: Optional[str] = "layer", exact_fp32: bool = False, c_dim: int = 0):
         super().__init__()
-        self.latent_dim, self.components_num = latent_dim, components_num
-        self.local = nn.ModuleList([FullyConnected(latent_dim, latent_dim, lr_mul=lr_mul, act="lrelu") for _ in range(num_layers)])
-        self.glob = nn.ModuleList([FullyConnected(latent_dim, latent_dim, lr_mul=lr_mul, act="lrelu") for _ in range(num_layers)])
+        if c_dim < 0:
+            raise ValueError(f"c_dim must be >= 0, got {c_dim}")
+        self.latent_dim, self.components_num, self.c_dim = latent_dim, components_num, int(c_dim)
+        fan0 = 2 * latent_dim if c_dim > 0 else latent_dim           # layer 0 reads [z || e] when conditional
+        self.local = nn.ModuleList([FullyConnected(fan0 if i == 0 else latent_dim, latent_dim, lr_mul=lr_mul, act="lrelu")
+                                    for i in range(num_layers)])
+        self.glob = nn.ModuleList([FullyConnected(fan0 if i == 0 else latent_dim, latent_dim, lr_mul=lr_mul, act="lrelu")
+                                   for i in range(num_layers)])
         self.register_buffer("w_avg", torch.zeros(2, latent_dim))
         self.self_att = None
         if ltnt2ltnt and components_num > 1:
             self.self_att = nn.ModuleList([BipartiteAttention(latent_dim, latent_dim, components_num, pos_dim=latent_dim, use_pos=False,
                                                               integration=integration, norm=norm, exact_fp32=exact_fp32)
                                            for _ in range(num_layers)])
+        if c_dim > 0:
+            self.embed = nn.Parameter(torch.randn(c_dim, latent_dim))
 
-    def forward(self, z: torch.Tensor, truncation_psi: float = 1.0) -> torch.Tensor:
+    def labels(self, c: Optional[torch.Tensor], batch: int, like: torch.Tensor) -> Optional[torch.Tensor]:
+        """The labels of a call as a [batch, c_dim] tensor of `like`'s dtype, or None for an unconditional network (which ignores c).
+        Raises ValueError when the network is conditional and c is missing or has the wrong shape."""
+        if self.c_dim == 0:
+            return None
+        if c is None:
+            raise ValueError(f"this network is conditional (c_dim={self.c_dim}): labels c [B, {self.c_dim}] are required")
+        c = torch.as_tensor(c)
+        if c.dim() != 2 or c.shape[0] != batch or c.shape[1] != self.c_dim:
+            raise ValueError(f"c must be [{batch}, {self.c_dim}], got {tuple(c.shape)}")
+        return c.to(device=like.device, dtype=like.dtype)
+
+    def forward(self, z: torch.Tensor, c: Optional[torch.Tensor] = None, truncation_psi: float = 1.0) -> torch.Tensor:
         k = self.components_num
         if z.dim() != 3 or z.shape[1] != k + 1 or z.shape[2] != self.latent_dim:
             raise ValueError(f"z must be [B, {k + 1}, {self.latent_dim}], got {tuple(z.shape)}")
+        c = self.labels(c, z.shape[0], z)
         params = [t for fc in list(self.local) + list(self.glob) for t in (fc.weight, fc.bias)]
-        if (self.self_att is None and z.is_cuda and z.dtype == torch.float32 and _inference(*params) and self.latent_dim <= 128
+        if c is not None and (self.self_att is None and z.is_cuda and z.dtype == torch.float32 and _inference(*params, self.embed)
+                              and self.latent_dim <= 128 and len(self.local) * self.latent_dim ** 2 * 8 <= 200 * 1024
+                              and not os.environ.get("GF_NO_MAPPING_KERNEL")):
+            # inference: the conditional mapping network is ONE kernel too (gf_mapping_fwd_cond): layer 0 [2, 2D, D], the rest
+            # [2, L-1, D, D]; cached until a parameter (the embedding included) changes
+            def stack_cond():
+                wl, bl = zip(*[fc.effective() for fc in self.local])
+                wg, bg = zip(*[fc.effective() for fc in self.glob])
+                w0 = torch.stack([wl[0], wg[0]]).contiguous()
+                rest = torch.stack([torch.stack(wl[1:]), torch.stack(wg[1:])]).contiguous() if len(wl) > 1 else None
+                return w0, rest, torch.stack([torch.stack(bl), torch.stack(bg)]).contiguous()
+            w0, w_rest, b_eff = _cached(self, "stack_cond", params + [self.embed], stack_cond)
+            return ops.mapping_fwd(z, w_rest, b_eff, self.w_avg, float(truncation_psi), k, c=c, embed=self.embed, w0=w0)
+        if (c is None and self.self_att is None and z.is_cuda and z.dtype == torch.float32 and _inference(*params) and self.latent_dim <= 128
                 and len(self.local) * self.latent_dim ** 2 * 8 <= 200 * 1024 and not os.environ.get("GF_NO_MAPPING_KERNEL")):
             # inference: the whole mapping network is ONE kernel (gf_mapping_fwd); effective weights cached until a parameter changes
             def stack():
@@ -181,6 +219,9 @@ class MappingNetwork(nn.Module):
                 return (torch.stack([torch.stack(wl), torch.stack(wg)]).contiguous(), torch.stack([torch.stack(bl), torch.stack(bg)]).contiguous())
             w_eff, b_eff = _cached(self, "stack", params, stack)
             return ops.mapping_fwd(z, w_eff, b_eff, self.w_avg, float(truncation_psi), k)
+        if c is not None:                           # [z || c embed], normalised over its 2D entries
+            e = c @ self.embed
+            z = torch.cat([z, e[:, None].expand(-1, k + 1, -1)], dim=2)
         z = z * torch.rsqrt(z.square().mean(dim=2, keepdim=True) + 1e-8)
         loc, glo = z[:, :k], z[:, k:]
         for i, fc in enumerate(self.local):
@@ -471,14 +512,17 @@ class SynthesisNetwork(nn.Module):
 
 
 class Generator(nn.Module):
-    """G_GANsformer.  ``G(z, c=None, truncation_psi=1.0, noise_mode='const', return_att=False) -> img [B,3,R,R]``."""
+    """G_GANsformer.  ``G(z, c=None, truncation_psi=1.0, noise_mode='const', return_att=False) -> img [B,3,R,R]``.
+
+    ``c_dim > 0``: class-conditional (SURVEY A.4 item 14).  Every call then takes labels c [B, c_dim] (one-hot or any real weights),
+    which act through the mapping network's label embedding only; with the default ``c_dim = 0`` c is ignored."""
 
     def __init__(self, resolution: int = 256, components_num: int = 16, latent_size: int = 512, latent_dim: Optional[int] = None,
                  transformer: bool = True, g_start_res: int = 8, g_end_res: Optional[int] = None, kmeans: bool = False,
                  kmeans_iters: int = 1, iterative: bool = False, integration: str = "mul", norm: Optional[str] = "layer",
                  use_pos: bool = True, pos_dim: Optional[int] = None, num_heads: int = 1, mapping_layers: int = 8,
                  fmap_base: int = 16384, fmap_max: int = 512, exact_fp32: bool = False, ltnt2ltnt: bool = False, g_img2ltnt: bool = False,
-                 att_dp: float = 0.0):
+                 att_dp: float = 0.0, c_dim: int = 0):
         super().__init__()
         # SURVEY A.4 item 1: D = latent_size // components_num unless given
         self.latent_dim = latent_dim if latent_dim is not None else max(latent_size // max(components_num, 1), 1)
@@ -487,14 +531,15 @@ class Generator(nn.Module):
                            kmeans_iters=kmeans_iters, use_pos=use_pos, exact_fp32=exact_fp32, iterative=iterative,
                            img2ltnt=bool(g_img2ltnt and kmeans), att_dp=att_dp)
         self.mapping = MappingNetwork(self.latent_dim, components_num, num_layers=mapping_layers, ltnt2ltnt=ltnt2ltnt,
-                                      integration=integration, norm=norm, exact_fp32=exact_fp32)
+                                      integration=integration, norm=norm, exact_fp32=exact_fp32, c_dim=c_dim)
+        self.c_dim = int(c_dim)
         self.synthesis = SynthesisNetwork(resolution, self.latent_dim, components_num, fmap_base=fmap_base, fmap_max=fmap_max,
                                           g_start_res=g_start_res, g_end_res=g_end_res, transformer=transformer,
                                           attn_kwargs=attn_kwargs)
 
     def forward(self, z: torch.Tensor, c=None, truncation_psi: float = 1.0, noise_mode: str = "const", return_att: bool = False,
                 return_features: bool = False):
-        ws = self.mapping(z, truncation_psi=truncation_psi)
+        ws = self.mapping(z, c, truncation_psi=truncation_psi)
         return self.synthesis(ws, noise_mode=noise_mode, return_att=return_att, return_features=return_features)
 
     def __deepcopy__(self, memo):
@@ -520,7 +565,8 @@ class Generator(nn.Module):
     # ------------------------------------------------------------------------------------------------------------
     @torch.no_grad()
     def graphed(self, batch_size: int, truncation_psi: float = 1.0, noise_mode: str = "const"):
-        """Returns ``fn(z_device) -> img`` replaying a captured CUDA graph of ``self(z)`` for this batch size.
+        """Returns ``fn(z_device, c_device=None) -> img`` replaying a captured CUDA graph of ``self(z, c)`` for this batch size (the
+        labels go through a static buffer of their own; an unconditional generator ignores them).
 
         The returned image tensor is a static buffer overwritten by the next replay.  Weight-derived tensors (folded
         attention weights, scaled conv weights) are baked at capture, so the graph is keyed on the parameters' storage,
@@ -535,17 +581,22 @@ class Generator(nn.Module):
         if dev.type != "cuda":
             raise RuntimeError("CUDA graphs need the generator on a CUDA device")
         static_z = torch.zeros(batch_size, self.components_num + 1, self.latent_dim, device=dev)
+        static_c = torch.zeros(batch_size, self.c_dim, device=dev) if self.c_dim > 0 else None
         side = torch.cuda.Stream(device=dev)
         side.wait_stream(torch.cuda.current_stream(dev))
         with torch.cuda.stream(side):
             for _ in range(3):                      # warm-up: cuDNN autotune, weight folding, workspace allocation
-                self(static_z, truncation_psi=truncation_psi, noise_mode=noise_mode)
+                self(static_z, static_c, truncation_psi=truncation_psi, noise_mode=noise_mode)
         torch.cuda.current_stream(dev).wait_stream(side)
         graph = torch.cuda.CUDAGraph()
         with torch.cuda.graph(graph):
-            static_img = self(static_z, truncation_psi=truncation_psi, noise_mode=noise_mode)
+            static_img = self(static_z, static_c, truncation_psi=truncation_psi, noise_mode=noise_mode)
 
-        def replay(z: torch.Tensor) -> torch.Tensor:
+        labels = self.mapping.labels        # not `self`: the cached closure must not keep the generator (and its graphs) alive
+
+        def replay(z: torch.Tensor, c: Optional[torch.Tensor] = None) -> torch.Tensor:
+            if static_c is not None:
+                static_c.copy_(labels(c, batch_size, static_c), non_blocking=True)
             static_z.copy_(z, non_blocking=True)
             graph.replay()
             return static_img
@@ -558,16 +609,21 @@ class Generator(nn.Module):
             cuda_graph: bool = False, out: Optional[torch.Tensor] = None):
         """``Gs.run``-shaped convenience wrapper (reference: dnnlib/tflib/network.py Network.run): host numpy/tensor
         latents in, host images out, processed in minibatches on this module's device.  ``cuda_graph=True`` replays a
-        captured graph for full minibatches; ``out`` may be a (pinned) host tensor to receive the images."""
+        captured graph for full minibatches; ``out`` may be a (pinned) host tensor to receive the images.  ``labels`` [N, c_dim]
+        go with the latents, minibatch by minibatch (required iff c_dim > 0; ignored otherwise)."""
         dev = next(self.parameters()).device
         lat = torch.as_tensor(np.asarray(latents) if not torch.is_tensor(latents) else latents, dtype=torch.float32)
         n = lat.shape[0]
+        lab = None
+        if self.c_dim > 0:
+            lab = self.mapping.labels(labels if labels is None or torch.is_tensor(labels) else np.asarray(labels), n, lat)
+        cs = lambda i, m: None if lab is None else lab[i:i + m].to(dev, non_blocking=True)
         noise_mode = "random" if randomize_noise else "const"
         res = out if out is not None else torch.empty((n, 3, self.resolution, self.resolution), dtype=torch.float32)
         if dev.type != "cuda":
             for i in range(0, n, minibatch_size):
                 z = lat[i:i + minibatch_size].to(dev)
-                res[i:i + z.shape[0]].copy_(self(z, truncation_psi=truncation_psi, noise_mode=noise_mode))
+                res[i:i + z.shape[0]].copy_(self(z, cs(i, z.shape[0]), truncation_psi=truncation_psi, noise_mode=noise_mode))
             return res
         # CUDA: the device->host copy of minibatch i runs on a copy stream while minibatch i+1 computes (two staging buffers;
         # effective with pinned `out` / latents)
@@ -583,10 +639,11 @@ class Generator(nn.Module):
         for idx, i in enumerate(range(0, n, minibatch_size)):
             z = lat[i:i + minibatch_size].to(dev, non_blocking=True)
             m = z.shape[0]
+            c = cs(i, m)
             if cuda_graph and m == minibatch_size:
-                img = self.graphed(minibatch_size, truncation_psi, noise_mode)(z)
+                img = self.graphed(minibatch_size, truncation_psi, noise_mode)(z, c)
             else:
-                img = self(z, truncation_psi=truncation_psi, noise_mode=noise_mode)
+                img = self(z, c, truncation_psi=truncation_psi, noise_mode=noise_mode)
             sidx = idx & 1
             if d2h_done[sidx] is not None:
                 main.wait_event(d2h_done[sidx])                 # the copy that last read this staging buffer has finished

@@ -314,13 +314,28 @@ def torgb(x: torch.Tensor, weight: torch.Tensor, styles: torch.Tensor, bias: Opt
     return rgb if next_styles is None else (rgb, x * next_styles[:, :, None, None].to(x.dtype))
 
 
-def mapping_fwd(z: torch.Tensor, w_eff: torch.Tensor, b_eff: torch.Tensor, w_avg: Optional[torch.Tensor], psi: float, k: int) -> torch.Tensor:
+def mapping_fwd(z: torch.Tensor, w_eff: torch.Tensor, b_eff: torch.Tensor, w_avg: Optional[torch.Tensor], psi: float, k: int,
+                c: Optional[torch.Tensor] = None, embed: Optional[torch.Tensor] = None, w0: Optional[torch.Tensor] = None) -> torch.Tensor:
     """G_mapping in one launch (gf_mapping_fwd): z [B, k+1, D]; w_eff [2, L, D, D] ([in, out], gains folded), b_eff [2, L, D];
-    w_avg [2, D] (applied with psi when psi != 1).  CUDA fp32 inference only -- the module keeps the torch form for autograd."""
+    w_avg [2, D] (applied with psi when psi != 1).  CUDA fp32 inference only -- the module keeps the torch form for autograd.
+
+    With labels c [B, c_dim] (gf_mapping_fwd_cond): embed [c_dim, D] is the label embedding, w0 [2, 2D, D] the effective layer 0
+    and w_eff [2, L-1, D, D] the layers after it (L = b_eff.shape[1])."""
     B, kp1, D = z.shape
-    L = w_eff.shape[1]
     out = torch.empty_like(z)
     wa = w_avg.contiguous() if (w_avg is not None and psi != 1.0) else None
+    if c is not None:
+        if embed is None or w0 is None:
+            raise ValueError("mapping_fwd with labels needs the label embedding and the layer-0 weight w0")
+        L = b_eff.shape[1]
+        cc, ec = c.contiguous(), embed.contiguous()
+        with torch.cuda.device(z.device):
+            _lib.check(_lib.load().gf_mapping_fwd_cond(z.contiguous().data_ptr(), cc.data_ptr(), cc.shape[1], ec.data_ptr(), w0.data_ptr(),
+                                                       w_eff.data_ptr() if L > 1 else None, b_eff.data_ptr(),
+                                                       wa.data_ptr() if wa is not None else None, float(psi), out.data_ptr(), B, k, D, L,
+                                                       _stream(z.device)), "gf_mapping_fwd_cond")
+        return out
+    L = w_eff.shape[1]
     with torch.cuda.device(z.device):
         _lib.check(_lib.load().gf_mapping_fwd(z.contiguous().data_ptr(), w_eff.data_ptr(), b_eff.data_ptr(), wa.data_ptr() if wa is not None else None,
                                               float(psi), out.data_ptr(), B, k, D, L, _stream(z.device)), "gf_mapping_fwd")

@@ -27,6 +27,11 @@ autograd.  Off by default.  Augmentation is out of scope.
 maps z and a second draw z2, and feeds the synthesis per-layer latents that switch from the first to the second at a cutoff drawn
 per minibatch on the device (``mixing_cutoff``, ``mix_latents``).  The path-length phase, the w_avg update and inference do not
 mix.  Off by default: with 0 the step makes the same calls and draws the same random numbers as without the option.
+
+Class-conditional training (SURVEY A.4 item 14): a generator and a discriminator built with the same ``c_dim > 0`` take labels.
+``step(z, reals, gen_c, real_c)``: the fakes of both phases, the path-length phase (on gen_c[:B']), both style-mixing draws and the
+w_avg update use gen_c, the discriminator's real logits and R1 use real_c.  The labels are sharded like z and reals.  With
+``c_dim = 0`` the labels are ignored and the step makes the same calls as before.
 """
 from __future__ import annotations
 
@@ -140,14 +145,19 @@ class Discriminator(nn.Module):
     both require grad under grad mode (the R1 pass), they run ``composite_forward`` instead, which has a second derivative.
     ``r1_kernels=True`` keeps the R1 pass on the kernels: the kernel backward, run with create_graph=True, is differentiated by
     the double-backward kernels, and only each layer's input and incoming gradient are kept for the second pass instead of the
-    composite's [B,n,C] projections.  The R1 gradients then differ from the default route by round-off."""
+    composite's [B,n,C] projections.  The R1 gradients then differ from the default route by round-off.
+
+    ``c_dim > 0`` (SURVEY A.4 item 14, StyleGAN2's projection discriminator): fc1 has c_dim outputs and ``D(img, c)`` returns the
+    sum over them weighted by the labels c [B, c_dim].  ``c_dim = 0`` (the default) is the unconditional network, and ignores c."""
 
     def __init__(self, resolution: int = 256, fmap_base: int = 16384, fmap_max: int = 512, mbstd_group: int = 4,
                  transformer: bool = False, components_num: int = 16, latent_dim: int = 32, d_start_res: int = 8,
                  d_end_res: Optional[int] = None, integration: str = "mul", norm: Optional[str] = "layer", use_pos: bool = True,
-                 exact_fp32: bool = False, r1_kernels: bool = False):
+                 exact_fp32: bool = False, r1_kernels: bool = False, c_dim: int = 0):
         super().__init__()
-        self.resolution, self.mbstd_group, self.transformer = resolution, mbstd_group, transformer
+        if c_dim < 0:
+            raise ValueError(f"c_dim must be >= 0, got {c_dim}")
+        self.resolution, self.mbstd_group, self.transformer, self.c_dim = resolution, mbstd_group, transformer, int(c_dim)
         log2 = int(math.log2(resolution))
         d_end_res = resolution if d_end_res is None else d_end_res
         att = dict(components_num=components_num, latent_dim=latent_dim, integration=integration, norm=norm, use_pos=use_pos,
@@ -159,11 +169,17 @@ class Discriminator(nn.Module):
         c4 = nf(4, fmap_base, fmap_max)
         self.conv4 = EqConv2d(c4 + 1, c4, 3)
         self.fc0 = FullyConnected(c4 * 16 + (components_num * latent_dim if transformer else 0), c4, act="lrelu")
-        self.fc1 = FullyConnected(c4, 1)
+        self.fc1 = FullyConnected(c4, max(c_dim, 1))
         if transformer:
             self.latents = nn.Parameter(torch.randn(components_num, latent_dim))
 
-    def forward(self, img):
+    def forward(self, img, c: Optional[torch.Tensor] = None):
+        if self.c_dim > 0:
+            if c is None:
+                raise ValueError(f"this discriminator is conditional (c_dim={self.c_dim}): labels c [B, {self.c_dim}] are required")
+            c = torch.as_tensor(c)
+            if c.dim() != 2 or c.shape[0] != img.shape[0] or c.shape[1] != self.c_dim:
+                raise ValueError(f"c must be [{img.shape[0]}, {self.c_dim}], got {tuple(c.shape)}")
         x = self.fromrgb(img.contiguous(memory_format=torch.channels_last))
         y, composite = None, False
         if self.transformer:
@@ -181,7 +197,10 @@ class Discriminator(nn.Module):
         x = self.conv4(torch.cat([x, s], dim=1)).reshape(B, -1)
         if y is not None:
             x = torch.cat([x, y.reshape(B, -1)], dim=1)
-        return self.fc1(self.fc0(x)).reshape(B)
+        out = self.fc1(self.fc0(x))
+        if self.c_dim > 0:                                              # projection onto the labels
+            return (out * c.to(device=out.device, dtype=out.dtype)).sum(dim=1)
+        return out.reshape(B)
 
 
 @dataclass
@@ -232,6 +251,9 @@ class Trainer:
 
     def __init__(self, G: nn.Module, D: nn.Module, cfg: Optional[TrainConfig] = None, world: int = 1):
         self.G, self.D, self.cfg, self.world = G, D, cfg or TrainConfig(), world
+        self.c_dim = getattr(G, "c_dim", 0)
+        if getattr(D, "c_dim", 0) != self.c_dim:
+            raise ValueError(f"G and D must have the same c_dim, got {self.c_dim} and {getattr(D, 'c_dim', 0)}")
         if not 0.0 <= self.cfg.style_mixing <= 1.0:
             raise ValueError(f"style_mixing must be in [0, 1], got {self.cfg.style_mixing}")
         if self.cfg.style_mixing > 0 and not (hasattr(G, "mapping") and hasattr(G, "synthesis")):
@@ -259,21 +281,36 @@ class Trainer:
         if buckets is not None:
             stats.allreduce_bytes += buckets.finish()      # joins the communication stream (the buckets overlapped backward)
 
+    def _labels(self, z: torch.Tensor, reals: torch.Tensor, gen_c, real_c):
+        """(gen_c, real_c) checked against the batch and moved to z's device and dtype: both required iff c_dim > 0; (None, None) for
+        an unconditional pair."""
+        if self.c_dim == 0:
+            return None, None
+        for name, c, n in (("gen_c", gen_c, z.shape[0]), ("real_c", real_c, reals.shape[0])):
+            if c is None:
+                raise ValueError(f"conditional training (c_dim={self.c_dim}) needs {name} [{n}, {self.c_dim}]")
+            if c.dim() != 2 or c.shape[0] != n or c.shape[1] != self.c_dim:
+                raise ValueError(f"{name} must be [{n}, {self.c_dim}], got {tuple(c.shape)}")
+        return gen_c.to(device=z.device, dtype=z.dtype), real_c.to(device=z.device, dtype=z.dtype)
+
     def _step_tensors(self, z: torch.Tensor, reals: torch.Tensor, do_r1: bool, stats: Optional[StepStats] = None,
-                      do_pl: bool = False):
+                      do_pl: bool = False, gen_c: Optional[torch.Tensor] = None, real_c: Optional[torch.Tensor] = None):
         """One D update + one G update (+ the path-length update with ``do_pl``); returns (loss_d, loss_g, r1, pl_penalty, cutoffs) as
         device tensors without synchronising (capturable); pl_penalty is None without ``do_pl``; cutoffs maps the StepStats.extra
-        names of the style-mixing cutoffs of the D and G phases to them (empty without style mixing)."""
+        names of the style-mixing cutoffs of the D and G phases to them (empty without style mixing).  gen_c / real_c: the labels
+        of the fakes and of the reals (None for an unconditional pair: the calls then pass no labels)."""
         G, D, cfg = self.G, self.D, self.cfg
+        gc = () if gen_c is None else (gen_c,)                          # label arguments of the calls on fakes / reals
+        rc = () if real_c is None else (real_c,)
         stats = stats if stats is not None else StepStats()
         cutoffs: Dict[str, torch.Tensor] = {}
         # ---- discriminator: logistic loss (+ lazy R1 on the reals)
         G.requires_grad_(False); D.requires_grad_(True)
         self._zero(self.opt_d, self.buckets_d)
         with torch.no_grad():
-            fakes = self._generate(z, cutoffs, "d")
+            fakes = self._generate(z, cutoffs, "d", gc)
         reals_in = reals.detach().requires_grad_(do_r1)
-        logit_real, logit_fake = D(reals_in), D(fakes)
+        logit_real, logit_fake = D(reals_in, *rc), D(fakes, *gc)
         loss_d = F.softplus(logit_fake).mean() + F.softplus(-logit_real).mean()
         r1 = torch.zeros((), device=z.device)
         if do_r1:
@@ -289,17 +326,17 @@ class Trainer:
             advance_dropout(z.device)                 # attention dropout: fresh masks for the G phase (device-side, capturable)
         G.requires_grad_(True); D.requires_grad_(False)
         self._zero(self.opt_g, self.buckets_g)
-        loss_g = F.softplus(-D(self._generate(z, cutoffs, "g"))).mean()
+        loss_g = F.softplus(-D(self._generate(z, cutoffs, "g", gc), *gc)).mean()
         loss_g.backward()
         self._allreduce(self.buckets_g, stats)
         self.opt_g.step()
         if z.is_cuda:
             advance_dropout(z.device)                 # ... and for the next step
-        pl_penalty = self._pl_phase(z, stats) if do_pl else None
+        pl_penalty = self._pl_phase(z, stats, gc) if do_pl else None
         # ---- moving average of the generator (and of the mapping outputs: the truncation trick's w_avg)
         with torch.no_grad():
             if hasattr(G, "mapping") and hasattr(G.mapping, "w_avg"):
-                ws = G.mapping(z)
+                ws = G.mapping(z, *gc)
                 k_ = G.mapping.components_num
                 cur = torch.stack([ws[:, :k_].mean(dim=(0, 1)), ws[:, k_:].mean(dim=(0, 1))])
                 G.mapping.w_avg.lerp_(cur, 1.0 - cfg.w_avg_beta)
@@ -310,28 +347,30 @@ class Trainer:
                 be.copy_(b)
         return loss_d.detach(), loss_g.detach(), r1.detach(), pl_penalty, cutoffs
 
-    def _generate(self, z: torch.Tensor, cutoffs: Dict[str, torch.Tensor], phase: str) -> torch.Tensor:
+    def _generate(self, z: torch.Tensor, cutoffs: Dict[str, torch.Tensor], phase: str, gc=()) -> torch.Tensor:
         """The fakes of one phase: G(z), or with style mixing (SURVEY A.4 item 13) the synthesis of per-layer latents that switch
-        from G.mapping(z) to the mapping of a second draw at a cutoff of their own.  Device-side throughout (capturable)."""
+        from G.mapping(z) to the mapping of a second draw at a cutoff of their own.  gc: () or (the labels,), which both draws take.
+        Device-side throughout (capturable)."""
         G, cfg = self.G, self.cfg
         if cfg.style_mixing <= 0.0:
-            return G(z, noise_mode=cfg.noise_mode)
+            return G(z, *gc, noise_mode=cfg.noise_mode)
         num_ws = G.synthesis.num_ws
         z2 = torch.randn_like(z)
-        ws1, ws2 = G.mapping(z), G.mapping(z2)
+        ws1, ws2 = G.mapping(z, *gc), G.mapping(z2, *gc)
         cutoff = mixing_cutoff(cfg.style_mixing, num_ws, z.device)
         cutoffs["style_mixing_cutoff_" + phase] = cutoff
         return G.synthesis(mix_latents(ws1, ws2, cutoff, num_ws), noise_mode=cfg.noise_mode)
 
-    def _pl_phase(self, z: torch.Tensor, stats: StepStats) -> torch.Tensor:
+    def _pl_phase(self, z: torch.Tensor, stats: StepStats, gc=()) -> torch.Tensor:
         """The lazy path-length update of G (StyleGAN2): returns the penalty as a device tensor (capturable: no host sync, the
-        noise is drawn on the device)."""
+        noise is drawn on the device).  gc: () or (the labels of z,), cut to the same first B' rows."""
         G, cfg = self.G, self.cfg
         if z.is_cuda:
             from .attention import advance_dropout
             advance_dropout(z.device)                 # fresh attention-dropout masks; the backward regenerates the same ones
         self._zero(self.opt_g, self.buckets_g)
-        ws = G.mapping(z[:max(1, z.shape[0] // cfg.pl_batch_shrink)])
+        nb = max(1, z.shape[0] // cfg.pl_batch_shrink)
+        ws = G.mapping(z[:nb], *[c[:nb] for c in gc])
         img = G.synthesis(ws, noise_mode=cfg.noise_mode)
         pl_noise = torch.randn_like(img) / math.sqrt(img.shape[2] * img.shape[3])
         (pl_grads,) = torch.autograd.grad((img * pl_noise).sum(), ws, create_graph=True)
@@ -359,48 +398,60 @@ class Trainer:
             stats.pl_mean = float(self.pl_mean)
         return stats
 
-    def step(self, z: torch.Tensor, reals: torch.Tensor) -> StepStats:
+    def step(self, z: torch.Tensor, reals: torch.Tensor, gen_c: Optional[torch.Tensor] = None,
+             real_c: Optional[torch.Tensor] = None) -> StepStats:
+        """gen_c [B, c_dim]: the labels of the fakes (one per z); real_c: those of the reals.  Required iff c_dim > 0."""
+        gen_c, real_c = self._labels(z, reals, gen_c, real_c)
         stats = StepStats()
         do_r1 = self.cfg.r1_gamma > 0 and self.it % self.cfg.d_reg_interval == 0
-        outs = self._step_tensors(z, reals, do_r1, stats, self._do_pl())
+        outs = self._step_tensors(z, reals, do_r1, stats, self._do_pl(), gen_c, real_c)
         self._finish_stats(stats, *outs)
         bump_weights_epoch()
         self.it += 1
         return stats
 
-    def step_graphed(self, z: torch.Tensor, reals: torch.Tensor) -> StepStats:
+    def step_graphed(self, z: torch.Tensor, reals: torch.Tensor, gen_c: Optional[torch.Tensor] = None,
+                     real_c: Optional[torch.Tensor] = None) -> StepStats:
         """The same step replayed from a CUDA graph (one graph per combination of the lazy R1 term and the lazy path-length
         phase that occurs, at most three with the default intervals): the eager step is bound by the host launching ~5000 small
-        kernels.  Shapes are fixed by the first call; the first calls warm up eagerly."""
+        kernels.  Shapes are fixed by the first call; the first calls warm up eagerly.  The labels, like z and reals, go through
+        static buffers."""
         from . import attention as _att, networks as _nets
         cfg = self.cfg
+        gen_c, real_c = self._labels(z, reals, gen_c, real_c)
         do_r1 = cfg.r1_gamma > 0 and self.it % cfg.d_reg_interval == 0
         st = self.__dict__.setdefault("_graphs", {})
         _nets.CACHE_BYPASS = _att.FORCE_REFOLD = True                  # weight-derived tensors are recomputed inside the graph
         try:
-            return self._step_graphed(z, reals, (do_r1, self._do_pl()), st)
+            return self._step_graphed(z, reals, (do_r1, self._do_pl()), st, gen_c, real_c)
         finally:
             _nets.CACHE_BYPASS = _att.FORCE_REFOLD = False
 
-    def _step_graphed(self, z, reals, key, st) -> StepStats:
+    def _step_graphed(self, z, reals, key, st, gen_c=None, real_c=None) -> StepStats:
         cfg = self.cfg
         if "z" not in st:
             st["z"], st["reals"] = torch.empty_like(z), torch.empty_like(reals)
             st["z"].copy_(z); st["reals"].copy_(reals)
+            st["gen_c"] = st["real_c"] = None
+            if gen_c is not None:
+                st["gen_c"], st["real_c"] = gen_c.clone(), real_c.clone()
+            lab = dict(gen_c=st["gen_c"], real_c=st["real_c"])
             side = torch.cuda.Stream(device=z.device)                 # warm-up off the capture stream: cuDNN autotune, workspaces
             side.wait_stream(torch.cuda.current_stream(z.device))
             with torch.cuda.stream(side):
                 for r in ([True, False] if cfg.r1_gamma > 0 else [False]):
-                    self._step_tensors(st["z"], st["reals"], r)
+                    self._step_tensors(st["z"], st["reals"], r, **lab)
                 if cfg.pl_weight > 0:
-                    self._step_tensors(st["z"], st["reals"], False, do_pl=True)
+                    self._step_tensors(st["z"], st["reals"], False, do_pl=True, **lab)
             torch.cuda.current_stream(z.device).wait_stream(side)
             torch.cuda.synchronize(z.device)
         st["z"].copy_(z); st["reals"].copy_(reals)
+        if gen_c is not None:
+            st["gen_c"].copy_(gen_c); st["real_c"].copy_(real_c)
         if key not in st:
             graph = torch.cuda.CUDAGraph()
             with torch.cuda.graph(graph):
-                outs = self._step_tensors(st["z"], st["reals"], key[0], do_pl=key[1])
+                outs = self._step_tensors(st["z"], st["reals"], key[0], do_pl=key[1], gen_c=st["gen_c"], real_c=st["real_c"])
             st[key] = (graph, outs)
             # (capture does not execute: fall through to the replay below)
         graph, outs = st[key]

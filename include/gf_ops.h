@@ -96,6 +96,16 @@ int gf_torgb_scale_nhwc(const float* x, const float* w, const float* styles, int
 int gf_mapping_fwd(const float* z, const float* w, const float* b, const float* w_avg, float psi, float* out,
                    int B, int k, int D, int L, void* stream);
 
+/* Class-conditional G_mapping (SURVEY A.4 item 14) as one kernel: gf_mapping_fwd with labels c [B, c_dim] and the label
+ * embedding E [c_dim, D].  Image b's embedding e_b = c_b E is concatenated to each of its k+1 latents, and every row
+ * [z_bj || e_b] is pixel-normalised over its 2D entries.  Layer 0 of both paths takes that 2D input: w0 [2, 2D(in), D(out)]
+ * (gain lr_mul/sqrt(2D), times sqrt(2), folded in).  Layers 1..L-1 are w [2, L-1, D, D] as in gf_mapping_fwd (NULL when L == 1);
+ * b [2, L, D] holds the biases of all L layers.  Zero label entries are skipped, so a one-hot label reads one row of E.
+ * E and the label half of w0 are read through L2; the rest of the weights are staged in shared memory, the same 2*L*D*D floats
+ * as gf_mapping_fwd, so the two serve the same shapes.  c_dim >= 1, D <= 128. */
+int gf_mapping_fwd_cond(const float* z, const float* c, int c_dim, const float* E, const float* w0, const float* w, const float* b,
+                        const float* w_avg, float psi, float* out, int B, int k, int D, int L, void* stream);
+
 /* Row f1, first kernel: the 3x3 stride-1 convolution of the synthesis layers (zero padding 1) as a wgmma implicit GEMM in TF32,
  * channels-last: y[b,h,w,o] = sum_{dy,dx,i} x[b,h+dy-1,w+dx-1,i] * wt[dy*3+dx][o][i].  This is the convolution inside the reference's
  * modulated_conv2d_layer in its activation-scaling form (x already carries the style, demodulation is applied by the consumer).
