@@ -13,7 +13,7 @@ from pathlib import Path
 PKG_DIR = Path(__file__).resolve().parent
 CSRC = PKG_DIR / "csrc"
 LIB_PATH = PKG_DIR / "libgf_attn.so"
-SOURCES = ["gf_api.cu", "gf_fold.cu", "gf_simt.cu", "gf_tc.cu", "gf_tc_cen.cu", "gf_tc_gemm.cu", "gf_bwd.cu", "gf_ops.cu", "gf_conv.cu"]
+SOURCES = ["gf_api.cu", "gf_fold.cu", "gf_simt.cu", "gf_tc.cu", "gf_tc_cen.cu", "gf_tc_gemm.cu", "gf_bwd.cu", "gf_ops.cu", "gf_conv.cu", "gf_augment.cu"]
 COMPILE_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
     "-lineinfo", "-O3", "-std=c++17",

@@ -1,8 +1,9 @@
 """Data-parallel plumbing: one process per GPU (torchrun), NCCL over NVLink/NVSwitch.
 
 The generator shards by images (SURVEY 8e): every image is independent through the whole network, so inference
-needs no collective; the only collective of the system is the gradient all-reduce of the G/D training step
-(reference: dnnlib/tflib/optimizer.py -> nccl_ops.all_sum over in-process towers, upstream; not in the checkout).
+needs no collective.  The collectives of the system are in the G/D training step: the gradient all-reduce (reference:
+dnnlib/tflib/optimizer.py -> nccl_ops.all_sum over in-process towers, upstream; not in the checkout) and, with adaptive
+augmentation, one two-float sum of the ADA accumulators per step (``allreduce_sum``).
 """
 from __future__ import annotations
 
@@ -159,6 +160,12 @@ class GradBuckets:
         if self._cuda:
             torch.cuda.current_stream(self.flat.device).wait_stream(self._comm)
         return self.bytes_per_step
+
+
+def allreduce_sum(t: torch.Tensor) -> None:
+    """In-place sum of a small tensor over ranks on the current stream (capturable with NCCL): the ADA accumulators of the training
+    step, so that every rank holds the same augmentation strength."""
+    dist.all_reduce(t, op=dist.ReduceOp.SUM)
 
 
 def max_over_ranks(value: float, device=None) -> float:

@@ -342,6 +342,130 @@ def mapping_fwd(z: torch.Tensor, w_eff: torch.Tensor, b_eff: torch.Tensor, w_avg
     return out
 
 
+def _augment_args(x: torch.Tensor, geom: torch.Tensor, color: Optional[torch.Tensor]):
+    """Checks of ops.augment (the same refusals as gf_augment_nchw); returns geom as int32 [B, 4] and color as [B, 12] on x's device."""
+    if x.dim() != 4:
+        raise ValueError(f"augment: x must be [B, C, H, W], got {tuple(x.shape)}")
+    B, C, H, W = x.shape
+    if H < 2 or W < 2:
+        raise ValueError(f"augment: H and W must be at least 2, got {H}x{W}")
+    if tuple(geom.shape) != (B, 4):
+        raise ValueError(f"augment: geom must be [{B}, 4], got {tuple(geom.shape)}")
+    geom = geom.to(device=x.device, dtype=torch.int32).contiguous()
+    if color is not None:
+        if C != 3:
+            raise ValueError(f"augment: a colour matrix needs C == 3, got C = {C}")
+        if color.numel() != B * 12 or color.shape[0] != B:
+            raise ValueError(f"augment: color must be [{B}, 12] or [{B}, 3, 4], got {tuple(color.shape)}")
+        color = color.reshape(B, 12).to(device=x.device, dtype=torch.float32 if x.is_cuda and x.dtype == torch.float32 else x.dtype)
+        color = color.contiguous()
+    return geom, color
+
+
+def augment_index(geom: torch.Tensor, H: int, W: int) -> torch.Tensor:
+    """Definition of the blit: the flat source index sy * W + sx [B, H * W] of every output pixel, (sx, sy) = R(D_b(x, y) - t_b),
+    with the parameter rules of gf_augment_nchw (code masked to 3 bits, bit 1 cleared when H != W, |t| clamped to N - 1)."""
+    g = geom.to(torch.int64)
+    code = g[:, 0] & 7
+    if H != W:
+        code = code & 5
+    tx = g[:, 1].clamp(-(W - 1), W - 1)[:, None, None]
+    ty = g[:, 2].clamp(-(H - 1), H - 1)[:, None, None]
+    yy, xx = torch.meshgrid(torch.arange(H, device=geom.device), torch.arange(W, device=geom.device), indexing="ij")
+    c = code[:, None, None]
+    xx = torch.where((c & 1) == 1, W - 1 - xx[None], xx[None])
+    yy = yy[None].expand_as(xx)
+    k = c >> 1
+    u = torch.where(k == 0, xx, torch.where(k == 1, yy, torch.where(k == 2, W - 1 - xx, H - 1 - yy)))
+    v = torch.where(k == 0, yy, torch.where(k == 1, W - 1 - xx, torch.where(k == 2, H - 1 - yy, xx)))
+
+    def mirror(i, N):
+        return torch.where(i < 0, -i, torch.where(i >= N, 2 * (N - 1) - i, i))
+    return (mirror(v - ty, H) * W + mirror(u - tx, W)).reshape(geom.shape[0], H * W)
+
+
+def augment_ref(x: torch.Tensor, geom: torch.Tensor, color: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """Definition of ops.augment: an index gather (the blit), then the colour matrix per pixel.  Any dtype and device; torch
+    autograd differentiates it to any order."""
+    geom, color = _augment_args(x, geom, color)
+    B, C, H, W = x.shape
+    idx = augment_index(geom, H, W)
+    y = x.reshape(B, C, H * W).gather(2, idx[:, None].expand(B, C, H * W)).reshape(B, C, H, W)
+    if color is None:
+        return y
+    M = color.reshape(B, 3, 4).to(x.dtype)
+    return torch.einsum("bij,bjhw->bihw", M[:, :, :3], y) + M[:, :, 3, None, None]
+
+
+def augment_adjoint_ref(gy: torch.Tensor, geom: torch.Tensor, color: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """Definition of the adjoint of ops.augment's linear part: the transposed 3x3 colour matrix (no offset), then a scatter-add
+    of every output pixel onto its source pixel."""
+    geom, color = _augment_args(gy, geom, color)
+    B, C, H, W = gy.shape
+    if color is not None:
+        gy = torch.einsum("bij,bihw->bjhw", color.reshape(B, 3, 4).to(gy.dtype)[:, :, :3], gy)
+    idx = augment_index(geom, H, W)
+    gx = gy.new_zeros(B, C, H * W).scatter_add(2, idx[:, None].expand(B, C, H * W), gy.reshape(B, C, H * W))
+    return gx.reshape(B, C, H, W)
+
+
+def _augment_native(name: str, x: torch.Tensor, geom: torch.Tensor, color: Optional[torch.Tensor]) -> torch.Tensor:
+    xc = x.detach().contiguous()
+    B, C, H, W = xc.shape
+    y = torch.empty_like(xc)
+    with torch.cuda.device(x.device):
+        _lib.check(getattr(_lib.load(), name)(xc.data_ptr(), y.data_ptr(), geom.data_ptr(), None if color is None else color.data_ptr(),
+                                              B, C, H, W, _stream(x.device)), name)
+    return y
+
+
+def _linear_part(color: Optional[torch.Tensor]) -> Optional[torch.Tensor]:
+    """The colour matrices [B, 12] with their offset column zeroed: the linear part of the map, whose derivative it is."""
+    if color is None:
+        return None
+    return torch.cat([color.reshape(-1, 3, 4)[:, :, :3], color.new_zeros(color.shape[0], 3, 1)], dim=2).reshape(-1, 12)
+
+
+class _Augment(torch.autograd.Function):
+    """gf_augment_nchw, differentiable to any order: the map is linear apart from the colour offset, so its gradient is the adjoint
+    (_AugmentAdjoint), whose gradient is the linear part of the map again."""
+
+    @staticmethod
+    def forward(ctx, x, geom, color):
+        ctx.save_for_backward(geom, color)
+        return _augment_native("gf_augment_nchw", x, geom, color)
+
+    @staticmethod
+    def backward(ctx, gy):
+        geom, color = ctx.saved_tensors
+        return _AugmentAdjoint.apply(gy, geom, color), None, None
+
+
+class _AugmentAdjoint(torch.autograd.Function):
+    """gf_augment_adjoint_nchw: gx = A^T gy (the offset does not take part)."""
+
+    @staticmethod
+    def forward(ctx, gy, geom, color):
+        ctx.save_for_backward(geom, color)
+        return _augment_native("gf_augment_adjoint_nchw", gy, geom, color)
+
+    @staticmethod
+    def backward(ctx, ggx):
+        geom, color = ctx.saved_tensors
+        return _Augment.apply(ggx, geom, _linear_part(color)), None, None
+
+
+def augment(x: torch.Tensor, geom: torch.Tensor, color: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """Adaptive discriminator augmentation of a batch (SURVEY A.4 item 15): x [B, C, H, W] -> the same shape, image b blitted by its
+    geom[b] = (dihedral code, tx, ty, unused) and, with color [B, 12] (row-major 3x4 matrices on (r, g, b, 1), C == 3), recoloured.
+    See include/gf_ops.h for the exact map.  CUDA fp32 tensors run gf_augment_nchw, and its adjoint in the backward (to any order);
+    anything else runs the definition augment_ref."""
+    geom, color = _augment_args(x, geom, color)
+    if x.is_cuda and x.dtype == torch.float32:
+        return _Augment.apply(x, geom, color)
+    return augment_ref(x, geom, color)
+
+
 def conv3x3_pack(weight: torch.Tensor, scale: float = 1.0) -> torch.Tensor:
     """weight [O, I, 3, 3] -> the tap-major, TF32-rounded [9, O, I] layout gf_conv3x3_nhwc_tf32 consumes (gf_conv3x3_pack_weights)."""
     O, I = weight.shape[:2]

@@ -5,7 +5,8 @@ What the reference does (expected upstream ``src/training/training_loop.py``, ``
 non-saturating logistic losses, R1 gradient penalty on the reals with lazy regularisation, Adam(beta1 = 0,
 beta2 = 0.99), an exponential moving average of the generator weights, data parallelism over GPUs with a summed
 gradient all-reduce.  Here: one process per GPU, gradients averaged through ONE flat fp32 buffer per network
-(``dist.allreduce_gradients``: NCCL over NVLink/NVSwitch, gloo in the CPU tests) -- the only collective of the system.
+(``dist.allreduce_gradients``: NCCL over NVLink/NVSwitch, gloo in the CPU tests).  The only other collective is the two-float sum of
+the ADA accumulators below.
 
 The attention layers run their CUDA forward.  Their backward (``autograd.py``) is the hand-written stage-T backward kernel for
 simplex layers, the same kernel plus the pass-A backward kernels for duplex layers with attention dropout, and the torch
@@ -21,7 +22,7 @@ step after the G update: on the first B // pl_batch_shrink latents, the gradient
 to the dlatents ws [B, k+1, D], its length over the k+1 latent components (SURVEY A.4 item 12), and the squared distance of that
 length to its running mean.  The backward of that gradient needs the generator's second derivative: the attention layers give it
 through the double-backward kernels (``gf_attn_simplex_bwd_vjp_ex``, with the forward's dropout mask) or, on the composite route, torch
-autograd.  Off by default.  Augmentation is out of scope.
+autograd.  Off by default.
 
 ``TrainConfig.style_mixing > 0`` adds StyleGAN2's style mixing (SURVEY A.4 item 13): each generator forward of the D and G phases
 maps z and a second draw z2, and feeds the synthesis per-layer latents that switch from the first to the second at a cutoff drawn
@@ -32,6 +33,15 @@ Class-conditional training (SURVEY A.4 item 14): a generator and a discriminator
 ``step(z, reals, gen_c, real_c)``: the fakes of both phases, the path-length phase (on gen_c[:B']), both style-mixing draws and the
 w_avg update use gen_c, the discriminator's real logits and R1 use real_c.  The labels are sharded like z and reals.  With
 ``c_dim = 0`` the labels are ignored and the step makes the same calls as before.
+
+``TrainConfig.augment`` adds adaptive discriminator augmentation (ADA, Karras et al. 2020; SURVEY A.4 item 15): every image batch
+the discriminator sees -- the reals of the D phase (R1 included: the gradient is taken with respect to the un-augmented reals,
+through the augmentation), the fakes of the D phase and the fakes of the G phase -- goes through ``ops.augment`` with per-image
+parameters of its own (``sample_augment``): integer blits (x flips, 90-degree rotations, integer translations with mirror padding)
+and a colour matrix, on the gf_augment_nchw kernel and its adjoint.  The strength p is a device tensor (``Trainer.augment_p``); with
+``ada_target`` it adapts to the sign of the real logits, summed over ranks, every ``ada_interval`` steps, without a host sync.  Not
+in the path-length phase, the w_avg update or inference.  Off by default: with "" the step makes the same calls and draws the same
+random numbers as without the option.
 """
 from __future__ import annotations
 
@@ -49,7 +59,7 @@ from .attention import BipartiteAttention
 from .autograd import _e, composite_forward
 from .networks import FullyConnected, nf
 from ._state import bump_weights_epoch
-from .ops import fir4, fir_filter, upfirdn2d_ref
+from .ops import augment, fir4, fir_filter, upfirdn2d_ref
 
 SQRT2 = math.sqrt(2.0)
 
@@ -217,6 +227,97 @@ class TrainConfig:
     pl_batch_shrink: int = 2            # the path-length phase runs on the first B // 2 latents
     pl_decay: float = 0.01              # decay of the running mean of the path lengths
     style_mixing: float = 0.0           # probability of style mixing per generator forward (StyleGAN2 / GANsformer: 0.9); 0 = off
+    augment: str = ""                   # discriminator augmentation: "" = off, "bc" = all of AUGMENT_OPS, or a comma list of them
+    augment_p: float = 0.0              # starting augmentation strength p
+    ada_target: Optional[float] = None  # adaptive p: target of the mean sign of the real logits (ADA: 0.6); None = p stays put
+    ada_interval: int = 4               # steps between updates of p
+    ada_kimg: float = 500.0             # p can go from 0 to 1 in this many thousand images
+
+
+AUGMENT_OPS = ("xflip", "rotate90", "xint", "brightness", "contrast", "lumaflip", "hue", "saturation")
+
+
+def parse_augment(spec: str) -> tuple:
+    """TrainConfig.augment -> the enabled transforms, in AUGMENT_OPS order: "" none, "bc" all eight, else a comma list of names."""
+    if not spec:
+        return ()
+    if spec == "bc":
+        return AUGMENT_OPS
+    names = {s.strip() for s in spec.split(",")}
+    unknown = sorted(names - set(AUGMENT_OPS))
+    if unknown:
+        raise ValueError(f"unknown augmentation(s) {unknown}: use 'bc' or a comma list of {AUGMENT_OPS}")
+    return tuple(n for n in AUGMENT_OPS if n in names)
+
+
+def sample_augment(ops_: tuple, p, B: int, H: int, W: int, device):
+    """Per-image augmentation parameters for ops.augment, drawn on ``device`` from torch's RNG without a host sync (capturable):
+    (geom int32 [B, 4], color float32 [B, 12] or None when no colour transform is enabled).  ``p`` (a float or a 0-d device tensor)
+    is the probability that each enabled transform applies to each image; a transform that does not apply contributes exactly the
+    identity, so p = 0 gives identity parameters.  Every enabled transform draws the same random numbers whatever p is.
+
+    Geometry (ADA's integer "pixel blitting"): xflip = a flip uniform in {none, flip}; rotate90 = k * 90 degrees, k uniform in 0..3
+    (H == W only); xint = t = round(U(-0.125, 0.125) * (W, H)).  Colour, composed in this order on (r, g, b, 1): brightness + N(0, 0.2);
+    contrast * lognormal(0, 0.5 ln 2); lumaflip I - 2 i v v^T, i uniform in {0, 1}, v = (1, 1, 1) / sqrt 3; hue = rotation about v
+    by U(-pi, pi); saturation v v^T + s (I - v v^T), s lognormal(0, ln 2)."""
+    if "rotate90" in ops_ and H != W:
+        raise ValueError(f"the rotate90 augmentation needs square images, got {H}x{W}")
+
+    def applies():
+        return torch.rand(B, device=device) < p
+
+    zero = torch.zeros(B, dtype=torch.int64, device=device)
+    code, tx, ty = zero, zero, zero
+    if "xflip" in ops_:
+        code = code + torch.where(applies(), torch.randint(0, 2, (B,), device=device), zero)
+    if "rotate90" in ops_:
+        code = code + 2 * torch.where(applies(), torch.randint(0, 4, (B,), device=device), zero)
+    if "xint" in ops_:
+        a = applies()
+        u = torch.rand(B, 2, device=device) * 2 - 1
+        tx = torch.where(a, torch.round(u[:, 0] * (0.125 * W)).long(), zero)
+        ty = torch.where(a, torch.round(u[:, 1] * (0.125 * H)).long(), zero)
+    geom = torch.stack([code, tx, ty, zero], dim=1).to(torch.int32)
+    if not any(n in ops_ for n in AUGMENT_OPS[3:]):
+        return geom, None
+    eye4 = torch.eye(4, device=device).expand(B, 4, 4)
+    v = torch.full((3,), 1.0 / math.sqrt(3.0), device=device)
+    vv = torch.outer(v, v)
+    eye3 = torch.eye(3, device=device)
+    M = eye4
+
+    def then(T, a):                                  # M <- T M where transform T applies, else I M (exact)
+        return torch.where(a[:, None, None], T, eye4) @ M
+
+    def lin(T3):                                     # [B, 3, 3] -> [B, 4, 4] with no offset
+        T = eye4.clone()
+        T[:, :3, :3] = T3
+        return T
+    if "brightness" in ops_:
+        a = applies()
+        T = eye4.clone()
+        T[:, :3, 3] = (torch.randn(B, device=device) * 0.2)[:, None]
+        M = then(T, a)
+    if "contrast" in ops_:
+        a = applies()
+        c = torch.exp2(torch.randn(B, device=device) * 0.5)
+        M = then(lin(c[:, None, None] * eye3), a)
+    if "lumaflip" in ops_:
+        a = applies()
+        i = torch.randint(0, 2, (B,), device=device).float()
+        M = then(lin(eye3 - 2 * i[:, None, None] * vv), a)
+    if "hue" in ops_:
+        a = applies()
+        th = (torch.rand(B, device=device) * 2 - 1) * math.pi
+        P = eye3.roll(1, dims=0)
+        K = (P - P.t()) / math.sqrt(3.0)              # the cross-product matrix [v]x of v = (1, 1, 1) / sqrt 3
+        cs, sn = torch.cos(th)[:, None, None], torch.sin(th)[:, None, None]
+        M = then(lin(cs * eye3 + sn * K + (1 - cs) * vv), a)
+    if "saturation" in ops_:
+        a = applies()
+        s = torch.exp2(torch.randn(B, device=device))[:, None, None]
+        M = then(lin(vv + s * (eye3 - vv)), a)
+    return geom, M[:, :3, :].reshape(B, 12).contiguous()
 
 
 def mixing_cutoff(p: float, num_ws: int, device) -> torch.Tensor:
@@ -244,6 +345,7 @@ class StepStats:
     extra: Dict[str, float] = field(default_factory=dict)
     pl_penalty: float = 0.0             # mean squared deviation of the path lengths from their running mean (a path-length step)
     pl_mean: float = 0.0                # the running mean of the path lengths (this rank's)
+    augment_p: float = 0.0              # the augmentation strength p after the step (the same on every rank)
 
 
 class Trainer:
@@ -258,6 +360,8 @@ class Trainer:
             raise ValueError(f"style_mixing must be in [0, 1], got {self.cfg.style_mixing}")
         if self.cfg.style_mixing > 0 and not (hasattr(G, "mapping") and hasattr(G, "synthesis")):
             raise ValueError("style_mixing needs a generator with `mapping` and `synthesis`")
+        self.augment_ops = parse_augment(self.cfg.augment)
+        self._check_augment()
         self.G_ema = copy.deepcopy(G).eval().requires_grad_(False)
         c = self.cfg.d_reg_interval / (self.cfg.d_reg_interval + 1.0)  # lazy regularisation: rescale lr and betas
         cap = next(G.parameters()).is_cuda                              # capturable: the step can be replayed from a CUDA graph
@@ -270,6 +374,53 @@ class Trainer:
         # data parallel: gradients live in one flat buffer per network, reduced bucket by bucket while backward still runs
         self.buckets_g = gdist.GradBuckets(G.parameters(), world, self.cfg.bucket_mb) if world > 1 else None
         self.buckets_d = gdist.GradBuckets(D.parameters(), world, self.cfg.bucket_mb) if world > 1 else None
+        # augmentation (SURVEY A.4 item 15): the strength p and, with ada_target, the accumulators of the adaptive update -- device
+        # tensors updated in place (capturable); callers may save and restore them
+        dev = next(G.parameters()).device
+        self.augment_p = torch.full((), float(self.cfg.augment_p), device=dev) if self.augment_ops else None
+        self.ada_stats = torch.zeros(2, device=dev) if self.cfg.ada_target is not None else None     # (sum of signs, count)
+        self.ada_steps = torch.zeros((), dtype=torch.int64, device=dev) if self.cfg.ada_target is not None else None
+
+    def _check_augment(self):
+        cfg = self.cfg
+        if not 0.0 <= cfg.augment_p <= 1.0:
+            raise ValueError(f"augment_p must be in [0, 1], got {cfg.augment_p}")
+        if cfg.ada_target is not None:
+            if not self.augment_ops:
+                raise ValueError("ada_target adapts the augmentation strength: it needs augment to be set")
+            if not -1.0 <= cfg.ada_target <= 1.0:
+                raise ValueError(f"ada_target is a mean sign and must be in [-1, 1], got {cfg.ada_target}")
+            if cfg.ada_interval < 1 or not cfg.ada_kimg > 0:
+                raise ValueError(f"need ada_interval >= 1 and ada_kimg > 0, got {cfg.ada_interval} and {cfg.ada_kimg}")
+
+    def _augment(self, img: torch.Tensor) -> torch.Tensor:
+        """One image batch on its way into D, augmented with parameters of its own (no call and no random number when off)."""
+        if not self.augment_ops:
+            return img
+        B, _, H, W = img.shape
+        geom, color = sample_augment(self.augment_ops, self.augment_p, B, H, W, img.device)
+        return augment(img, geom, color)
+
+    def _ada_accumulate(self, logit_real: torch.Tensor):
+        """Adds (sum of the signs, count) of this step's real logits, summed over ranks, to the ADA accumulators."""
+        l = logit_real.detach()
+        inc = torch.stack([l.sign().sum(), torch.ones_like(l).sum()]).float()
+        if self.world > 1:
+            gdist.allreduce_sum(inc)
+        self.ada_stats.add_(inc)
+
+    def _ada_update(self, batch: int):
+        """Every ada_interval-th step: p <- clamp(p + sign(mean sign - target) * B_global * interval / (kimg * 1000), 0, 1), then the
+        accumulators reset.  Decided on the device from a step counter, so a replayed graph does the same."""
+        cfg = self.cfg
+        step = batch * self.world * cfg.ada_interval / (cfg.ada_kimg * 1000.0)
+        with torch.no_grad():
+            boundary = torch.remainder(self.ada_steps + 1, cfg.ada_interval) == 0
+            mean = self.ada_stats[0] / self.ada_stats[1].clamp(min=1.0)
+            p_new = (self.augment_p + torch.sign(mean - cfg.ada_target) * step).clamp(0.0, 1.0)
+            self.augment_p.copy_(torch.where(boundary, p_new, self.augment_p))
+            self.ada_stats.copy_(torch.where(boundary, torch.zeros_like(self.ada_stats), self.ada_stats))
+            self.ada_steps.add_(1)
 
     def _zero(self, opt, buckets):
         if buckets is not None:
@@ -310,8 +461,10 @@ class Trainer:
         with torch.no_grad():
             fakes = self._generate(z, cutoffs, "d", gc)
         reals_in = reals.detach().requires_grad_(do_r1)
-        logit_real, logit_fake = D(reals_in, *rc), D(fakes, *gc)
+        logit_real, logit_fake = D(self._augment(reals_in), *rc), D(self._augment(fakes), *gc)
         loss_d = F.softplus(logit_fake).mean() + F.softplus(-logit_real).mean()
+        if self.ada_stats is not None:
+            self._ada_accumulate(logit_real)
         r1 = torch.zeros((), device=z.device)
         if do_r1:
             (grad,) = torch.autograd.grad(logit_real.sum(), reals_in, create_graph=True)
@@ -326,7 +479,7 @@ class Trainer:
             advance_dropout(z.device)                 # attention dropout: fresh masks for the G phase (device-side, capturable)
         G.requires_grad_(True); D.requires_grad_(False)
         self._zero(self.opt_g, self.buckets_g)
-        loss_g = F.softplus(-D(self._generate(z, cutoffs, "g", gc), *gc)).mean()
+        loss_g = F.softplus(-D(self._augment(self._generate(z, cutoffs, "g", gc)), *gc)).mean()
         loss_g.backward()
         self._allreduce(self.buckets_g, stats)
         self.opt_g.step()
@@ -345,6 +498,8 @@ class Trainer:
                 pe.lerp_(p.detach(), 1.0 - beta)
             for be, b in zip(self.G_ema.buffers(), G.buffers()):
                 be.copy_(b)
+        if self.ada_stats is not None:
+            self._ada_update(z.shape[0])
         return loss_d.detach(), loss_g.detach(), r1.detach(), pl_penalty, cutoffs
 
     def _generate(self, z: torch.Tensor, cutoffs: Dict[str, torch.Tensor], phase: str, gc=()) -> torch.Tensor:
@@ -396,6 +551,8 @@ class Trainer:
             stats.pl_penalty = float(pl_penalty)
         if self.pl_mean is not None:
             stats.pl_mean = float(self.pl_mean)
+        if self.augment_p is not None:
+            stats.augment_p = float(self.augment_p)
         return stats
 
     def step(self, z: torch.Tensor, reals: torch.Tensor, gen_c: Optional[torch.Tensor] = None,
@@ -436,6 +593,7 @@ class Trainer:
             if gen_c is not None:
                 st["gen_c"], st["real_c"] = gen_c.clone(), real_c.clone()
             lab = dict(gen_c=st["gen_c"], real_c=st["real_c"])
+            ada = [t.clone() for t in (self.augment_p, self.ada_stats, self.ada_steps) if t is not None]
             side = torch.cuda.Stream(device=z.device)                 # warm-up off the capture stream: cuDNN autotune, workspaces
             side.wait_stream(torch.cuda.current_stream(z.device))
             with torch.cuda.stream(side):
@@ -444,6 +602,8 @@ class Trainer:
                 if cfg.pl_weight > 0:
                     self._step_tensors(st["z"], st["reals"], False, do_pl=True, **lab)
             torch.cuda.current_stream(z.device).wait_stream(side)
+            for t, saved in zip([t for t in (self.augment_p, self.ada_stats, self.ada_steps) if t is not None], ada):
+                t.copy_(saved)                                        # the warm-up steps do not count towards the ADA schedule
             torch.cuda.synchronize(z.device)
         st["z"].copy_(z); st["reals"].copy_(reals)
         if gen_c is not None:

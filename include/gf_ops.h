@@ -122,6 +122,27 @@ int gf_conv3x3_nhwc_tf32(const float* x, const float* wt, float* y, int B, int H
 int gf_upconv3x3_blur_nhwc_tf32(const float* x, const float* wt, const float* scale, float* y, int B, int H, int W, int Cin, int Cout,
                                 float gain, void* stream);
 
+/* Adaptive discriminator augmentation (SURVEY A.4 item 15): ADA's integer "pixel blitting" and a per-image colour matrix in one
+ * pass over an NCHW fp32 image (csrc/gf_augment.cu).  x, y [B, C, H, W]:
+ *   y[b,c,y,x] = sum_j M_b[c][j] x[b,j,R_H(sy),R_W(sx)] + M_b[c][3]   (colour given; without it y[b,c,..] = x[b,c,R_H(sy),R_W(sx)])
+ * with (sx, sy) = D_b(x, y) - (tx_b, ty_b) and R_N the mirror that does not repeat the edge pixel: R_N(i) = -i for i < 0,
+ * 2(N-1) - i for i >= N.
+ *   geom  int32 [B, 4] = (code, tx, ty, unused).  D_b = rotation by k*90 degrees (k = code >> 1) after an x flip (code bit 0):
+ *         code 0..7 are the 8 dihedral maps of the grid onto itself.
+ *   color float [B, 12] = M_b, a row-major 3x4 matrix applied to (r, g, b, 1); NULL: geometry only.
+ * The parameters live on the device, so the kernels define every stored value: the code is masked to 3 bits, and when H != W its
+ * bit 1 is cleared (rotations by 90 / 270 degrees would transpose the grid, so they fall back to 0 / 180); tx and ty are clamped to
+ * [-(W-1), W-1] and [-(H-1), H-1], so one reflection brings every index back onto the grid.
+ * Errors, before touching the device: GF_ERR_INVALID for a NULL x / y / geom or a size <= 0; GF_ERR_UNSUPPORTED for H or W < 2,
+ * a colour matrix with C != 3, and H or W > 32768 or C*H*W >= 2^31.  y must not alias x. */
+int gf_augment_nchw(const float* x, float* y, const int* geom, const float* color, int B, int C, int H, int W, void* stream);
+
+/* The adjoint of gf_augment_nchw's linear part: gx = A^T gy, the transposed 3x3 colour matrix (the offset column does not take
+ * part) followed by the adjoint of the blit.  The mirror lets one source pixel be read by up to 2 outputs per axis; every source
+ * pixel gathers its preimages and sums them in a fixed order, without atomics, so the result is the same bits on every run and
+ * under CUDA-graph replay.  Same arguments, parameter rules and errors as gf_augment_nchw; gx must not alias gy. */
+int gf_augment_adjoint_nchw(const float* gy, float* gx, const int* geom, const float* color, int B, int C, int H, int W, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
