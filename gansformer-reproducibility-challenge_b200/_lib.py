@@ -34,7 +34,8 @@ EXPORTS = ("gf_attn_abi_version", "gf_last_error", "gf_attn_last_path", "gf_attn
            "gf_attn_centroid_stats", "gf_attn_centroid_bwd", "gf_attn_simplex_bwd_vjp", "gf_attn_centroid_bwd_vjp",
            "gf_attn_simplex_bwd_vjp_ex")
 # include/gf_ops.h
-OPS_EXPORTS = ("gf_chan_scale_nhwc", "gf_blur_up_nhwc", "gf_upsample2x_nchw", "gf_bias_act_nhwc", "gf_demod_coef", "gf_torgb_nhwc", "gf_fir4_nhwc", "gf_blur_up_phases_nhwc", "gf_torgb_scale_nhwc", "gf_mapping_fwd", "gf_conv3x3_pack_weights", "gf_conv3x3_nhwc_tf32", "gf_demod_coef_batch", "gf_upconv3x3_blur_nhwc_tf32", "gf_mapping_fwd_cond", "gf_augment_nchw", "gf_augment_adjoint_nchw")
+OPS_EXPORTS = ("gf_chan_scale_nhwc", "gf_blur_up_nhwc", "gf_upsample2x_nchw", "gf_bias_act_nhwc", "gf_demod_coef", "gf_torgb_nhwc", "gf_fir4_nhwc", "gf_blur_up_phases_nhwc", "gf_torgb_scale_nhwc", "gf_mapping_fwd", "gf_conv3x3_pack_weights", "gf_conv3x3_nhwc_tf32", "gf_demod_coef_batch", "gf_upconv3x3_blur_nhwc_tf32", "gf_mapping_fwd_cond", "gf_augment_nchw", "gf_augment_adjoint_nchw",
+               "gf_augment_resample_nchw", "gf_augment_resample_adjoint_nchw")
 
 
 class GfAttnDesc(ctypes.Structure):
@@ -121,6 +122,8 @@ def load() -> ctypes.CDLL:
     lib.gf_torgb_nhwc.argtypes = [c_void_p, c_void_p, c_void_p, c_int, c_void_p, ctypes.c_float, c_void_p, c_int, c_int, c_int, c_void_p]
     lib.gf_augment_nchw.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]
     lib.gf_augment_adjoint_nchw.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]
+    lib.gf_augment_resample_nchw.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]
+    lib.gf_augment_resample_adjoint_nchw.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]
     for name in OPS_EXPORTS:
         getattr(lib, name).restype = c_int
     for name in EXPORTS:

@@ -342,8 +342,15 @@ def mapping_fwd(z: torch.Tensor, w_eff: torch.Tensor, b_eff: torch.Tensor, w_avg
     return out
 
 
-def _augment_args(x: torch.Tensor, geom: torch.Tensor, color: Optional[torch.Tensor]):
-    """Checks of ops.augment (the same refusals as gf_augment_nchw); returns geom as int32 [B, 4] and color as [B, 12] on x's device."""
+def _augment_args(x: torch.Tensor, geom: torch.Tensor, color: Optional[torch.Tensor], frac: Optional[torch.Tensor] = None):
+    """Checks of ops.augment (the same refusals as gf_augment_nchw); returns geom as int32 [B, 4] and color as [B, 12] on x's device,
+    and with ``frac`` given (geom, color, frac) with frac as float32 [B, 6] on x's device."""
+    if frac is not None:
+        geom, color = _augment_args(x, geom, color)
+        B = x.shape[0]
+        if frac.dim() < 2 or frac.shape[0] != B or tuple(frac.shape[1:]) not in ((6,), (2, 3)):
+            raise ValueError(f"augment: frac must be [{B}, 6] or [{B}, 2, 3], got {tuple(frac.shape)}")
+        return geom, color, frac.reshape(B, 6).to(device=x.device, dtype=torch.float32).contiguous()
     if x.dim() != 4:
         raise ValueError(f"augment: x must be [B, C, H, W], got {tuple(x.shape)}")
     B, C, H, W = x.shape
@@ -384,29 +391,151 @@ def augment_index(geom: torch.Tensor, H: int, W: int) -> torch.Tensor:
     return (mirror(v - ty, H) * W + mirror(u - tx, W)).reshape(geom.shape[0], H * W)
 
 
-def augment_ref(x: torch.Tensor, geom: torch.Tensor, color: Optional[torch.Tensor] = None) -> torch.Tensor:
-    """Definition of ops.augment: an index gather (the blit), then the colour matrix per pixel.  Any dtype and device; torch
-    autograd differentiates it to any order."""
-    geom, color = _augment_args(x, geom, color)
+def augment_ref(x: torch.Tensor, geom: torch.Tensor, color: Optional[torch.Tensor] = None,
+                frac: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """Definition of ops.augment: an index gather (the blit) -- or, with ``frac``, the band-limited resampler for every image whose
+    fractional map is not the identity (resample_ref) -- then the colour matrix per pixel.  Any dtype and device; torch autograd
+    differentiates it to any order."""
+    if frac is not None:
+        geom, color, frac = _augment_args(x, geom, color, frac)
+    else:
+        geom, color = _augment_args(x, geom, color)
     B, C, H, W = x.shape
     idx = augment_index(geom, H, W)
     y = x.reshape(B, C, H * W).gather(2, idx[:, None].expand(B, C, H * W)).reshape(B, C, H, W)
+    if frac is not None:
+        y = _frac_select(y, resample_ref(x, geom, frac), frac, H, W)
     if color is None:
         return y
     M = color.reshape(B, 3, 4).to(x.dtype)
     return torch.einsum("bij,bjhw->bihw", M[:, :, :3], y) + M[:, :, 3, None, None]
 
 
-def augment_adjoint_ref(gy: torch.Tensor, geom: torch.Tensor, color: Optional[torch.Tensor] = None) -> torch.Tensor:
+def augment_adjoint_ref(gy: torch.Tensor, geom: torch.Tensor, color: Optional[torch.Tensor] = None,
+                        frac: Optional[torch.Tensor] = None) -> torch.Tensor:
     """Definition of the adjoint of ops.augment's linear part: the transposed 3x3 colour matrix (no offset), then a scatter-add
-    of every output pixel onto its source pixel."""
-    geom, color = _augment_args(gy, geom, color)
+    of every output pixel onto its source pixel (the blit), or with ``frac`` the adjoint of the resampler (torch autograd's
+    vector-Jacobian product of resample_ref) for every image whose fractional map is not the identity."""
+    if frac is not None:
+        geom, color, frac = _augment_args(gy, geom, color, frac)
+    else:
+        geom, color = _augment_args(gy, geom, color)
     B, C, H, W = gy.shape
     if color is not None:
         gy = torch.einsum("bij,bihw->bjhw", color.reshape(B, 3, 4).to(gy.dtype)[:, :, :3], gy)
     idx = augment_index(geom, H, W)
     gx = gy.new_zeros(B, C, H * W).scatter_add(2, idx[:, None].expand(B, C, H * W), gy.reshape(B, C, H * W))
-    return gx.reshape(B, C, H, W)
+    gx = gx.reshape(B, C, H, W)
+    if frac is not None:
+        with torch.enable_grad():
+            x0 = gy.new_zeros(gy.shape).requires_grad_(True)
+            (gr,) = torch.autograd.grad(resample_ref(x0, geom, frac), x0, gy, create_graph=gy.requires_grad)
+        gx = _frac_select(gx, gr, frac, H, W)
+    return gx
+
+
+# ------------------------------------------------------------------------------------------------ ADA's fractional geometry
+# The 12 taps of the Daubechies symlet sym6: orthonormal under even shifts (sum sqrt 2), six vanishing moments.  ADA's geometric
+# low-pass; the resampler uses it normalised to sum 1.
+SYM6 = (0.015404109327027373, 0.0034907120842174702, -0.11799011114819057, -0.048311742585633, 0.4910559419267466,
+        0.787641141030194, 0.3379294217276218, -0.07263752278646252, -0.021060292512300564, 0.04472490177066578,
+        0.0017677118642428036, -0.007800708325034148)
+FRAC_SV_MAX = 16.0          # domain of a fractional map: singular values of its 2x2 part in [1/16, 16] ...
+FRAC_T_MAX = 64             # ... and |translation| <= 64 * max(H, W) in each coordinate
+
+
+def sym6_filter(device=None, dtype=torch.float64) -> torch.Tensor:
+    f = torch.tensor(SYM6, dtype=torch.float64)
+    return (f / f.sum()).to(device=device, dtype=dtype)
+
+
+def frac_flags(frac: torch.Tensor, H: int, W: int):
+    """(identity [B], in_domain [B]) of fractional maps [B, 6]: exactly [1, 0, 0; 0, 1, 0]; finite, both singular values of the 2x2
+    part in [1/16, 16] and |translation| <= 64 * max(H, W) in each coordinate."""
+    f = frac.reshape(-1, 6).double()
+    ident = (f == f.new_tensor([1.0, 0.0, 0.0, 0.0, 1.0, 0.0])).all(dim=1)
+    a, b, c, d = f[:, 0], f[:, 1], f[:, 3], f[:, 4]
+    s2 = a * a + b * b + c * c + d * d
+    det = (a * d - b * c).abs()
+    smax2 = (s2 + (s2 * s2 - 4 * det * det).clamp(min=0).sqrt()) / 2
+    smin2 = det * det / smax2
+    ok = (torch.isfinite(f).all(dim=1) & (smax2 <= FRAC_SV_MAX ** 2) & (smin2 >= FRAC_SV_MAX ** -2)
+          & (f[:, [2, 5]].abs() <= FRAC_T_MAX * max(H, W)).all(dim=1))
+    return ident, ok
+
+
+def _frac_select(blit: torch.Tensor, res: torch.Tensor, frac: torch.Tensor, H: int, W: int) -> torch.Tensor:
+    """Per image: the blit where the fractional map is the identity, else the resampled image, NaN outside the domain."""
+    ident, ok = frac_flags(frac, H, W)
+    ident, ok = ident.to(blit.device)[:, None, None, None], ok.to(blit.device)[:, None, None, None]
+    return torch.where(ident, blit, torch.where(ok, res, torch.full_like(res, float("nan"))))
+
+
+def resample_map(geom: torch.Tensor, frac: torch.Tensor, H: int, W: int, dtype=torch.float64):
+    """(L [B, 2, 2], e [B, 2]): the point q = (qx, qy) of the 2x output grid (q = 1 .. 2N + 10 per axis; output pixel o sits at
+    q = 2o + 6) reads the 2x source grid at nu = L q + e, nu = 2 * (source pixel index).  The composition of the fractional map
+    F^-1 = frac[b] (centred pixel coordinates) and then the blit B^-1(v) = D v - t of geom[b] (code and t under gf_augment_nchw's
+    rules)."""
+    B = geom.shape[0]
+    g = geom.to(torch.int64)
+    code = g[:, 0] & 7
+    if H != W:
+        code = code & 5
+    flip = (1 - 2 * (code & 1)).to(dtype)
+    k = code >> 1
+    cs = torch.where(k == 0, 1, torch.where(k == 2, -1, 0)).to(dtype)
+    sn = torch.where(k == 1, 1, torch.where(k == 3, -1, 0)).to(dtype)
+    D = torch.stack([torch.stack([cs * flip, sn], 1), torch.stack([-sn * flip, cs], 1)], 1)        # (u, v) = R_k (flip * x, y)
+    t = torch.stack([g[:, 1].clamp(-(W - 1), W - 1), g[:, 2].clamp(-(H - 1), H - 1)], 1).to(dtype)
+    A = frac.reshape(B, 2, 3).to(dtype=dtype, device=geom.device)
+    L = D @ A[:, :, :2]
+    cen = torch.tensor([(W - 1) / 2, (H - 1) / 2], dtype=dtype, device=geom.device)
+    off = (D @ (A[:, :, 2] - A[:, :, :2] @ cen)[:, :, None])[:, :, 0] - t + cen
+    return L, 2 * off - 6 * L.sum(dim=2)
+
+
+def resample_ref(x: torch.Tensor, geom: torch.Tensor, frac: torch.Tensor, taps: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """Definition of the resampler (SURVEY A.4 item 16), every image, in x's dtype: (1) mirror-extend the source by R_N to
+    [-(N-1), 2(N-1)] per axis, zeros beyond; (2) upsample 2x with the normalised sym6 taps as a convolution, gain 2 per axis, pads
+    (6, 5); (3) sample that grid bilinearly, zeros outside it, at nu = L q + e (resample_map) for the (2N + 10)^2 points of the 2x output
+    grid that (4) the 2x downsampling reads: the same taps as a correlation, pads (-1, -1).  ``taps`` replaces the 12 taps (the
+    tests' magnitude companion runs |taps|)."""
+    B, C, H, W = x.shape
+    dev, dt = x.device, x.dtype
+    f = sym6_filter(dev, dt) if taps is None else taps.to(device=dev, dtype=dt)
+    fl = f.flip(0)
+
+    def mirror(N):
+        i = torch.arange(-(N - 1), 2 * N - 1, device=dev)
+        return torch.where(i < 0, -i, torch.where(i >= N, 2 * (N - 1) - i, i))
+    E = x[:, :, mirror(H)][:, :, :, mirror(W)].reshape(B * C, 1, 3 * H - 2, 3 * W - 2)
+    Z = E.new_zeros(B * C, 1, 6 * H - 4, 6 * W - 4)
+    Z[:, :, ::2, ::2] = E
+    Z = F.pad(Z, [6, 5, 6, 5])
+    U = F.conv2d(F.conv2d(Z, 2 * fl.reshape(1, 1, 1, 12)), 2 * fl.reshape(1, 1, 12, 1))       # [B*C, 1, 6H-4, 6W-4]
+    UH, UW = 6 * H - 4, 6 * W - 4
+    ok = frac_flags(frac, H, W)[1].to(frac.device)[:, None]                                     # outside the domain: any finite map
+    frac = torch.where(ok, frac.reshape(B, 6), frac.new_tensor([1.0, 0.0, 0.0, 0.0, 1.0, 0.0]))
+    L, e = resample_map(geom.to(dev), frac, H, W, dt)
+    qx = torch.arange(1, 2 * W + 11, device=dev, dtype=dt)[None, None, :]
+    qy = torch.arange(1, 2 * H + 11, device=dev, dtype=dt)[None, :, None]
+    bl = lambda v: v[:, None, None]
+    nx = bl(L[:, 0, 0]) * qx + bl(L[:, 0, 1]) * qy + bl(e[:, 0]) + 2 * (W - 1)                      # index into U
+    ny = bl(L[:, 1, 0]) * qx + bl(L[:, 1, 1]) * qy + bl(e[:, 1]) + 2 * (H - 1)
+    x0, y0 = nx.floor(), ny.floor()
+    ax, ay = nx - x0, ny - y0
+    Uf = U.reshape(B, C, UH * UW)
+    V = 0
+    for dy, wy in ((0, 1 - ay), (1, ay)):
+        for dx, wx in ((0, 1 - ax), (1, ax)):
+            ix, iy = x0 + dx, y0 + dy
+            inside = (ix >= 0) & (ix < UW) & (iy >= 0) & (iy < UH)
+            idx = (iy.clamp(0, UH - 1) * UW + ix.clamp(0, UW - 1)).long().reshape(B, 1, -1).expand(B, C, -1)
+            w = torch.where(inside, wx * wy, torch.zeros_like(wx)).reshape(B, 1, -1)
+            V = V + w * Uf.gather(2, idx)
+    V = V.reshape(B * C, 1, 2 * H + 10, 2 * W + 10)
+    y = F.conv2d(F.conv2d(V, f.reshape(1, 1, 1, 12), stride=(1, 2)), f.reshape(1, 1, 12, 1), stride=(2, 1))
+    return y.reshape(B, C, H, W)
 
 
 def _augment_native(name: str, x: torch.Tensor, geom: torch.Tensor, color: Optional[torch.Tensor]) -> torch.Tensor:
@@ -455,11 +584,59 @@ class _AugmentAdjoint(torch.autograd.Function):
         return _Augment.apply(ggx, geom, _linear_part(color)), None, None
 
 
-def augment(x: torch.Tensor, geom: torch.Tensor, color: Optional[torch.Tensor] = None) -> torch.Tensor:
-    """Adaptive discriminator augmentation of a batch (SURVEY A.4 item 15): x [B, C, H, W] -> the same shape, image b blitted by its
-    geom[b] = (dihedral code, tx, ty, unused) and, with color [B, 12] (row-major 3x4 matrices on (r, g, b, 1), C == 3), recoloured.
-    See include/gf_ops.h for the exact map.  CUDA fp32 tensors run gf_augment_nchw, and its adjoint in the backward (to any order);
-    anything else runs the definition augment_ref."""
+def _augment_resample_native(name: str, x: torch.Tensor, geom: torch.Tensor, color: Optional[torch.Tensor],
+                             frac: torch.Tensor) -> torch.Tensor:
+    xc = x.detach().contiguous()
+    B, C, H, W = xc.shape
+    y = torch.empty_like(xc)
+    with torch.cuda.device(x.device):
+        _lib.check(getattr(_lib.load(), name)(xc.data_ptr(), y.data_ptr(), geom.data_ptr(), frac.data_ptr(),
+                                              None if color is None else color.data_ptr(), B, C, H, W, _stream(x.device)), name)
+    return y
+
+
+class _AugmentResample(torch.autograd.Function):
+    """gf_augment_resample_nchw, differentiable to any order like _Augment: its gradient is _AugmentResampleAdjoint, whose gradient
+    is the linear part of the map again."""
+
+    @staticmethod
+    def forward(ctx, x, geom, color, frac):
+        ctx.save_for_backward(geom, color, frac)
+        return _augment_resample_native("gf_augment_resample_nchw", x, geom, color, frac)
+
+    @staticmethod
+    def backward(ctx, gy):
+        geom, color, frac = ctx.saved_tensors
+        return _AugmentResampleAdjoint.apply(gy, geom, color, frac), None, None, None
+
+
+class _AugmentResampleAdjoint(torch.autograd.Function):
+    """gf_augment_resample_adjoint_nchw: gx = A^T gy (the offset does not take part)."""
+
+    @staticmethod
+    def forward(ctx, gy, geom, color, frac):
+        ctx.save_for_backward(geom, color, frac)
+        return _augment_resample_native("gf_augment_resample_adjoint_nchw", gy, geom, color, frac)
+
+    @staticmethod
+    def backward(ctx, ggx):
+        geom, color, frac = ctx.saved_tensors
+        return _AugmentResample.apply(ggx, geom, _linear_part(color), frac), None, None, None
+
+
+def augment(x: torch.Tensor, geom: torch.Tensor, color: Optional[torch.Tensor] = None,
+            frac: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """Adaptive discriminator augmentation of a batch (SURVEY A.4 items 15, 16): x [B, C, H, W] -> the same shape, image b blitted by
+    its geom[b] = (dihedral code, tx, ty, unused) and, with color [B, 12] (row-major 3x4 matrices on (r, g, b, 1), C == 3), recoloured.
+    With frac [B, 6] (row-major 2x3 inverse maps F_b^-1 in centred pixel coordinates) every image whose F_b^-1 is not exactly the
+    identity is resampled through the composition of F_b^-1 and its blit instead (ADA's general geometry, band-limited).
+    See include/gf_ops.h for the exact map.  CUDA fp32 tensors run gf_augment_nchw (gf_augment_resample_nchw with frac), and its
+    adjoint in the backward (to any order); anything else runs the definition augment_ref."""
+    if frac is not None:
+        geom, color, frac = _augment_args(x, geom, color, frac)
+        if x.is_cuda and x.dtype == torch.float32:
+            return _AugmentResample.apply(x, geom, color, frac)
+        return augment_ref(x, geom, color, frac)
     geom, color = _augment_args(x, geom, color)
     if x.is_cuda and x.dtype == torch.float32:
         return _Augment.apply(x, geom, color)

@@ -227,7 +227,8 @@ class TrainConfig:
     pl_batch_shrink: int = 2            # the path-length phase runs on the first B // 2 latents
     pl_decay: float = 0.01              # decay of the running mean of the path lengths
     style_mixing: float = 0.0           # probability of style mixing per generator forward (StyleGAN2 / GANsformer: 0.9); 0 = off
-    augment: str = ""                   # discriminator augmentation: "" = off, "bc" = all of AUGMENT_OPS, or a comma list of them
+    augment: str = ""                   # discriminator augmentation: "" = off, "bc" = all of AUGMENT_OPS, "bgc" = those and GEOM_OPS,
+                                        # or a comma list of names from both
     augment_p: float = 0.0              # starting augmentation strength p
     ada_target: Optional[float] = None  # adaptive p: target of the mean sign of the real logits (ADA: 0.6); None = p stays put
     ada_interval: int = 4               # steps between updates of p
@@ -235,19 +236,79 @@ class TrainConfig:
 
 
 AUGMENT_OPS = ("xflip", "rotate90", "xint", "brightness", "contrast", "lumaflip", "hue", "saturation")
+GEOM_OPS = ("scale", "rotate", "aniso", "xfrac")                     # ADA's general geometry (SURVEY A.4 item 16)
+_ADA_ORDER = AUGMENT_OPS[:3] + GEOM_OPS + AUGMENT_OPS[3:]
 
 
 def parse_augment(spec: str) -> tuple:
-    """TrainConfig.augment -> the enabled transforms, in AUGMENT_OPS order: "" none, "bc" all eight, else a comma list of names."""
+    """TrainConfig.augment -> the enabled transforms, in ADA's order: "" none, "bc" the eight of AUGMENT_OPS, "bgc" those and
+    GEOM_OPS, else a comma list of names from both."""
     if not spec:
         return ()
     if spec == "bc":
         return AUGMENT_OPS
+    if spec == "bgc":
+        return _ADA_ORDER
     names = {s.strip() for s in spec.split(",")}
-    unknown = sorted(names - set(AUGMENT_OPS))
+    unknown = sorted(names - set(_ADA_ORDER))
     if unknown:
-        raise ValueError(f"unknown augmentation(s) {unknown}: use 'bc' or a comma list of {AUGMENT_OPS}")
-    return tuple(n for n in AUGMENT_OPS if n in names)
+        raise ValueError(f"unknown augmentation(s) {unknown}: use 'bc', 'bgc' or a comma list of {_ADA_ORDER}")
+    return tuple(n for n in _ADA_ORDER if n in names)
+
+
+def sample_augment_frac(ops_: tuple, p, B: int, H: int, W: int, device):
+    """Per-image fractional inverse maps F^-1 [B, 6] for ops.augment (row-major 2x3, centred pixel coordinates), or None when no
+    GEOM_OPS transform is enabled (then no random number is drawn).  Drawn on ``device`` without a host sync (capturable), the same
+    random numbers whatever p is; a transform that does not apply contributes exactly the identity, so p = 0 gives the identity.
+
+    F^-1 = S^-1 R_pre^-1 A^-1 R_post^-1 T^-1 (ADA's order): scale s = exp2(N(0, 0.2^2)), S^-1 = diag(1/s, 1/s); rotate: two
+    rotations by U(-pi, pi), each applying with p_rot = 1 - sqrt(1 - p), so that at least one applies with probability p; aniso
+    a = exp2(N(0, 0.2^2)), A^-1 = diag(1/a, a); xfrac t = N(0, 0.125^2) * (W, H) pixels, T^-1 a translation by -t."""
+    if not any(n in ops_ for n in GEOM_OPS):
+        return None
+    eye = torch.eye(3, device=device).expand(B, 3, 3)
+    G = eye
+
+    def applies(q):
+        return torch.rand(B, device=device) < q
+
+    def then(T, a):                                  # G <- G T^-1 where the transform applies, else G I (exact)
+        T = torch.where(a[:, None, None], T, eye)    # products and sums, not a matmul: TF32 matmuls would round the maps
+        return (G[:, :, :, None] * T[:, None, :, :]).sum(dim=2)
+
+    def diag(sx, sy):
+        T = eye.clone()
+        T[:, 0, 0], T[:, 1, 1] = sx, sy
+        return T
+
+    def rot():
+        th = (torch.rand(B, device=device) * 2 - 1) * math.pi
+        T = eye.clone()
+        c, s = torch.cos(th), torch.sin(th)
+        T[:, 0, 0], T[:, 0, 1], T[:, 1, 0], T[:, 1, 1] = c, -s, s, c
+        return T
+    p_rot = 1 - (1 - p) ** 0.5
+    if "scale" in ops_:
+        a = applies(p)
+        s = torch.exp2(torch.randn(B, device=device) * 0.2)
+        G = then(diag(1 / s, 1 / s), a)
+    if "rotate" in ops_:
+        a = applies(p_rot)
+        G = then(rot(), a)
+    if "aniso" in ops_:
+        a = applies(p)
+        s = torch.exp2(torch.randn(B, device=device) * 0.2)
+        G = then(diag(1 / s, s), a)
+    if "rotate" in ops_:
+        a = applies(p_rot)
+        G = then(rot(), a)
+    if "xfrac" in ops_:
+        a = applies(p)
+        t = torch.randn(B, 2, device=device) * 0.125
+        T = eye.clone()
+        T[:, 0, 2], T[:, 1, 2] = -t[:, 0] * W, -t[:, 1] * H
+        G = then(T, a)
+    return G[:, :2, :].reshape(B, 6).contiguous()
 
 
 def sample_augment(ops_: tuple, p, B: int, H: int, W: int, device):
@@ -399,7 +460,10 @@ class Trainer:
             return img
         B, _, H, W = img.shape
         geom, color = sample_augment(self.augment_ops, self.augment_p, B, H, W, img.device)
-        return augment(img, geom, color)
+        frac = sample_augment_frac(self.augment_ops, self.augment_p, B, H, W, img.device)
+        if frac is None:
+            return augment(img, geom, color)
+        return augment(img, geom, color, frac)
 
     def _ada_accumulate(self, logit_real: torch.Tensor):
         """Adds (sum of the signs, count) of this step's real logits, summed over ranks, to the ADA accumulators."""

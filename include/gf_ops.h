@@ -143,6 +143,24 @@ int gf_augment_nchw(const float* x, float* y, const int* geom, const float* colo
  * under CUDA-graph replay.  Same arguments, parameter rules and errors as gf_augment_nchw; gx must not alias gy. */
 int gf_augment_adjoint_nchw(const float* gy, float* gx, const int* geom, const float* color, int B, int C, int H, int W, void* stream);
 
+/* ADA's general geometry (SURVEY A.4 item 16): gf_augment_nchw with, per image, a fractional inverse map
+ *   frac  float [B, 6] = F_b^-1, a row-major 2x3 affine map in centred pixel coordinates (pixel (i, j) sits at (j - (W-1)/2, i - (H-1)/2)).
+ * An image whose F_b^-1 is exactly the identity is blitted, bit for bit as gf_augment_nchw.  Every other image reads the source at
+ * B_b^-1(F_b^-1(u)), B_b^-1(v) = D_b v - t_b the blit of geom[b], through ADA's band-limited resampler: mirror extension by R_N to
+ * [-(N-1), 2(N-1)] per axis (zeros beyond), 2x upsampling with the 12-tap sym6 low-pass (normalised to sum 1, a convolution, gain 2
+ * per axis, pads (6, 5)), bilinear sampling of that grid (zeros outside it) on a 2x output grid of (N + 6) * 2 points per axis with
+ * ADA's -0.5 origin shift between the grids, and 2x downsampling with the same taps as a correlation, pads (-1, -1).  Colour after.
+ * Domain, per image: finite entries, both singular values of the 2x2 part in [1/16, 16], |translation| <= 64 * max(H, W) in each
+ * coordinate; an image outside it is written as NaN (other images are untouched).  One launch on `stream`, no workspace, no host
+ * sync, no atomics.  The arguments, parameter rules and errors of gf_augment_nchw, plus GF_ERR_INVALID for a NULL frac. */
+int gf_augment_resample_nchw(const float* x, float* y, const int* geom, const float* frac, const float* color, int B, int C, int H, int W,
+                             void* stream);
+
+/* The adjoint of gf_augment_resample_nchw's linear part: gx = A^T gy (the colour offset does not take part), gathered per source
+ * pixel over the mirrored copies of it that the output can reach, in a fixed order: the same bits on every run and under replay. */
+int gf_augment_resample_adjoint_nchw(const float* gy, float* gx, const int* geom, const float* frac, const float* color, int B, int C,
+                                     int H, int W, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
