@@ -116,6 +116,18 @@ int gf_attn_debug_layout(const gf_attn_desc* desc, long long* out, int n) {
   return GF_OK;
 }
 
+int gf_attn_debug_tc_schedule(const gf_attn_desc* desc, int rule, int* out, int n) {
+  Layout L;
+  int rc = make_layout(desc, &L);
+  if (rc) return rc;
+  if ((rc = check_device())) return rc;
+  int v[4] = {0, 0, 0, 0};
+  if ((rc = tc_schedule(L, desc, rule, v))) return rc;
+  if (desc->flags & GF_FLAG_FP32_EXACT) v[0] = v[1] = v[2] = v[3] = 0;   // the CUDA-core kernel serves it
+  for (int i = 0; i < n && i < 4; ++i) out[i] = v[i];
+  return GF_OK;
+}
+
 int gf_attn_folded_floats(const gf_attn_desc* desc, size_t* out_floats) {
   Layout L;
   int rc = make_layout(desc, &L);

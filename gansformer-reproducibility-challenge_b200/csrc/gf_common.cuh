@@ -149,5 +149,7 @@ int centroid_pass_tc(const Layout& L, const float* X, float* ws, cudaStream_t st
 // wgmma / TMA path (gf_tc.cu).  tc_supported() says whether the shape is served by it.
 bool tc_supported(const Layout& L, const gf_attn_desc* d);
 int token_pass_tc(const Layout& L, const gf_attn_desc* d, const float* X, float* Xout, float* att, float* ws, const gf_attn_postop* post, cudaStream_t st);
+// launch configuration of token_pass_tc under a schedule rule (see gf_attn_debug_tc_schedule), which becomes the calling thread's
+int tc_schedule(const Layout& L, const gf_attn_desc* d, int rule, int* out4);
 
 }  // namespace gf

@@ -5,7 +5,7 @@
 // transformer_layer (Q projection folded into K', QK^T, softmax, PV), integrate and att_norm.  Same algorithm as
 // oracle/folded.py per_token(); operands of both contractions are rounded to TF32 by the tensor cores.
 //
-// One persistent CTA per SM, 9 warps:
+// Persistent CTAs (one or two per SM, see schedule()), 9 warps each:
 //   warp 8       TMA producer: X slabs (128 tokens x 32 channels, 16 KB, SWIZZLE_128B) into a ring; K'/V^T per image
 //   warps 0-3,   two consumer warpgroups; warpgroup g owns token rows [64 g, 64 g + 64) of every tile and runs, for them:
 //   warps 4-7      GEMM1  S[64,KP] = X[64,C] . K'^T (wgmma, A and B from shared memory), the LayerNorm statistics of the rows
@@ -91,8 +91,8 @@ __device__ __forceinline__ float quad_max(float v) {
   return fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 2));
 }
 
-template <int KP, int NS, int MODE, bool TWO_PASS>
-__global__ void __launch_bounds__(NUM_THREADS, 1)
+template <int KP, int NS, int MODE, bool TWO_PASS, int CTAS>
+__global__ void __launch_bounds__(NUM_THREADS, CTAS)
 token_tc_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmO0, const __grid_constant__ CUtensorMap tmO1,
                 const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV, const Params P) {
   using CF = Cfg<KP, NS, MODE>;
@@ -517,14 +517,60 @@ static int stages_for(int smem_limit) {
 #endif
 template <int NS> constexpr bool two_pass_shape() { return NS >= GF_TWO_PASS_MIN_NS; }
 template <int NS> constexpr int min_stages() { return two_pass_shape<NS>() ? 4 : NS; }
+// Two CTAs per SM give every SM a second, independent chain GEMM1 -> statistics -> softmax -> GEMM2 -> modulation -> store, so
+// one CTA's loads and stores overlap the other's arithmetic.  Register budget: 18 warps on the 4 SM sub-partitions (16 K registers
+// each, 5 warps on some) leave 96 per thread under __launch_bounds__(288, 2).  ptxas (sm_90a, -Xptxas -v) fits every instantiation
+// there without spills (85-96) except KP = 32 with both integrations, which needs 120 at one CTA per SM.
+template <int KP, int MODE> constexpr bool two_cta_regs() { return KP == 16 || MODE != GF_INT_BOTH; }
+
+// shared memory one CTA may use when `ctas` CTAs share an SM
+static int smem_per_cta(int ctas) {
+  if (ctas == 1) return device_smem_optin();
+  static int per_sm = -1, reserved = -1;
+  if (per_sm < 0) {
+    int dev = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&per_sm, cudaDevAttrMaxSharedMemoryPerMultiprocessor, dev) != cudaSuccess ||
+        cudaDeviceGetAttribute(&reserved, cudaDevAttrReservedSharedMemoryPerBlock, dev) != cudaSuccess) { per_sm = 0; reserved = 0; }
+  }
+  const int v = per_sm / ctas - reserved;
+  return v < device_smem_optin() ? v : device_smem_optin();
+}
+
+// Launch configuration of one shape: CTAs per SM and the per-CTA ring.  Rule 0 is the library's; rule 1 is the configuration
+// before two CTAs per SM (one CTA, the deepest ring), kept so the tests can check the two give the same bits.
+struct Sched { int ctas, nstages; };
+static thread_local int g_sched_rule = 0;
 
 template <int KP, int NS, int MODE>
-static int launch(const Layout& L, const gf_attn_desc* d, const float* X, float* Xout, float* att, float* ws, const gf_attn_postop* post, cudaStream_t st) {
+static Sched schedule(int rule) {
+  if (rule == 0 && two_cta_regs<KP, MODE>()) {
+    const int st2 = stages_for<KP, NS, MODE>(smem_per_cta(2));
+    if (st2 >= min_stages<NS>()) return {2, st2};
+  }
+  return {1, stages_for<KP, NS, MODE>(smem_per_cta(1))};
+}
+
+template <int KP, int NS, int MODE, int CTAS>
+static int run(const Layout& L, const gf_attn_desc* d, const float* X, float* Xout, float* att, float* ws, const gf_attn_postop* post, cudaStream_t st,
+               int nst, int* grid_out) {
   using CF = Cfg<KP, NS, MODE>;
   constexpr bool TWO = two_pass_shape<NS>();
-  int nst = stages_for<KP, NS, MODE>(device_smem_optin());
-  if (const char* e = getenv("GF_TC_MAX_STAGES")) { const int v = atoi(e); if (v >= min_stages<NS>() && v < nst) nst = v; }   // tuning aid: ring-depth sensitivity
-  if (nst < min_stages<NS>()) { set_error("tensor path: shared memory too small for C=%d KP=%d mode=%d", L.C, KP, MODE); return GF_ERR_UNSUPPORTED; }
+  const int smem_bytes = CF::FIXED_BYTES + nst * SLAB_BYTES + 1024;
+  auto kern = token_tc_kernel<KP, NS, MODE, TWO, CTAS>;
+  // resident CTAs per SM as the occupancy calculator reports them for this ring (cached per ring size)
+  static int occ_bytes = -1, occ = 0;
+  if (occ_bytes != smem_bytes) {
+    GF_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
+    GF_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
+    GF_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, NUM_THREADS, smem_bytes));
+    if (occ < 1) { set_error("tensor path: no CTA of C=%d KP=%d mode=%d fits an SM", L.C, KP, MODE); return GF_ERR_UNSUPPORTED; }
+    occ_bytes = smem_bytes;
+  }
+  const int tiles_per_image = (L.n + TILE - 1) / TILE;
+  const long long total_tiles = (long long)L.B * tiles_per_image;
+  long long grid = (long long)occ * device_sms();          // contiguous tile ranges, one per resident CTA
+  if (grid > total_tiles) grid = total_tiles;
+  if (grid_out) { *grid_out = (int)grid; return GF_OK; }
   CUtensorMap tmX, tmO0, tmO1, tmK, tmV;
   int rc;
   const uint64_t rows = (uint64_t)L.B * L.n;
@@ -543,9 +589,9 @@ static int launch(const Layout& L, const gf_attn_desc* d, const float* X, float*
   P.norm_layer = d->norm == GF_NORM_LAYER ? 1 : 0;
   P.nstages = nst;
   P.nwg = nwg;
-  P.tiles_per_image = (L.n + TILE - 1) / TILE;
+  P.tiles_per_image = tiles_per_image;
   P.rows = trows;
-  P.total_tiles = (long long)L.B * P.tiles_per_image;
+  P.total_tiles = total_tiles;
   P.has_post = post ? 1 : 0;
   P.pbias = post ? post->bias : nullptr; P.pnoise = post ? post->noise : nullptr; P.pstrength = post ? post->strength : nullptr;
   P.pnoise_bstride = post ? post->noise_bstride : 0; P.pact = post ? post->act : 0; P.pgain = post ? post->gain : 1.f;
@@ -555,23 +601,38 @@ static int launch(const Layout& L, const gf_attn_desc* d, const float* X, float*
   P.heads = L.heads; P.seg_shift = L.seg == 8 ? 3 : (L.seg == 16 ? 4 : 5);
   if ((rc = dropout_args(post, &P.dp))) return rc;
   P.cb = ws + L.w_CB;
-  const int smem_bytes = CF::FIXED_BYTES + nst * SLAB_BYTES + 1024;
-  auto kern = token_tc_kernel<KP, NS, MODE, TWO>;
-  GF_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
-  long long grid = device_sms();
-  if (grid > P.total_tiles) grid = P.total_tiles;
   kern<<<(unsigned)grid, NUM_THREADS, smem_bytes, st>>>(tmX, tmO0, tmO1, tmK, tmV, P);
   GF_LAUNCH_OK();
   set_path(GF_PATH_WGMMA_TF32);
   return GF_OK;
 }
 
+template <int KP, int NS, int MODE>
+static int launch(const Layout& L, const gf_attn_desc* d, const float* X, float* Xout, float* att, float* ws, const gf_attn_postop* post, cudaStream_t st,
+                  int* sched_out = nullptr) {
+  const Sched s = schedule<KP, NS, MODE>(g_sched_rule);
+  int nst = s.nstages;
+  if (const char* e = getenv("GF_TC_MAX_STAGES")) { const int v = atoi(e); if (v >= min_stages<NS>() && v < nst) nst = v; }   // tuning aid: ring-depth sensitivity
+  if (nst < min_stages<NS>()) { set_error("tensor path: shared memory too small for C=%d KP=%d mode=%d", L.C, KP, MODE); return GF_ERR_UNSUPPORTED; }
+  int grid = 0;
+  int* g = sched_out ? &grid : nullptr;
+  int rc;
+  if constexpr (two_cta_regs<KP, MODE>()) {
+    rc = s.ctas == 2 ? run<KP, NS, MODE, 2>(L, d, X, Xout, att, ws, post, st, nst, g) : run<KP, NS, MODE, 1>(L, d, X, Xout, att, ws, post, st, nst, g);
+  } else {
+    rc = run<KP, NS, MODE, 1>(L, d, X, Xout, att, ws, post, st, nst, g);
+  }
+  if (sched_out && rc == GF_OK) { sched_out[0] = two_pass_shape<NS>() ? 1 : 0; sched_out[1] = s.ctas; sched_out[2] = nst; sched_out[3] = grid; }
+  return rc;
+}
+
 template <int KP, int NS>
-static int launch_mode(const Layout& L, const gf_attn_desc* d, const float* X, float* Xout, float* att, float* ws, const gf_attn_postop* post, cudaStream_t st) {
+static int launch_mode(const Layout& L, const gf_attn_desc* d, const float* X, float* Xout, float* att, float* ws, const gf_attn_postop* post, cudaStream_t st,
+                       int* sched_out) {
   switch (d->integration) {
-    case GF_INT_MUL: return launch<KP, NS, GF_INT_MUL>(L, d, X, Xout, att, ws, post, st);
-    case GF_INT_ADD: return launch<KP, NS, GF_INT_ADD>(L, d, X, Xout, att, ws, post, st);
-    default: return launch<KP, NS, GF_INT_BOTH>(L, d, X, Xout, att, ws, post, st);
+    case GF_INT_MUL: return launch<KP, NS, GF_INT_MUL>(L, d, X, Xout, att, ws, post, st, sched_out);
+    case GF_INT_ADD: return launch<KP, NS, GF_INT_ADD>(L, d, X, Xout, att, ws, post, st, sched_out);
+    default: return launch<KP, NS, GF_INT_BOTH>(L, d, X, Xout, att, ws, post, st, sched_out);
   }
 }
 
@@ -595,12 +656,13 @@ static bool fits_ns(int ns, int integration, int limit) {
 }
 
 template <int KP>
-static int launch_ns(int ns, const Layout& L, const gf_attn_desc* d, const float* X, float* Xout, float* att, float* ws, const gf_attn_postop* post, cudaStream_t st) {
+static int launch_ns(int ns, const Layout& L, const gf_attn_desc* d, const float* X, float* Xout, float* att, float* ws, const gf_attn_postop* post, cudaStream_t st,
+                     int* sched_out = nullptr) {
   switch (ns) {
-    case 2: return launch_mode<KP, 2>(L, d, X, Xout, att, ws, post, st);
-    case 4: return launch_mode<KP, 4>(L, d, X, Xout, att, ws, post, st);
-    case 8: return launch_mode<KP, 8>(L, d, X, Xout, att, ws, post, st);
-    default: return launch_mode<KP, 16>(L, d, X, Xout, att, ws, post, st);
+    case 2: return launch_mode<KP, 2>(L, d, X, Xout, att, ws, post, st, sched_out);
+    case 4: return launch_mode<KP, 4>(L, d, X, Xout, att, ws, post, st, sched_out);
+    case 8: return launch_mode<KP, 8>(L, d, X, Xout, att, ws, post, st, sched_out);
+    default: return launch_mode<KP, 16>(L, d, X, Xout, att, ws, post, st, sched_out);
   }
 }
 
@@ -620,6 +682,14 @@ bool tc_supported(const Layout& L, const gf_attn_desc* d) {
 int token_pass_tc(const Layout& L, const gf_attn_desc* d, const float* X, float* Xout, float* att, float* ws, const gf_attn_postop* post, cudaStream_t st) {
   if (L.KP == 16) return tc::launch_ns<16>(L.C / 32, L, d, X, Xout, att, ws, post, st);
   return tc::launch_ns<32>(L.C / 32, L, d, X, Xout, att, ws, post, st);
+}
+
+int tc_schedule(const Layout& L, const gf_attn_desc* d, int rule, int* out4) {
+  if (rule != 0 && rule != 1) { set_error("tc_schedule: rule must be 0 or 1, got %d", rule); return GF_ERR_INVALID; }
+  tc::g_sched_rule = rule;
+  if (!tc_supported(L, d)) { out4[0] = out4[1] = out4[2] = out4[3] = 0; return GF_OK; }
+  if (L.KP == 16) return tc::launch_ns<16>(L.C / 32, L, d, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, out4);
+  return tc::launch_ns<32>(L.C / 32, L, d, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, out4);
 }
 
 }  // namespace gf

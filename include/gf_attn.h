@@ -142,6 +142,12 @@ int gf_attn_tc_eligible(const gf_attn_desc* desc);
  * five duplex offsets w_PART, w_XBAR, w_M, w_Rt2 and w_Ct2 are 0 for a simplex layer.  Values past the 15th are not written. */
 int gf_attn_debug_layout(const gf_attn_desc* desc, long long* out, int n);
 
+/* Debug aid for the kernel tests: up to n of {two_pass, ctas_per_sm, ring_stages, grid} of the wgmma stage-T launch of this layer
+ * (all 0 when the CUDA-core kernel serves it) under schedule `rule`, which also becomes the rule of the calling thread's following
+ * stage-T launches: 0 = the library's (the default: two CTAs per SM where registers and shared memory allow), 1 = one CTA per SM
+ * with the deepest ring.  Both compute the same bits.  Needs the device. */
+int gf_attn_debug_tc_schedule(const gf_attn_desc* desc, int rule, int* out, int n);
+
 /* Size in floats of the folded-weight buffer (stage W output + its scratch). */
 int gf_attn_folded_floats(const gf_attn_desc* desc, size_t* out_floats);
 
