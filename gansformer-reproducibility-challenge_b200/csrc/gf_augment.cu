@@ -593,6 +593,180 @@ __global__ void __launch_bounds__(RS_T * RS_T) augment_resample_adjoint_kernel(c
   }
 }
 
+// ================================================================================================ image-space filter (item 17)
+// ADA's imgfilter: per image, 43 taps h_b = sum_i gains[b][i] bank[i] applied separably with the mirror R_N (21-pixel halo), then
+// the additive noise y += sigma_b n.  Both kernels walk 64 x 32 output tiles of one (b, c) plane with a tile-stride loop: the tile's
+// 74 x 106 input box goes to shared memory (mirrored forward, zero-padded in the adjoint), a vertical pass writes 32 x 106 partial
+// sums, a horizontal pass the 64 x 32 outputs.  Each thread of a pass keeps a window of its column (row) in registers and
+// accumulates 16 (8) outputs, so each shared-memory value it loads feeds 16 (8) FMAs.
+constexpr int FL_TAPS = 43, FL_R = 21;                               // taps, halo
+constexpr int FL_TW = 64, FL_TH = 32;                                // output tile
+constexpr int FL_IW = FL_TW + 2 * FL_R, FL_IH = FL_TH + 2 * FL_R;    // input box: 106 x 74
+constexpr int FL_PITCH = FL_IW + 1;                                  // odd pitch: a warp reading down 32 rows hits 32 banks
+constexpr int FL_RV = 16, FL_RH = 8;                                 // outputs per thread: vertical pass, horizontal pass
+constexpr int FL_THREADS = 256;
+static_assert(FL_TH % FL_RV == 0 && FL_TW % FL_RH == 0 && FL_TH * (FL_TW / FL_RH) == FL_THREADS, "filter tile shape");
+static_assert(FL_TH > FL_R && FL_TW > FL_R, "a tile holding a pixel within the halo of an edge must start at that edge");
+
+// The bank [4, 43] as integer numerators over 2^15 (SURVEY A.4 item 17): every entry and every sum of entries of the four rows is
+// exact in fp32.  Row i (i >= 1) is band i's high-pass.
+__constant__ short fl_bank[4][FL_TAPS] = {
+    {-1, 0, 9, 16, 18, 0, -66, -144, -207, -256, -297, -288, -212, 0, 468, 1056, 1674, 2304, 2918, 3456, 3888, 4096, 3888, 3456, 2918,
+     2304, 1674, 1056, 468, 0, -212, -288, -297, -256, -207, -144, -66, 0, 18, 16, 9, 0, -1},
+    {1, 0, -9, -16, -18, 0, 66, 144, 207, 256, 297, 288, 244, 0, -756, -1568, -2250, -2304, -806, 1152, 3024, 4096, 3024, 1152, -806,
+     -2304, -2250, -1568, -756, 0, 244, 288, 297, 256, 207, 144, 66, 0, -18, -16, -9, 0, 1},
+    {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, -32, 0, 288, 512, 576, 0, -3136, -4608, 2304, 8192, 2304, -4608, -3136, 0, 576, 512, 288, 0,
+     -32, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0},
+    {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 1024, 0, -9216, 16384, -9216, 0, 1024, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0,
+     0, 0, 0, 0, 0}};
+
+// Gains exactly (1, 1, 1, 1): the taps are exactly the unit impulse, and the kernels copy the plane (bit for bit, -0 and non-finite
+// neighbours included) instead of filtering it.
+__device__ __forceinline__ bool fl_identity(const float* __restrict__ gains, int b) {
+  return __ldg(gains + 4 * b) == 1.f && __ldg(gains + 4 * b + 1) == 1.f && __ldg(gains + 4 * b + 2) == 1.f && __ldg(gains + 4 * b + 3) == 1.f;
+}
+
+// The reflected preimages' contributions to the adjoint along one axis at source index m (N the axis length), read from a line
+// `s` of the tile's zero-padded buffer whose element 0 is index o - 21: e[-m] for 1 <= m <= 21, e[2(N-1) - m] for N-22 <= m <= N-2,
+// with e[k] = sum_t h[t] g[k - t + 21] (only the terms with g inside [0, N) are summed).  Returned separately, to be added in order.
+__device__ __forceinline__ float2 fl_reflected(const float* s, int stride, const float* h, int m, int N, int o) {
+  float lo = 0.f, hi = 0.f;
+  if (m >= 1 && m <= FL_R)
+    for (int t = 0; t <= FL_R - m; ++t) lo = fmaf(h[t], s[(FL_R - m - t - o + FL_R) * stride], lo);
+  if (m >= N - 1 - FL_R && m <= N - 2)
+    for (int t = N + FL_R - 1 - m; t < FL_TAPS; ++t) hi = fmaf(h[t], s[(2 * N + FL_R - 2 - m - t - o + FL_R) * stride], hi);
+  return make_float2(lo, hi);
+}
+
+// ADJ = false: y = V H x (+ sigma n).  ADJ = true: gx = H^T V^T gy, each source pixel summing its at most 3 preimages per axis
+// (itself, -m, 2(N-1) - m) in that order; with symmetric taps the transposed pass is the same correlation with h[42 - t].
+template <bool ADJ>
+__global__ void __launch_bounds__(FL_THREADS, 2) augment_filter_kernel(const float* __restrict__ x, float* __restrict__ y,
+                                                                    const float* __restrict__ gains, const float* __restrict__ sigma,
+                                                                    const float* __restrict__ noise, int C, int H, int W,
+                                                                    long long tiles, int tiles_x, int tiles_y) {
+  __shared__ float s_in[FL_IH * FL_PITCH];
+  __shared__ float s_v[FL_TH * FL_PITCH];
+  __shared__ float s_h[FL_TAPS + 1];
+  const size_t HW = (size_t)H * W;
+  const int tid = threadIdx.x;
+  for (long long tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
+    const long long plane = tile / ((long long)tiles_x * tiles_y);
+    const int rem = (int)(tile % ((long long)tiles_x * tiles_y));
+    const int b = (int)(plane / C);
+    const int x0 = (rem % tiles_x) * FL_TW, y0 = (rem / tiles_x) * FL_TH;
+    const float* src = x + (size_t)plane * HW;
+    float* dst = y + (size_t)plane * HW;
+    const float* nz = noise ? noise + (size_t)plane * HW : nullptr;
+    const float sig = (!ADJ && sigma) ? __ldg(sigma + b) : 0.f;
+    if (fl_identity(gains, b)) {
+      for (int i = tid; i < FL_TH * FL_TW; i += FL_THREADS) {
+        const int gy = y0 + i / FL_TW, gx = x0 + i % FL_TW;
+        if (gy >= H || gx >= W) continue;
+        const size_t o = (size_t)gy * W + gx;
+        float v = __ldg(src + o);
+        if (sig != 0.f) v = fmaf(sig, __ldg(nz + o), v);
+        dst[o] = v;
+      }
+      continue;
+    }
+    if (tid < FL_TAPS) {                                              // h_b[t], summed over the bands in a fixed order
+      const float* g = gains + 4 * b;
+      float h = __ldg(g) * ((float)fl_bank[0][tid] * (1.f / 32768.f));
+#pragma unroll
+      for (int i = 1; i < 4; ++i) h = fmaf(__ldg(g + i), (float)fl_bank[i][tid] * (1.f / 32768.f), h);
+      s_h[tid] = h;
+    }
+    for (int i = tid; i < FL_IH * FL_IW; i += FL_THREADS) {           // the input box: mirrored (forward) or zero-padded (adjoint)
+      const int r = i / FL_IW, c = i - r * FL_IW;
+      int gy = y0 - FL_R + r, gx = x0 - FL_R + c;
+      float v;
+      if (ADJ) {
+        v = (gy >= 0 && gy < H && gx >= 0 && gx < W) ? __ldg(src + (size_t)gy * W + gx) : 0.f;
+      } else {                                                        // beyond N + 20 only feeds outputs past the edge
+        gy = aug_mirror(min(gy, H - 1 + FL_R), H);
+        gx = aug_mirror(min(gx, W - 1 + FL_R), W);
+        v = __ldg(src + (size_t)gy * W + gx);
+      }
+      s_in[r * FL_PITCH + c] = v;
+    }
+    __syncthreads();
+    for (int it = tid; it < FL_IW * (FL_TH / FL_RV); it += FL_THREADS) {   // vertical pass: FL_RV rows of one column
+      const int c = it % FL_IW, r0 = (it / FL_IW) * FL_RV;
+      float w[FL_RV + FL_TAPS - 1], acc[FL_RV];
+#pragma unroll
+      for (int k = 0; k < FL_RV + FL_TAPS - 1; ++k) w[k] = s_in[(r0 + k) * FL_PITCH + c];
+#pragma unroll
+      for (int k = 0; k < FL_RV; ++k) acc[k] = 0.f;
+#pragma unroll
+      for (int t = 0; t < FL_TAPS; ++t) {
+        const float h = s_h[ADJ ? FL_TAPS - 1 - t : t];
+#pragma unroll
+        for (int k = 0; k < FL_RV; ++k) acc[k] = fmaf(h, w[k + t], acc[k]);
+      }
+#pragma unroll
+      for (int k = 0; k < FL_RV; ++k) s_v[(r0 + k) * FL_PITCH + c] = acc[k];
+      if (ADJ && (y0 <= FL_R || y0 + FL_TH >= H - 1 - FL_R)) {        // tiles that hold a row within the halo of an edge
+#pragma unroll 1
+        for (int k = 0; k < FL_RV; ++k) {                             // this thread's own sums: no barrier needed
+          const float2 e = fl_reflected(s_in + c, FL_PITCH, s_h, y0 + r0 + k, H, y0);
+          float v = s_v[(r0 + k) * FL_PITCH + c];
+          v += e.x;
+          v += e.y;
+          s_v[(r0 + k) * FL_PITCH + c] = v;
+        }
+      }
+    }
+    __syncthreads();
+    {                                                                 // horizontal pass: FL_RH columns of one row per thread
+      const int r = tid % FL_TH, c0 = (tid / FL_TH) * FL_RH;
+      const float* row = s_v + r * FL_PITCH;
+      float w[FL_RH + FL_TAPS - 1], acc[FL_RH];
+#pragma unroll
+      for (int k = 0; k < FL_RH + FL_TAPS - 1; ++k) w[k] = row[c0 + k];
+#pragma unroll
+      for (int k = 0; k < FL_RH; ++k) acc[k] = 0.f;
+#pragma unroll
+      for (int t = 0; t < FL_TAPS; ++t) {
+        const float h = s_h[ADJ ? FL_TAPS - 1 - t : t];
+#pragma unroll
+        for (int k = 0; k < FL_RH; ++k) acc[k] = fmaf(h, w[k + t], acc[k]);
+      }
+      const int gy = y0 + r;
+      if (gy < H) {
+#pragma unroll
+        for (int k = 0; k < FL_RH; ++k) {
+          const int gx = x0 + c0 + k;
+          if (gx >= W) continue;
+          float v = acc[k];
+          if (ADJ) {
+            const float2 e = fl_reflected(row, 1, s_h, gx, W, x0);
+            v += e.x;
+            v += e.y;
+          }
+          const size_t o = (size_t)gy * W + gx;
+          if (sig != 0.f) v = fmaf(sig, __ldg(nz + o), v);
+          dst[o] = v;
+        }
+      }
+    }
+    __syncthreads();
+  }
+}
+
+// No filter: y = x, plus sigma_b n where sigma_b != 0 (an image with sigma_b == 0 does not read n).
+__global__ void augment_noise_kernel(const float* __restrict__ x, float* __restrict__ y, const float* __restrict__ sigma,
+                                     const float* __restrict__ noise, size_t n, size_t per_image) {
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+    float v = __ldg(x + i);
+    if (sigma) {
+      const float s = __ldg(sigma + i / per_image);
+      if (s != 0.f) v = fmaf(s, __ldg(noise + i), v);
+    }
+    y[i] = v;
+  }
+}
+
 }  // namespace gf
 
 using namespace gf;
@@ -649,6 +823,48 @@ int gf_augment_resample_nchw(const float* x, float* y, const int* geom, const fl
 int gf_augment_resample_adjoint_nchw(const float* gy, float* gx, const int* geom, const float* frac, const float* color, int B, int C, int H,
                                      int W, void* stream) {
   return augment_resample_launch("gf_augment_resample_adjoint_nchw", true, gy, gx, geom, frac, color, B, C, H, W, stream);
+}
+
+// Both filter entry points: the checks, then one launch (the tiled filter, or the elementwise noise pass without gains).
+static int augment_filter_launch(const char* name, bool adjoint, const float* in, float* out, const float* gains, const float* sigma,
+                                 const float* noise, int B, int C, int H, int W, void* stream) {
+  if (!in || !out || (adjoint && !gains)) { set_error("%s: null pointer", name); return GF_ERR_INVALID; }
+  if ((sigma == nullptr) != (noise == nullptr)) {
+    set_error("%s: sigma and noise must both be given or both be NULL", name); return GF_ERR_INVALID;
+  }
+  if (B <= 0 || C <= 0 || H <= 0 || W <= 0) { set_error("%s: bad sizes B=%d C=%d H=%d W=%d", name, B, C, H, W); return GF_ERR_INVALID; }
+  if (gains && (H < FL_R + 1 || W < FL_R + 1)) {
+    set_error("%s: the 43-tap filter's mirror needs H and W of at least 22 (H=%d W=%d)", name, H, W); return GF_ERR_UNSUPPORTED;
+  }
+  if (H > 32768 || W > 32768 || (long long)C * H * W > 0x7fffffffLL) {
+    set_error("%s: image too large (C=%d H=%d W=%d): H, W <= 32768 and C*H*W < 2^31", name, C, H, W); return GF_ERR_UNSUPPORTED;
+  }
+  const size_t n = (size_t)B * C * H * W;
+  if (in < out + n && out < in + n) { set_error("%s: the output must not alias the input", name); return GF_ERR_INVALID; }
+  const cudaStream_t st = (cudaStream_t)stream;
+  if (!gains) {
+    const size_t blocks = (n + 255) / 256, cap = (size_t)num_sms() * 8;
+    augment_noise_kernel<<<(int)(blocks < cap ? blocks : cap), 256, 0, st>>>(in, out, sigma, noise, n, (size_t)C * H * W);
+  } else {
+    const int tx = (W + FL_TW - 1) / FL_TW, ty = (H + FL_TH - 1) / FL_TH;
+    const long long tiles = (long long)B * C * tx * ty, cap = (long long)num_sms() * 2;   // 2 CTAs per SM (registers)
+    const int grid = (int)(tiles < cap ? tiles : cap);
+    if (adjoint)
+      augment_filter_kernel<true><<<grid, FL_THREADS, 0, st>>>(in, out, gains, nullptr, nullptr, C, H, W, tiles, tx, ty);
+    else
+      augment_filter_kernel<false><<<grid, FL_THREADS, 0, st>>>(in, out, gains, sigma, noise, C, H, W, tiles, tx, ty);
+  }
+  GF_LAUNCH_OK();
+  return GF_OK;
+}
+
+int gf_augment_filter_nchw(const float* x, float* y, const float* gains, const float* sigma, const float* noise, int B, int C, int H, int W,
+                           void* stream) {
+  return augment_filter_launch("gf_augment_filter_nchw", false, x, y, gains, sigma, noise, B, C, H, W, stream);
+}
+
+int gf_augment_filter_adjoint_nchw(const float* gy, float* gx, const float* gains, int B, int C, int H, int W, void* stream) {
+  return augment_filter_launch("gf_augment_filter_adjoint_nchw", true, gy, gx, gains, nullptr, nullptr, B, C, H, W, stream);
 }
 
 }  // extern "C"

@@ -643,6 +643,153 @@ def augment(x: torch.Tensor, geom: torch.Tensor, color: Optional[torch.Tensor] =
     return augment_ref(x, geom, color)
 
 
+# ------------------------------------------------------------------------------------------------ ADA's image-space filter and noise
+# The lifting steps of ADA's filter bank: lo2 = conv(h, h[::-1]) / 2 and hi2 (h modulated by (-1)^n) of the sym2 wavelet are, in R,
+# the Deslauriers-Dubuc filters below (numerators over 32).  SURVEY A.4 item 17.
+IMGFILTER_LO2 = (-1, 0, 9, 16, 9, 0, -1)
+IMGFILTER_HI2 = (1, 0, -9, 16, -9, 0, 1)
+IMGFILTER_TAPS = 43
+IMGFILTER_HALO = IMGFILTER_TAPS // 2          # 21: one reflection covers it when H, W >= 22
+
+
+def imgfilter_bank_numerators() -> list:
+    """The bank [4, 43] as integer numerators over 2^15, by ADA's recipe in exact arithmetic: row 0 starts as e_0; for each band
+    i = 1..3 every row is upsampled by 2 (zeros between, the last dropped) and convolved with lo2, then hi2 is added at the centre of
+    row i.  After three rounds every entry has the denominator 32^3 = 2^15."""
+    rows = [[1], [0], [0], [0]]
+    for i in range(1, 4):
+        ups = [[v for a in r for v in (a, 0)][:-1] for r in rows]
+        rows = [[sum(u[j - k] * IMGFILTER_LO2[k] for k in range(7) if 0 <= j - k < len(u)) for j in range(len(u) + 6)] for u in ups]
+        s = (len(rows[i]) - 7) // 2
+        for k, v in enumerate(IMGFILTER_HI2):
+            rows[i][s + k] += v * 32 ** (i - 1)
+    return rows
+
+
+def imgfilter_bank(device=None, dtype=torch.float64) -> torch.Tensor:
+    """ADA's image-space filter bank [4, 43] (SURVEY A.4 item 17), exact in any float dtype: numerators over 2^15 of magnitude at most
+    2^14.  Row 0 is the low band, rows 1..3 the high-pass bands; the four rows sum to the unit impulse at tap 21."""
+    return (torch.tensor(imgfilter_bank_numerators(), dtype=torch.float64) / 2 ** 15).to(device=device, dtype=dtype)
+
+
+def _augment_filter_args(x: torch.Tensor, gains: Optional[torch.Tensor], sigma: Optional[torch.Tensor],
+                         noise: Optional[torch.Tensor]):
+    """Checks of ops.augment_filter (the refusals of gf_augment_filter_nchw); returns (gains [B, 4], sigma [B], noise [B, C, H, W]),
+    each None or contiguous on x's device, in float32 for CUDA fp32 x and in x's dtype otherwise."""
+    if x.dim() != 4:
+        raise ValueError(f"augment_filter: x must be [B, C, H, W], got {tuple(x.shape)}")
+    B, C, H, W = x.shape
+    dt = x.dtype
+    if (sigma is None) != (noise is None):
+        raise ValueError("augment_filter: sigma and noise must both be given or both be None")
+    if gains is not None:
+        if tuple(gains.shape) != (B, 4):
+            raise ValueError(f"augment_filter: gains must be [{B}, 4], got {tuple(gains.shape)}")
+        if H <= IMGFILTER_HALO or W <= IMGFILTER_HALO:
+            raise ValueError(f"augment_filter: the 43-tap filter needs H and W of at least 22, got {H}x{W}")
+        gains = gains.to(device=x.device, dtype=dt).contiguous()
+    if sigma is not None:
+        if sigma.dim() < 1 or sigma.shape[0] != B or sigma.numel() != B:
+            raise ValueError(f"augment_filter: sigma must be [{B}] or [{B}, 1, 1, 1], got {tuple(sigma.shape)}")
+        if tuple(noise.shape) != (B, C, H, W):
+            raise ValueError(f"augment_filter: noise must be [{B}, {C}, {H}, {W}], got {tuple(noise.shape)}")
+        sigma = sigma.reshape(B).to(device=x.device, dtype=dt).contiguous()
+        noise = noise.detach().to(device=x.device, dtype=dt).contiguous()
+    return gains, sigma, noise
+
+
+def augment_filter_ref(x: torch.Tensor, gains: Optional[torch.Tensor] = None, sigma: Optional[torch.Tensor] = None,
+                       noise: Optional[torch.Tensor] = None, bank: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """Definition of ops.augment_filter, any dtype and device, differentiable to any order by torch autograd: per image the taps
+    h_b = gains[b] @ bank (elementwise products and a sum, no TF32 matmul), a ``reflect`` pad of 21 and a grouped conv2d along each
+    axis (every image whose gains are exactly (1, 1, 1, 1) is copied instead); then y_b + sigma_b noise_b where sigma_b != 0.
+    ``bank`` replaces the bank (the tests' magnitude companion runs |bank|)."""
+    gains, sigma, noise = _augment_filter_args(x, gains, sigma, noise)
+    B, C, H, W = x.shape
+    y = x
+    if gains is not None:
+        bk = imgfilter_bank(x.device, x.dtype) if bank is None else bank.to(device=x.device, dtype=x.dtype)
+        h = (gains[:, :, None] * bk[None]).sum(dim=1).repeat_interleave(C, dim=0)         # [B * C, 43]
+        p = IMGFILTER_HALO
+        z = F.pad(x.reshape(1, B * C, H, W), [p, p, p, p], mode="reflect")
+        z = F.conv2d(z, h[:, None, None, :], groups=B * C)
+        z = F.conv2d(z, h[:, None, :, None], groups=B * C).reshape(B, C, H, W)
+        ident = (gains == 1).all(dim=1)[:, None, None, None]
+        y = torch.where(ident, x, z)
+    if sigma is not None:
+        s = sigma[:, None, None, None]
+        y = torch.where(s != 0, y + s * noise, y)
+    return y
+
+
+def augment_filter_adjoint_ref(gy: torch.Tensor, gains: torch.Tensor, bank: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """Definition of the adjoint of the filter, gx = H_b^T V_b^T gy (the noise does not take part): torch autograd's vector-Jacobian
+    product of augment_filter_ref."""
+    with torch.enable_grad():
+        x0 = gy.new_zeros(gy.shape).requires_grad_(True)
+        (gx,) = torch.autograd.grad(augment_filter_ref(x0, gains, bank=bank), x0, gy, create_graph=gy.requires_grad)
+    return gx
+
+
+def _augment_filter_native(name: str, x: torch.Tensor, gains: Optional[torch.Tensor], sigma: Optional[torch.Tensor] = None,
+                           noise: Optional[torch.Tensor] = None) -> torch.Tensor:
+    xc = x.detach().contiguous()
+    B, C, H, W = xc.shape
+    y = torch.empty_like(xc)
+    ptr = lambda t: None if t is None else t.data_ptr()
+    with torch.cuda.device(x.device):
+        lib = _lib.load()
+        if name == "gf_augment_filter_nchw":
+            rc = lib.gf_augment_filter_nchw(xc.data_ptr(), y.data_ptr(), ptr(gains), ptr(sigma), ptr(noise), B, C, H, W, _stream(x.device))
+        else:
+            rc = getattr(lib, name)(xc.data_ptr(), y.data_ptr(), ptr(gains), B, C, H, W, _stream(x.device))
+        _lib.check(rc, name)
+    return y
+
+
+class _AugmentFilter(torch.autograd.Function):
+    """gf_augment_filter_nchw, differentiable to any order: the filter is linear and the noise an offset, so the gradient is the
+    adjoint (_AugmentFilterAdjoint), whose gradient is the filter again without the noise."""
+
+    @staticmethod
+    def forward(ctx, x, gains, sigma, noise):
+        ctx.save_for_backward(gains)
+        return _augment_filter_native("gf_augment_filter_nchw", x, gains, sigma, noise)
+
+    @staticmethod
+    def backward(ctx, gy):
+        (gains,) = ctx.saved_tensors
+        return (gy if gains is None else _AugmentFilterAdjoint.apply(gy, gains)), None, None, None
+
+
+class _AugmentFilterAdjoint(torch.autograd.Function):
+    """gf_augment_filter_adjoint_nchw: gx = H_b^T V_b^T gy."""
+
+    @staticmethod
+    def forward(ctx, gy, gains):
+        ctx.save_for_backward(gains)
+        return _augment_filter_native("gf_augment_filter_adjoint_nchw", gy, gains)
+
+    @staticmethod
+    def backward(ctx, ggx):
+        (gains,) = ctx.saved_tensors
+        return _AugmentFilter.apply(ggx, gains, None, None), None
+
+
+def augment_filter(x: torch.Tensor, gains: Optional[torch.Tensor] = None, sigma: Optional[torch.Tensor] = None,
+                   noise: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """ADA's image-space filtering and additive noise (SURVEY A.4 item 17), applied after ops.augment: x [B, C, H, W] -> the same
+    shape.  gains [B, 4] (or None: no filter) weight the four bands of imgfilter_bank; sigma [B] with noise [B, C, H, W] (both or
+    neither) add sigma_b noise_b.  See include/gf_ops.h for the exact map.  CUDA fp32 tensors run gf_augment_filter_nchw and its
+    adjoint in the backward (to any order); anything else runs the definition augment_filter_ref."""
+    gains, sigma, noise = _augment_filter_args(x, gains, sigma, noise)
+    if gains is None and sigma is None:
+        return x
+    if x.is_cuda and x.dtype == torch.float32:
+        return _AugmentFilter.apply(x, gains, sigma, noise)
+    return augment_filter_ref(x, gains, sigma, noise)
+
+
 def conv3x3_pack(weight: torch.Tensor, scale: float = 1.0) -> torch.Tensor:
     """weight [O, I, 3, 3] -> the tap-major, TF32-rounded [9, O, I] layout gf_conv3x3_nhwc_tf32 consumes (gf_conv3x3_pack_weights)."""
     O, I = weight.shape[:2]

@@ -41,7 +41,9 @@ parameters of its own (``sample_augment``): integer blits (x flips, 90-degree ro
 and a colour matrix, on the gf_augment_nchw kernel and its adjoint.  The strength p is a device tensor (``Trainer.augment_p``); with
 ``ada_target`` it adapts to the sign of the real logits, summed over ranks, every ``ada_interval`` steps, without a host sync.  Not
 in the path-length phase, the w_avg update or inference.  Off by default: with "" the step makes the same calls and draws the same
-random numbers as without the option.
+random numbers as without the option.  "bgc" adds ADA's fractional geometry (``sample_augment_frac``, SURVEY A.4 item 16); "bgcf" and
+"bgcfn" add, after it, ADA's image-space filtering and additive noise (``sample_augment_filter``, ``ops.augment_filter``, SURVEY A.4
+item 17).
 """
 from __future__ import annotations
 
@@ -59,7 +61,7 @@ from .attention import BipartiteAttention
 from .autograd import _e, composite_forward
 from .networks import FullyConnected, nf
 from ._state import bump_weights_epoch
-from .ops import augment, fir4, fir_filter, upfirdn2d_ref
+from .ops import IMGFILTER_HALO, augment, augment_filter, fir4, fir_filter, upfirdn2d_ref
 
 SQRT2 = math.sqrt(2.0)
 
@@ -228,7 +230,7 @@ class TrainConfig:
     pl_decay: float = 0.01              # decay of the running mean of the path lengths
     style_mixing: float = 0.0           # probability of style mixing per generator forward (StyleGAN2 / GANsformer: 0.9); 0 = off
     augment: str = ""                   # discriminator augmentation: "" = off, "bc" = all of AUGMENT_OPS, "bgc" = those and GEOM_OPS,
-                                        # or a comma list of names from both
+                                        # "bgcf" / "bgcfn" = those and "imgfilter" / both FILTER_OPS, or a comma list of names
     augment_p: float = 0.0              # starting augmentation strength p
     ada_target: Optional[float] = None  # adaptive p: target of the mean sign of the real logits (ADA: 0.6); None = p stays put
     ada_interval: int = 4               # steps between updates of p
@@ -238,22 +240,25 @@ class TrainConfig:
 AUGMENT_OPS = ("xflip", "rotate90", "xint", "brightness", "contrast", "lumaflip", "hue", "saturation")
 GEOM_OPS = ("scale", "rotate", "aniso", "xfrac")                     # ADA's general geometry (SURVEY A.4 item 16)
 _ADA_ORDER = AUGMENT_OPS[:3] + GEOM_OPS + AUGMENT_OPS[3:]
+FILTER_OPS = ("imgfilter", "noise")                                  # ADA's image-space filtering and noise (SURVEY A.4 item 17)
+_ALL_OPS = _ADA_ORDER + FILTER_OPS
+_PRESETS = {"bc": AUGMENT_OPS, "bgc": _ADA_ORDER, "bgcf": _ADA_ORDER + FILTER_OPS[:1], "bgcfn": _ALL_OPS}
+IMGFILTER_EXPECTED_POWER = (10.0, 1.0, 1.0, 1.0)                     # ADA's 1/f power spectrum of the four bands, over 13
+NOISE_STD = 0.1
 
 
 def parse_augment(spec: str) -> tuple:
     """TrainConfig.augment -> the enabled transforms, in ADA's order: "" none, "bc" the eight of AUGMENT_OPS, "bgc" those and
-    GEOM_OPS, else a comma list of names from both."""
+    GEOM_OPS, "bgcf" those and "imgfilter", "bgcfn" those and "noise", else a comma list of names from all of them."""
     if not spec:
         return ()
-    if spec == "bc":
-        return AUGMENT_OPS
-    if spec == "bgc":
-        return _ADA_ORDER
+    if spec in _PRESETS:
+        return _PRESETS[spec]
     names = {s.strip() for s in spec.split(",")}
-    unknown = sorted(names - set(_ADA_ORDER))
+    unknown = sorted(names - set(_ALL_OPS))
     if unknown:
-        raise ValueError(f"unknown augmentation(s) {unknown}: use 'bc', 'bgc' or a comma list of {_ADA_ORDER}")
-    return tuple(n for n in _ADA_ORDER if n in names)
+        raise ValueError(f"unknown augmentation(s) {unknown}: use one of {tuple(_PRESETS)} or a comma list of {_ALL_OPS}")
+    return tuple(n for n in _ALL_OPS if n in names)
 
 
 def sample_augment_frac(ops_: tuple, p, B: int, H: int, W: int, device):
@@ -381,6 +386,35 @@ def sample_augment(ops_: tuple, p, B: int, H: int, W: int, device):
     return geom, M[:, :3, :].reshape(B, 12).contiguous()
 
 
+def sample_augment_filter(ops_: tuple, p, B: int, C: int, H: int, W: int, device):
+    """Per-image parameters for ops.augment_filter: (gains [B, 4] or None, sigma [B] or None, noise [B, C, H, W] or None), None where
+    the transform is not enabled (then no random number is drawn for it).  Drawn on ``device`` without a host sync (capturable), in
+    ADA's order and the same random numbers whatever p is.
+
+    imgfilter: g = (1, 1, 1, 1); for each band i, t_i = exp2(N(0, 1)) (randn(B)), applying with probability p (rand(B)); where it
+    applies, t = (1, .., t_i, .., 1) and g <- g * t / sqrt(sum_j ep_j t_j^2), ep = (10, 1, 1, 1) / 13; where it does not, g is left
+    exactly unchanged, so p = 0 gives exactly (1, 1, 1, 1).  noise: sigma = |N(0, 1)| * 0.1 (randn(B)), applying with probability p
+    (rand(B)), else 0; then the field n = randn(B, C, H, W)."""
+    gains = sigma = noise = None
+    if "imgfilter" in ops_:
+        ep = torch.cat([torch.full((1,), IMGFILTER_EXPECTED_POWER[0] / 13, device=device),      # fills, no host copy: capturable
+                        torch.full((3,), IMGFILTER_EXPECTED_POWER[1] / 13, device=device)])
+        gains = torch.ones(B, 4, device=device)
+        for i in range(4):
+            t_i = torch.exp2(torch.randn(B, device=device))
+            a = torch.rand(B, device=device) < p
+            t = torch.ones(B, 4, device=device)
+            t[:, i] = t_i
+            t = t / (ep * t.square()).sum(dim=1, keepdim=True).sqrt()
+            gains = torch.where(a[:, None], gains * t, gains)
+    if "noise" in ops_:
+        s = torch.randn(B, device=device).abs() * NOISE_STD
+        a = torch.rand(B, device=device) < p
+        sigma = torch.where(a, s, torch.zeros_like(s))
+        noise = torch.randn(B, C, H, W, device=device)
+    return gains, sigma, noise
+
+
 def mixing_cutoff(p: float, num_ws: int, device) -> torch.Tensor:
     """The style-mixing cutoff of one minibatch as a 0-d int64 tensor on ``device``, drawn without a host sync: with probability
     ``p`` uniform in [1, num_ws - 1], else num_ws (no mixing).  ``p == 0`` draws no random number and returns num_ws."""
@@ -453,17 +487,24 @@ class Trainer:
                 raise ValueError(f"ada_target is a mean sign and must be in [-1, 1], got {cfg.ada_target}")
             if cfg.ada_interval < 1 or not cfg.ada_kimg > 0:
                 raise ValueError(f"need ada_interval >= 1 and ada_kimg > 0, got {cfg.ada_interval} and {cfg.ada_kimg}")
+        res = getattr(self.D, "resolution", None)
+        if "imgfilter" in self.augment_ops and res is not None and res <= IMGFILTER_HALO:
+            raise ValueError(f"the imgfilter augmentation needs images of at least 22x22 (its 43-tap filter reflects a 21-pixel "
+                             f"border once), got a {res}x{res} discriminator")
 
     def _augment(self, img: torch.Tensor) -> torch.Tensor:
         """One image batch on its way into D, augmented with parameters of its own (no call and no random number when off)."""
         if not self.augment_ops:
             return img
-        B, _, H, W = img.shape
-        geom, color = sample_augment(self.augment_ops, self.augment_p, B, H, W, img.device)
-        frac = sample_augment_frac(self.augment_ops, self.augment_p, B, H, W, img.device)
-        if frac is None:
-            return augment(img, geom, color)
-        return augment(img, geom, color, frac)
+        B, C, H, W = img.shape
+        if any(n in self.augment_ops for n in _ADA_ORDER):
+            geom, color = sample_augment(self.augment_ops, self.augment_p, B, H, W, img.device)
+            frac = sample_augment_frac(self.augment_ops, self.augment_p, B, H, W, img.device)
+            img = augment(img, geom, color) if frac is None else augment(img, geom, color, frac)
+        if any(n in self.augment_ops for n in FILTER_OPS):
+            gains, sigma, noise = sample_augment_filter(self.augment_ops, self.augment_p, B, C, H, W, img.device)
+            img = augment_filter(img, gains, sigma, noise)
+        return img
 
     def _ada_accumulate(self, logit_real: torch.Tensor):
         """Adds (sum of the signs, count) of this step's real logits, summed over ranks, to the ADA accumulators."""

@@ -161,6 +161,23 @@ int gf_augment_resample_nchw(const float* x, float* y, const int* geom, const fl
 int gf_augment_resample_adjoint_nchw(const float* gy, float* gx, const int* geom, const float* frac, const float* color, int B, int C,
                                      int H, int W, void* stream);
 
+/* ADA's image-space filtering and additive noise (SURVEY A.4 item 17), after the geometry and colour above.  x, y [B, C, H, W]:
+ *   gains  float [B, 4] or NULL (no filter): per image the taps h_b = sum_i gains[b][i] bank[i] of the fixed [4, 43] bank (exact
+ *          dyadic entries, numerators over 2^15), and y_b = V_b H_b x_b for every channel, (H x)[j] = sum_t h_b[t] x[R_N(j + t - 21)]
+ *          along each axis, R_N the mirror of gf_augment_nchw.  An image whose gains are exactly (1, 1, 1, 1) is copied.
+ *   sigma  float [B] and noise float [B, C, H, W], both given or both NULL: y_b += sigma_b noise_b; an image with sigma_b == 0 does
+ *          not read noise.
+ * One launch on `stream`, no workspace, no host sync, no atomics.  Errors, before touching the device: GF_ERR_INVALID for a NULL x / y,
+ * only one of sigma and noise, a size <= 0, or y overlapping x; GF_ERR_UNSUPPORTED for H or W < 22 with gains given (one reflection
+ * must cover the 21-pixel halo), and H or W > 32768 or C*H*W >= 2^31. */
+int gf_augment_filter_nchw(const float* x, float* y, const float* gains, const float* sigma, const float* noise, int B, int C, int H, int W,
+                           void* stream);
+
+/* The adjoint of the filter: gx = H_b^T V_b^T gy (the noise does not take part).  Gather only: each source pixel sums its at most
+ * 3 preimages per axis under R_N (itself, -m, 2(N-1) - m) in that order, so the result is the same bits on every run and under
+ * CUDA-graph replay.  gains is required; otherwise the arguments and errors of gf_augment_filter_nchw. */
+int gf_augment_filter_adjoint_nchw(const float* gy, float* gx, const float* gains, int B, int C, int H, int W, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
