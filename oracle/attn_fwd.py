@@ -41,10 +41,11 @@ def _combine(Xn, GB, integration, C):
 
 
 def stage_t_forward(X, Kp, Vt, Rt, Ct, *, H, W, k, integration, norm, heads=1, mult=None, cb=None,
-                    post: Optional[dict] = None) -> Dict[str, Optional[Tensor]]:
+                    post: Optional[dict] = None, nscale=None, nshift=None) -> Dict[str, Optional[Tensor]]:
     """What gf_attn_simplex_fwd_ex writes for tables in natural-log units, in fp64: Xout [B,n,C], att [B,n,k] and rgb [B,3,n]
     (None without a tRGB).  Kp is the table as stage I writes it (in_scale folded in).  post: in_scale [B,C], bias [C],
-    noise [n] or [B,n], strength, act (0 / 1), gain, post_scale [B,C], rgb_w [B,3,C], rgb_bias [3]; any may be missing."""
+    noise [n] or [B,n], strength, act (0 / 1), gain, post_scale [B,C], rgb_w [B,3,C], rgb_bias [3]; any may be missing.
+    nscale / nshift [B,C]: the instance / batch statistics as NSCALE / NSHIFT hold them (x_n = x nscale + nshift)."""
     post = post or {}
     X, Kp, Vt, Rt, Ct = (t.double() for t in (X, Kp, Vt, Rt, Ct))
     B, n, C = X.shape
@@ -54,8 +55,9 @@ def stage_t_forward(X, Kp, Vt, Rt, Ct, *, H, W, k, integration, norm, heads=1, m
     Xin = X * d
     cbd = None if cb is None else cb.double()
     if heads == 1:
+        affine = None if nscale is None else (nscale.double(), nshift.double())
         out, att = of.per_token(Xin, Kp / d, Vt, Rt, Ct, H=H, W=W, integration=integration, norm=norm, return_att=True, k=k,
-                                att_mult=mult, cb=cbd)
+                                att_mult=mult, cb=cbd, affine=affine)
     else:
         assert mult is None and norm in (None, "none")
         seg = KP // heads

@@ -26,20 +26,32 @@ Tensor = torch.Tensor
 
 
 def _e(w: Tensor) -> Tensor:
-    """equalised-LR effective weight"""
-    return w * (1.0 / math.sqrt(w.shape[0]))
+    """equalised-LR effective weight (an empty weight, pos_dim = 0, stays empty)"""
+    return w * (1.0 / math.sqrt(w.shape[0])) if w.shape[0] else w
 
 
 def pad_k(k: int) -> int:
     return 16 if k <= 16 else 32
 
 
+def head_segment(k: int, num_heads: int) -> int:
+    """Table columns per head: one head uses all KP columns; 2 or 4 heads use segments of 8 or 16 (KP = heads * seg)."""
+    return pad_k(k) if num_heads == 1 else (8 if k <= 8 else 16)
+
+
 def fold_weights(w: Dict[str, Tensor], *, C: int, k: int, integration: str, duplex: bool,
                  use_pos: bool = True, num_heads: int = 1) -> Dict[str, Tensor]:
-    """Stage W.  Column layout of the key-side matrices: [K' (C) | kappa_p (p) | kappa_0 (1) | pad (3)]."""
-    assert num_heads == 1
+    """Stage W.  Column layout of the key-side matrices: [K' (C) | kappa_p (p) | kappa_0 (1) | pad (3)].
+
+    num_heads > 1 (simplex only): AK [h, D, C+p+4], CK [h, k, C+p+4], AV [h, D, Cout] and CV [h, Cout] hold one fold per head,
+    from that head's C/h channels of the key and value, with the logit scale 1/sqrt(C/h); bo and the +1 ride on head 0 only
+    (every head's probabilities sum to one).  Duplex layers also get the keys straight from Xbar (AK2 = WV2 AK, CK2 = bv2 AK + CK)
+    and, when w holds wcq, the query fold of the centroids ACQ (k-means iterations >= 2 and carried-in centroids).  CB is the
+    constant part of the control signal (bo, +1 on the gain half)."""
     p = w["pos_latent"].shape[1]
-    s = 1.0 / math.sqrt(C)
+    h = num_heads
+    assert h == 1 or not duplex
+    s = 1.0 / math.sqrt(C // h)
     dt = w["wq"].dtype
     wq, wpq = _e(w["wq"]), _e(w["wpq"])
     # query-side fold target: Q-space vector t  ->  [t Wq^T s | t Wpq^T s | t.bq s | 0 0 0]
@@ -67,16 +79,32 @@ def fold_weights(w: Dict[str, Tensor], *, C: int, k: int, integration: str, dupl
             qconst = qconst + w["pos_latent"] @ _e(w["wpq2"])
         out["AM"] = _e(w["wq2"]) @ m_fold                               # [D, C+p+4]
         out["CM"] = qconst @ m_fold                                     # [k, C+p+4]
-    else:
+        out["AK2"] = out["WV2"] @ akcen                                 # keys from Xbar: (Xbar WV2 + bv2) AK + CK
+        out["CK2"] = (w["bv2"] @ akcen)[None, :] + out["CK"]
+        if "wcq" in w:
+            out["ACQ"] = _e(w["wcq"]) @ m_fold                          # queries from the centroids: Cen ACQ + CM
+    elif h == 1:
         out["AK"] = _e(w["wk"]) @ qfold                                 # [D, C+p+4]
         out["CK"] = kconst @ qfold
+    else:
+        hs = [slice(i * (C // h), (i + 1) * (C // h)) for i in range(h)]
+        out["AK"] = torch.stack([_e(w["wk"])[:, sl] @ qfold[sl] for sl in hs])
+        out["CK"] = torch.stack([kconst[:, sl] @ qfold[sl] for sl in hs])
     wo = _e(w["wo"])
-    out["AV"] = _e(w["wv"]) @ wo                                        # [D, Cout]
-    cv = w["bv"] @ wo + w["bo"]
+    cb = w["bo"].clone()
     if integration in ("mul", "both"):
-        cv = cv.clone()
-        cv[:C] += 1.0                                                   # the "1 +" of x*(1+gain)
-    out["CV"] = cv                                                      # [Cout]
+        cb[:C] += 1.0                                                   # the "1 +" of x*(1+gain)
+    out["CB"] = cb
+    if h == 1:
+        out["AV"] = _e(w["wv"]) @ wo                                    # [D, Cout]
+        cv = w["bv"] @ wo + w["bo"]
+        if integration in ("mul", "both"):
+            cv = cv.clone()
+            cv[:C] += 1.0
+        out["CV"] = cv                                                  # [Cout]
+    else:
+        out["AV"] = torch.stack([_e(w["wv"])[:, sl] @ wo[sl] for sl in hs])
+        out["CV"] = torch.stack([w["bv"][sl] @ wo[sl] + (cb if i == 0 else 0.0) for i, sl in enumerate(hs)])
     return out
 
 
@@ -100,9 +128,24 @@ def _pos_tables(kp_all: Tensor, C: int, p: int, H: int, W: int, KP: int, use_pos
 
 
 def prologue(y: Tensor, f: Dict[str, Tensor], *, C: int, H: int, W: int, p: int, use_pos: bool = True,
-             key_source: Optional[Tensor] = None):
-    """Stage I.  key_source = centroids [B,k,C] for duplex pass B, else the latents y."""
+             key_source: Optional[Tensor] = None, num_heads: int = 1):
+    """Stage I.  key_source = centroids [B,k,C] for duplex pass B, else the latents y.  num_heads > 1: head h's latent j is
+    table column h * seg + j (head_segment), the other columns of its segment are padding."""
     B, k, _ = y.shape
+    if num_heads > 1:
+        seg = head_segment(k, num_heads)
+        KP = num_heads * seg
+        Kp = torch.zeros(B, KP, C, dtype=y.dtype)
+        Rt = torch.full((B, H, KP), -math.inf, dtype=y.dtype)
+        Ct = torch.zeros(B, W, KP, dtype=y.dtype)
+        Vt = torch.zeros(B, f["AV"].shape[2], KP, dtype=y.dtype)
+        for i in range(num_heads):
+            kp_all = y @ f["AK"][i] + f["CK"][i][None]
+            cols = slice(i * seg, i * seg + k)
+            Kp[:, cols] = kp_all[:, :, :C]
+            Rt[:, :, i * seg:(i + 1) * seg], Ct[:, :, i * seg:(i + 1) * seg] = _pos_tables(kp_all, C, p, H, W, seg, use_pos)
+            Vt[:, :, cols] = (y @ f["AV"][i] + f["CV"][i][None, None]).transpose(1, 2)
+        return Kp, Vt, Rt, Ct
     KP = pad_k(k)
     z = y if key_source is None else key_source
     kp_all = z @ f["AK"] + f["CK"][None]                                # [B,k,C+p+4]
@@ -117,13 +160,15 @@ def prologue(y: Tensor, f: Dict[str, Tensor], *, C: int, H: int, W: int, p: int,
 
 def per_token(X: Tensor, Kp: Tensor, Vt: Tensor, Rt: Tensor, Ct: Tensor, *, H: int, W: int,
               integration: str, norm: Optional[str], return_att: bool = False, k: Optional[int] = None,
-              att_mult: Optional[Tensor] = None, cb: Optional[Tensor] = None, retain: Optional[dict] = None):
+              att_mult: Optional[Tensor] = None, cb: Optional[Tensor] = None, retain: Optional[dict] = None,
+              affine: Optional[tuple] = None):
     """Stage T.  X [B,n,C] channels-last tokens.
 
     att_mult [B,n,KP] (or [B,n,k]) and cb [Cout] (attention dropout, the form the kernels use): q = p * mult weights the
     values, and the constants cb (bo, +1 on the gain half) that dropout leaves unscaled are re-added,
     ctl = sum_j q_j (Vt_j - cb) + cb.  retain (a dict) receives the logits "S", the probabilities "P", the dropped
-    probabilities "Q" and the control signal "ctl", so that a caller can take gradients with respect to them."""
+    probabilities "Q" and the control signal "ctl", so that a caller can take gradients with respect to them.  affine
+    (scale [B,C], shift [B,C]) replaces the instance / batch statistics of X by given ones: Xn = X scale + shift."""
     B, n, C = X.shape
     S = X @ Kp.transpose(1, 2)                                          # [B,n,KP]
     S = S + (Rt[:, :, None, :] + Ct[:, None, :, :]).reshape(B, n, -1)
@@ -139,7 +184,9 @@ def per_token(X: Tensor, Kp: Tensor, Vt: Tensor, Rt: Tensor, Ct: Tensor, *, H: i
         GB = Q @ (Vt - cb[None, :, None]).transpose(1, 2) + cb
     if retain is not None:
         retain.update(S=S, P=P, Q=Q, ctl=GB)
-    if norm == "layer":
+    if affine is not None:
+        Xn = X * affine[0][:, None, :] + affine[1][:, None, :]
+    elif norm == "layer":
         mu = X.mean(dim=2, keepdim=True)
         var = ((X - mu) ** 2).mean(dim=2, keepdim=True)
         Xn = (X - mu) / torch.sqrt(var + LN_EPS)
