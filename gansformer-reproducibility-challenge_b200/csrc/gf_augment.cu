@@ -556,14 +556,22 @@ __global__ void __launch_bounds__(RS_T * RS_T) augment_resample_adjoint_kernel(c
             for (int i = tid; i < noy * nqx; i += RS_T * RS_T) {      // transposed down-filter along x
               const int iy = i / nqx, jx = i - iy * nqx, q = cx0 + jx;
               float acc = 0.f;
-              for (int o = max(cdiv2(q - 12), ox0); o <= min(fdiv2(q - 1), ox1); ++o) acc = fmaf(rs_f[q - 1 - 2 * o], sA[iy * nox + o - ox0], acc);
+#pragma unroll
+              for (int t = 0; t < 6; ++t) {                               // o = cdiv2(q - 12) + t: taps 11 - 2t or 10 - 2t
+                const int o = cdiv2(q - 12) + t;
+                if (o >= ox0 && o <= ox1) acc = fmaf(rs_f[q - 1 - 2 * o], sA[iy * nox + o - ox0], acc);
+              }
               sB[i] = acc;
             }
             __syncthreads();
             for (int i = tid; i < nqy * nqx; i += RS_T * RS_T) {      // ... along y: gV
               const int jy = i / nqx, jx = i - jy * nqx, q = cy0 + jy;
               float acc = 0.f;
-              for (int o = max(cdiv2(q - 12), oy0); o <= min(fdiv2(q - 1), oy1); ++o) acc = fmaf(rs_f[q - 1 - 2 * o], sB[(o - oy0) * nqx + jx], acc);
+#pragma unroll
+              for (int t = 0; t < 6; ++t) {
+                const int o = cdiv2(q - 12) + t;
+                if (o >= oy0 && o <= oy1) acc = fmaf(rs_f[q - 1 - 2 * o], sB[(o - oy0) * nqx + jx], acc);
+              }
               sA[i] = acc;
             }
             __syncthreads();
