@@ -44,10 +44,7 @@ def composite_forward(x, y, p, *, integration, norm, duplex, use_pos, centroids=
     X = x.reshape(B, n, C)
     s = 1.0 / math.sqrt(C)
     if use_pos:
-        pd = p["pos_latent"].shape[1]
-        half = pd // 2
-        row, col = _axis(H, half, x.device).to(x.dtype), _axis(W, half, x.device).to(x.dtype)
-        Pg = torch.cat([row[:, None, :].expand(H, W, half), col[None, :, :].expand(H, W, half)], dim=2).reshape(n, pd)
+        Pg = grid_pos_table(H, W, p["pos_latent"].shape[1], x.device, x.dtype)
         Pl = p["pos_latent"]
     cen = None
     if duplex:
@@ -87,6 +84,19 @@ def composite_forward(x, y, p, *, integration, norm, duplex, use_pos, centroids=
         sp = lambda t, L: t.reshape(B, L, h, C // h).permute(0, 2, 1, 3)
         Ph = torch.softmax((sp(Q, n) @ sp(K, kk).transpose(2, 3)) * (1.0 / math.sqrt(C / h)), dim=3)
         ctl = (Ph @ sp(V, kk)).permute(0, 2, 1, 3).reshape(B, n, C) @ _e(p["wo"]) + p["bo"]
+    return integrate(X, ctl, integration, norm).reshape(B, H, W, C), cen
+
+
+def grid_pos_table(H, W, pd, device, dtype):
+    """The grid's sinusoidal table Pg [H*W, pd]: the row embedding of h, then the column embedding of w (pd / 2 each)."""
+    half = pd // 2
+    row, col = _axis(H, half, device).to(dtype), _axis(W, half, device).to(dtype)
+    return torch.cat([row[:, None, :].expand(H, W, half), col[None, :, :].expand(H, W, half)], dim=2).reshape(H * W, pd)
+
+
+def integrate(X, ctl, integration, norm):
+    """X [B,n,C] normalised (att_norm, eps 1e-8) and modulated by the control signal ctl [B,n,C or 2C] (after its dense)."""
+    C = X.shape[-1]
     if norm == "layer":
         mu = X.mean(dim=2, keepdim=True)
         Xn = (X - mu) * torch.rsqrt(((X - mu) ** 2).mean(dim=2, keepdim=True) + 1e-8)
@@ -97,12 +107,10 @@ def composite_forward(x, y, p, *, integration, norm, duplex, use_pos, centroids=
         mu = X.mean(dim=dims, keepdim=True)
         Xn = (X - mu) * torch.rsqrt(((X - mu) ** 2).mean(dim=dims, keepdim=True) + 1e-8)
     if integration == "mul":
-        out = Xn * (1.0 + ctl)
-    elif integration == "add":
-        out = Xn + ctl
-    else:
-        out = Xn * (1.0 + ctl[..., :C]) + ctl[..., C:]
-    return out.reshape(B, H, W, C), cen
+        return Xn * (1.0 + ctl)
+    if integration == "add":
+        return Xn + ctl
+    return Xn * (1.0 + ctl[..., :C]) + ctl[..., C:]
 
 
 def centroid_tables(y, p, H, W, C, use_pos):

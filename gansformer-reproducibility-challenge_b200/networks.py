@@ -22,6 +22,7 @@ from torch import nn
 
 from .attention import BipartiteAttention, _Plan, prologue_batch, tc_eligible
 from . import ops
+from .self_attention import ImageSelfAttention
 from ._state import weights_epoch, bump_weights_epoch
 from .ops import fir_filter
 
@@ -352,9 +353,12 @@ class SynthesisNetwork(nn.Module):
     """G_synthesis, skip architecture.  Attention on both conv layers of every resolution in [start_res, end_res]."""
 
     def __init__(self, resolution: int, latent_dim: int, components_num: int, fmap_base: int = 16384, fmap_max: int = 512,
-                 g_start_res: int = 8, g_end_res: Optional[int] = None, transformer: bool = True, attn_kwargs: Optional[dict] = None):
+                 g_start_res: int = 8, g_end_res: Optional[int] = None, transformer: bool = True, attn_kwargs: Optional[dict] = None,
+                 img2img: int = 0):
         super().__init__()
         assert resolution >= 4 and resolution & (resolution - 1) == 0
+        if img2img and not (8 <= img2img <= resolution and img2img & (img2img - 1) == 0):
+            raise ValueError(f"img2img must be 0 (off) or a block resolution in 8 .. {resolution}, got {img2img}")
         self.resolution, self.components_num = resolution, components_num
         g_end_res = resolution if g_end_res is None else g_end_res
         self.block_resolutions = [2 ** i for i in range(2, int(math.log2(resolution)) + 1)]
@@ -378,6 +382,14 @@ class SynthesisNetwork(nn.Module):
             self.layer_res.append(res)
             self.torgbs.append(ToRGB(out_ch, latent_dim))
         self.register_buffer("fir", fir_filter())
+        # img2img (SURVEY A.4 item 18): image self-attention on the output of block `img2img`, before its tRGB
+        self.img2img_res = int(img2img)
+        self.img2img = None
+        if img2img:
+            a = attn_kwargs
+            self.img2img = ImageSelfAttention(nf(img2img, fmap_base, fmap_max), a.get("pos_dim") or latent_dim,
+                                              integration=a.get("integration", "mul"), norm=a.get("norm", "layer"),
+                                              use_pos=a.get("use_pos", True), exact_fp32=a.get("exact_fp32", False))
         self.num_attention_layers = sum(1 for l in self.layers if l.attention is not None)
         # index into per-layer latents [B, num_ws, k+1, D] of every style affine (conv layers, then tRGBs): conv layer i reads
         # index i, the tRGB of a block reads the index after its block's last conv layer (SURVEY A.4 item 13)
@@ -476,7 +488,8 @@ class SynthesisNetwork(nn.Module):
                 if j == 0 and nl == 2 and styles_all[li + 1] is not None and layer.fusable(x) and not return_features:
                     post_scale = styles_all[li + 1]
                 rgb_args = None
-                if j == nl - 1 and layer.fusable(x) and not return_features and not os.environ.get("GF_NO_TORGB_EPILOGUE"):
+                if j == nl - 1 and layer.fusable(x) and not return_features and res != self.img2img_res \
+                        and not os.environ.get("GF_NO_TORGB_EPILOGUE"):
                     # last layer of the block on the wgmma path (C <= 256, or 512 with k <= 16): the attention kernel's store side computes the
                     # tRGB planes from the layer output and writes x * (next block's style): the tRGB pass disappears
                     C_ = layer.weight.shape[0]
@@ -499,6 +512,8 @@ class SynthesisNetwork(nn.Module):
                     atts.append(att)
                 if return_features and layer.attention is not None:
                     feats.append(x)
+            if res == self.img2img_res:        # the block's activation is attended, then read by its tRGB (and scaled for the next block)
+                x = self.img2img(x.permute(0, 2, 3, 1).contiguous()).permute(0, 3, 1, 2)
             if rgb is not None:
                 block_prescaled = nxt is not None
             else:
@@ -515,14 +530,19 @@ class Generator(nn.Module):
     """G_GANsformer.  ``G(z, c=None, truncation_psi=1.0, noise_mode='const', return_att=False) -> img [B,3,R,R]``.
 
     ``c_dim > 0``: class-conditional (SURVEY A.4 item 14).  Every call then takes labels c [B, c_dim] (one-hot or any real weights),
-    which act through the mapping network's label embedding only; with the default ``c_dim = 0`` c is ignored."""
+    which act through the mapping network's label embedding only; with the default ``c_dim = 0`` c is ignored.
+
+    ``img2img = r`` (SURVEY A.4 item 18): image self-attention (``ImageSelfAttention``, with the generator's integration, norm and
+    use_pos) on the output of block r, after its last synthesis layer and before its tRGB; r is a block resolution in 8 .. resolution.
+    The layer has no latent input: num_ws, style mixing and the latent routing are unchanged.  0 (the default) builds exactly the
+    network without it."""
 
     def __init__(self, resolution: int = 256, components_num: int = 16, latent_size: int = 512, latent_dim: Optional[int] = None,
                  transformer: bool = True, g_start_res: int = 8, g_end_res: Optional[int] = None, kmeans: bool = False,
                  kmeans_iters: int = 1, iterative: bool = False, integration: str = "mul", norm: Optional[str] = "layer",
                  use_pos: bool = True, pos_dim: Optional[int] = None, num_heads: int = 1, mapping_layers: int = 8,
                  fmap_base: int = 16384, fmap_max: int = 512, exact_fp32: bool = False, ltnt2ltnt: bool = False, g_img2ltnt: bool = False,
-                 att_dp: float = 0.0, c_dim: int = 0):
+                 att_dp: float = 0.0, c_dim: int = 0, img2img: int = 0):
         super().__init__()
         # SURVEY A.4 item 1: D = latent_size // components_num unless given
         self.latent_dim = latent_dim if latent_dim is not None else max(latent_size // max(components_num, 1), 1)
@@ -535,7 +555,7 @@ class Generator(nn.Module):
         self.c_dim = int(c_dim)
         self.synthesis = SynthesisNetwork(resolution, self.latent_dim, components_num, fmap_base=fmap_base, fmap_max=fmap_max,
                                           g_start_res=g_start_res, g_end_res=g_end_res, transformer=transformer,
-                                          attn_kwargs=attn_kwargs)
+                                          attn_kwargs=attn_kwargs, img2img=img2img)
 
     def forward(self, z: torch.Tensor, c=None, truncation_psi: float = 1.0, noise_mode: str = "const", return_att: bool = False,
                 return_features: bool = False):

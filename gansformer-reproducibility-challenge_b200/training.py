@@ -61,6 +61,7 @@ from .attention import BipartiteAttention
 from .autograd import _e, composite_forward
 from .networks import FullyConnected, nf
 from ._state import bump_weights_epoch
+from .self_attention import ImageSelfAttention
 from .ops import IMGFILTER_HALO, augment, augment_filter, fir4, fir_filter, upfirdn2d_ref
 
 SQRT2 = math.sqrt(2.0)
@@ -160,21 +161,28 @@ class Discriminator(nn.Module):
     composite's [B,n,C] projections.  The R1 gradients then differ from the default route by round-off.
 
     ``c_dim > 0`` (SURVEY A.4 item 14, StyleGAN2's projection discriminator): fc1 has c_dim outputs and ``D(img, c)`` returns the
-    sum over them weighted by the labels c [B, c_dim].  ``c_dim = 0`` (the default) is the unconditional network, and ignores c."""
+    sum over them weighted by the labels c [B, c_dim].  ``c_dim = 0`` (the default) is the unconditional network, and ignores c.
+
+    ``img2img = r`` (SURVEY A.4 item 18): image self-attention (``ImageSelfAttention``, with the discriminator's integration, norm and
+    use_pos, positional width latent_dim) on the activation entering the block of input resolution r, in 8 .. resolution.  Its R1
+    pass differentiates the layer's backward through the torch composite."""
 
     def __init__(self, resolution: int = 256, fmap_base: int = 16384, fmap_max: int = 512, mbstd_group: int = 4,
                  transformer: bool = False, components_num: int = 16, latent_dim: int = 32, d_start_res: int = 8,
                  d_end_res: Optional[int] = None, integration: str = "mul", norm: Optional[str] = "layer", use_pos: bool = True,
-                 exact_fp32: bool = False, r1_kernels: bool = False, c_dim: int = 0):
+                 exact_fp32: bool = False, r1_kernels: bool = False, c_dim: int = 0, img2img: int = 0):
         super().__init__()
         if c_dim < 0:
             raise ValueError(f"c_dim must be >= 0, got {c_dim}")
+        if img2img and not (8 <= img2img <= resolution and img2img & (img2img - 1) == 0):
+            raise ValueError(f"img2img must be 0 (off) or a block resolution in 8 .. {resolution}, got {img2img}")
         self.resolution, self.mbstd_group, self.transformer, self.c_dim = resolution, mbstd_group, transformer, int(c_dim)
         log2 = int(math.log2(resolution))
         d_end_res = resolution if d_end_res is None else d_end_res
         att = dict(components_num=components_num, latent_dim=latent_dim, integration=integration, norm=norm, use_pos=use_pos,
                    exact_fp32=exact_fp32, r1_kernels=r1_kernels) if transformer else None
         self.fromrgb = EqConv2d(3, nf(resolution, fmap_base, fmap_max), 1)
+        self.block_resolutions = [2 ** i for i in range(log2, 2, -1)]                    # input resolution of each block
         self.blocks = nn.ModuleList([DiscriminatorBlock(nf(2 ** i, fmap_base, fmap_max), nf(2 ** (i - 1), fmap_base, fmap_max), 2 ** i,
                                                         att if d_start_res <= 2 ** i <= d_end_res else None)
                                      for i in range(log2, 2, -1)])
@@ -184,6 +192,10 @@ class Discriminator(nn.Module):
         self.fc1 = FullyConnected(c4, max(c_dim, 1))
         if transformer:
             self.latents = nn.Parameter(torch.randn(components_num, latent_dim))
+        self.img2img_res = int(img2img)
+        if img2img:
+            self.img2img = ImageSelfAttention(nf(img2img, fmap_base, fmap_max), latent_dim, integration=integration, norm=norm,
+                                              use_pos=use_pos, exact_fp32=exact_fp32)
 
     def forward(self, img, c: Optional[torch.Tensor] = None):
         if self.c_dim > 0:
@@ -197,7 +209,9 @@ class Discriminator(nn.Module):
         if self.transformer:
             y = self.latents[None].expand(img.shape[0], -1, -1).contiguous()
             composite = torch.is_grad_enabled() and img.requires_grad and any(p.requires_grad for p in self.parameters())
-        for blk in self.blocks:
+        for blk, res in zip(self.blocks, self.block_resolutions):
+            if res == self.img2img_res:
+                x = self.img2img(x.permute(0, 2, 3, 1).contiguous()).permute(0, 3, 1, 2)
             x, y = blk(x, y, composite)
         B, C, H, W = x.shape                                            # minibatch standard deviation, one feature map
         G = min(self.mbstd_group, B)

@@ -178,6 +178,23 @@ int gf_augment_filter_nchw(const float* x, float* y, const float* gains, const f
  * CUDA-graph replay.  gains is required; otherwise the arguments and errors of gf_augment_filter_nchw. */
 int gf_augment_filter_adjoint_nchw(const float* gy, float* gx, const float* gains, int B, int C, int H, int W, void* stream);
 
+/* Image self-attention (img2img, SURVEY A.4 item 18): the n x n part of the layer, per image b and head j, on wgmma (TF32 operands,
+ * fp32 accumulation), streamed over 64-token tiles with an online softmax; no n x n tensor is stored (csrc/gf_self_attn.cu).
+ * Tensors are channels-last [B, n, C]; head j is the column segment [j d, (j+1) d), h = C / d heads.
+ *   O_j = softmax_keys(Q_j K_j^T * scale) V_j,   lse [B, h, n] = log2 sum_keys 2^(Q_j K_j^T * scale * log2 e)  (base-2 units).
+ * wgmma reads 32-bit operands along their contraction index only, so the products that contract over tokens take per-head
+ * transposed copies instead of the natural tensors: vt = V^T, qt = Q^T, kt = K^T, dOt = dO^T, each [B, C, n] (= [B, h, d, n]).
+ * The backward recomputes P from q, k and lse and writes dq, dk, dv [B, n, C]; delta [B, h, n] is scratch it fills with
+ * rowsum(dO o O).  Every output element is accumulated by one thread in a fixed order (no atomics): the same bits on every call.
+ * Both enqueue on `stream` only: no allocation, no host synchronisation (CUDA-graph capturable).
+ * Errors, before the device is touched: GF_ERR_INVALID for a NULL or not 16-byte aligned pointer, a size <= 0, C % d != 0 or a
+ * scale that is not positive and finite; GF_ERR_UNSUPPORTED for d not in {32, 64}, n % 64 != 0, B > 65535 or B*n*C >= 2^31. */
+int gf_self_attn_fwd(const float* q, const float* k, const float* vt, float* o, float* lse, int B, int n, int C, int d, float scale,
+                     void* stream);
+int gf_self_attn_bwd(const float* q, const float* qt, const float* k, const float* kt, const float* v, const float* o, const float* lse,
+                     const float* dO, const float* dOt, float* delta, float* dq, float* dk, float* dv, int B, int n, int C, int d,
+                     float scale, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
