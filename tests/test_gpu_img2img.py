@@ -4,7 +4,7 @@
   units (every other exp2 underflows to exactly 0) give O equal to that key's V row and, backward, dQ = dK = 0 and dV = P^T dO, bit for
   bit; all-zero queries give P = 1/n exactly, so O is the exact mean of integer V; another head's channels and other images do not
   change a head's bits.
-* Against the fp64 oracle (oracle/self_attention.py) at n in {64, 256, 1024, 4096}, d in {32, 64}, B in {1, 3}: O and the three
+* Against the fp64 oracle (oracle/self_attention.py) at n in {64, 192, 256, 576, 1024, 4096}, d in {32, 64}, B in {1, 3}: O and the three
   gradients under frozen bounds; the backward is deterministic.
 * ``ImageSelfAttention`` on the kernels against its torch composite (exact_fp32=True), and the composite against fp64.
 * Generator and discriminator with img2img against tests/img2img_ref.py in both precision modes; a small training run with R1, path
@@ -63,7 +63,7 @@ def _one_hot_case(B, n, h, d, dev, seed=0):
     return [t.to(dev) for t in (q, k, v, do)] + [win]
 
 
-@pytest.mark.parametrize("n,d", [(64, 32), (64, 64), (256, 64), (1024, 32)])
+@pytest.mark.parametrize("n,d", [(64, 32), (64, 64), (192, 32), (256, 64), (576, 64), (1024, 32)])
 def test_one_hot_forward_and_backward_exact(gf, cuda_dev, n, d):
     sa = _sa()
     B, h = 2, 2
@@ -121,7 +121,7 @@ def test_heads_and_images_are_independent(gf, cuda_dev):
 
 @pytest.mark.parametrize("B", [1, 3])
 @pytest.mark.parametrize("d", [32, 64])
-@pytest.mark.parametrize("n", [64, 256, 1024, 4096])
+@pytest.mark.parametrize("n", [64, 192, 256, 576, 1024, 4096])
 def test_against_fp64(gf, cuda_dev, n, d, B):
     sa = _sa()
     h = 2

@@ -1,7 +1,7 @@
-"""Image self-attention (img2img, SURVEY A.4 item 18) without a GPU: the oracle against an online-softmax restatement, the argument
+"""Image self-attention (img2img, SURVEY A.4 item 18) without a GPU: the oracle against the kernels' online softmax (restated in
+oracle/self_attention_exact.py with its roundings off), the argument
 checks of gf_self_attn_fwd / gf_self_attn_bwd through ctypes, and the construction of G and D with and without the layer."""
 import json
-import math
 import os
 import subprocess
 import sys
@@ -11,31 +11,11 @@ import pytest
 import torch
 
 from oracle import self_attention as osa
+from oracle import self_attention_exact as sx
 from tests import img2img_ref as iref
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 TRAIN = "gansformer-reproducibility-challenge_b200.training"
-
-
-def _online(q, k, v, heads, tile=64):
-    """The n x n part as the kernels stream it: 64-key tiles, running maximum and sum in log2 units, rescaled accumulators."""
-    B, n, C = q.shape
-    d = C // heads
-    sl2 = 1.0 / math.sqrt(d) / math.log(2.0)
-    sp = lambda t: t.reshape(B, n, heads, d).transpose(1, 2)
-    qh, kh, vh = sp(q), sp(k), sp(v)
-    m = torch.full((B, heads, n, 1), -math.inf, dtype=q.dtype)
-    l = torch.zeros(B, heads, n, 1, dtype=q.dtype)
-    o = torch.zeros(B, heads, n, d, dtype=q.dtype)
-    for k0 in range(0, n, tile):
-        x = (qh @ kh[:, :, k0:k0 + tile].transpose(2, 3)) * sl2
-        mn = torch.maximum(m, x.amax(dim=3, keepdim=True))
-        alpha = torch.exp2(m - mn)
-        p = torch.exp2(x - mn)
-        l = l * alpha + p.sum(dim=3, keepdim=True)
-        o = o * alpha + p @ vh[:, :, k0:k0 + tile]
-        m = mn
-    return (o / l).transpose(1, 2).reshape(B, n, C), (m + torch.log2(l))[..., 0]
 
 
 @pytest.mark.parametrize("n,C", [(64, 32), (256, 128), (1024, 64)])
@@ -44,7 +24,7 @@ def test_oracle_against_online_softmax(n, C):
     q, k, v = (torch.randn(2, n, C, generator=g, dtype=torch.float64) * 3 for _ in range(3))
     h = osa.heads_of(C)
     o, lse = osa.attention(q, k, v, h)
-    o2, lse2 = _online(q, k, v, h)
+    o2, lse2 = sx.forward(q, k, v, h, rounded=False)              # the kernels' 64-key streaming in float64
     assert torch.allclose(o, o2, rtol=1e-12, atol=1e-12)
     assert torch.allclose(lse, lse2, rtol=1e-12, atol=1e-12)
 
