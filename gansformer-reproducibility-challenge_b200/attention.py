@@ -366,11 +366,11 @@ class BipartiteAttention(nn.Module):
     """
 
     # Opt-in (per module) for a duplex layer: the backward is always the duplex kernel backward (autograd._duplex_kernel_backward),
-    # with or without dropout, and the centroids output is differentiable.  That backward has no derivative of its own, so it
-    # raises when called with grad mode on (create_graph).  The discriminator sets it; generator layers keep their routes.
+    # with or without dropout, and the centroids output is differentiable.  Without kernel_double_backward that backward raises
+    # when called with grad mode on (create_graph).  The discriminator sets it; generator layers keep their routes.
     kernel_backward = False
     # Opt-in on top of kernel_backward: that backward, run with grad mode on, builds a graph the double-backward kernels
-    # differentiate (autograd._duplex_kernel_backward_graph) instead of raising.  Discriminator(r1_kernels=True) sets it.
+    # differentiate (the same autograd._duplex_kernel_backward) instead of raising.  Discriminator(r1_kernels=True) sets it.
     kernel_double_backward = False
 
     def __init__(self, dim: int, latent_dim: int, components_num: int, pos_dim: Optional[int] = None,
@@ -407,14 +407,17 @@ class BipartiteAttention(nn.Module):
             return {}
         return dict(att_dp=self.att_dp, dp_salt=self.dp_salt, dp_state=dropout_state(device))
 
+    def backward_kernels_serve(self) -> bool:
+        """Whether the attention backward kernels serve this layer (on float32 CUDA tensors): one head, norm layer / none, simplex
+        or duplex with kmeans_iters == 1."""
+        return self.num_heads == 1 and self.norm in ("layer", None, "none") and (not self.duplex or self.kmeans_iters == 1)
+
     def _check_dropout_supported(self, centroids_init=None) -> None:
-        """Attention dropout in training mode runs on single-head layers: simplex, or duplex with kmeans_iters == 1, norm layer /
-        none and no carried-in centroids (`iterative`).  Anything else raises NotImplementedError."""
+        """Attention dropout in training mode runs on the layers the backward kernels serve (the torch composite cannot regenerate
+        the kernels' mask), without carried-in centroids (`iterative`).  Anything else raises NotImplementedError."""
         if not (self.training and self.att_dp > 0.0):
             return
-        if self.num_heads == 1 and not self.duplex:
-            return
-        if self.num_heads == 1 and self.kmeans_iters == 1 and self.norm in ("layer", None, "none") and centroids_init is None:
+        if self.backward_kernels_serve() and (centroids_init is None or not self.duplex):
             return
         raise NotImplementedError("attention dropout is implemented for single-head layers: simplex, or duplex with kmeans_iters == 1, "
                                   "norm layer / none and no iterative centroid carry")

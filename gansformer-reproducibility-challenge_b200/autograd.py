@@ -1,29 +1,31 @@
 """Differentiable wrapper of the fused attention op (needed by the G/D training step, SURVEY row f2).
 
-Forward = the C-ABI CUDA kernels.  Backward of a simplex layer with layer norm (or none): the hand-written stage-T
-backward kernel ``gf_attn_simplex_bwd`` (activation gradient + the per-token gradients of logits / control signal), two
-batched GEMMs for the reductions over tokens, and torch autograd through the tiny per-image tables of stages W and I
-(``folded_tables``).  Backward of a duplex layer (one k-means iteration, layer norm / none) whose forward ran with attention
-dropout: the same stage-T kernel with keys from the centroids, plus the pass-A kernels ``gf_attn_centroid_stats`` /
-``gf_attn_centroid_bwd`` and autograd through the pass-A tables (``centroid_tables``), see ``_duplex_kernel_backward``.
-A duplex module with ``kernel_backward = True`` (the discriminator's layers) takes that route without dropout too, and its
-centroids output is differentiable (the cotangent joins the same autograd call).  With ``kernel_double_backward = True`` as well,
-that backward run with create_graph=True (the discriminator's R1 penalty) builds a graph of three Functions, each differentiable once more,
-whose own backward are the double-backward kernels ``gf_attn_simplex_bwd_vjp`` / ``gf_attn_centroid_bwd_vjp``, see
-``_duplex_kernel_backward_graph``.
-A generator layer's backward run with create_graph=True (the path-length penalty) builds a graph on every route: the simplex kernel
-route through ``_simplex_kernel_backward_graph``, the duplex route with dropout through ``_duplex_kernel_backward_graph``, both
-with the forward's dropout mask in ``gf_attn_simplex_bwd_vjp_ex``, and the composite route through autograd with create_graph=True.
-Everything else (duplex without dropout, instance / batch norm, multi-head, CPU tensors): PyTorch autograd through a
-recomputation of the direct-form algebra with torch ops (``composite_forward``).
+Forward = the C-ABI CUDA kernels.  ``_FusedAttention.backward`` takes one of three routes:
+* simplex kernels (``_simplex_kernel_backward``), for a simplex layer with layer norm (or none): the hand-written stage-T backward
+  kernel ``gf_attn_simplex_bwd_ex`` (activation gradient + the per-token gradients of logits / control signal), two batched GEMMs
+  for the reductions over tokens, and torch autograd through the tiny per-image tables of stages W and I (``folded_tables``);
+* duplex kernels (``_duplex_kernel_backward``), for a duplex layer (one k-means iteration, layer norm / none) whose forward ran with
+  attention dropout, or whose module sets ``kernel_backward`` (the discriminator's layers, whose centroids output is then
+  differentiable): the same stage-T kernel with keys from the centroids, plus the pass-A kernels ``gf_attn_centroid_stats`` /
+  ``gf_attn_centroid_bwd`` and autograd through the pass-A tables (``centroid_tables``);
+* composite (``_composite_backward``), everything else (duplex without dropout, instance / batch norm, multi-head, CPU tensors):
+  PyTorch autograd through a recomputation of the direct-form algebra with torch ops (``composite_forward``).
+Each route serves both orders.  Run with create_graph=True (the generator's path-length penalty; the discriminator's R1 penalty
+when its modules set ``kernel_double_backward``), a kernel route builds a graph: the per-token work runs in three Functions,
+``_StageTBackward``, ``_CentroidStats`` and ``_CentroidBackward``, whose own backward are the double-backward kernels
+``gf_attn_simplex_bwd_vjp`` (``_ex`` with the forward's dropout mask) / ``gf_attn_centroid_bwd_vjp``.  A first-order backward calls
+their forward bodies directly and leaves no graph behind.
 """
 from __future__ import annotations
 
 import contextlib
+import ctypes
 import math
 
 import torch
 from torch.autograd.function import once_differentiable
+
+from . import _lib
 
 
 def _e(w):
@@ -186,15 +188,6 @@ def folded_tables(y, p, *, H, W, C, integration, use_pos, centroids=None, img2lt
     return Kp.contiguous(), Vt.contiguous(), Rt.contiguous(), Ct.contiguous(), cb.contiguous()
 
 
-def _kernel_backward_ok(m, x) -> bool:
-    return (not m.duplex) and m.norm in ("layer", None, "none") and m.num_heads == 1 and x.is_cuda and x.dtype == torch.float32
-
-
-def _duplex_kernel_backward_ok(m, x) -> bool:
-    return m.duplex and m.kmeans_iters == 1 and m.norm in ("layer", None, "none") and m.num_heads == 1 and x.is_cuda \
-        and x.dtype == torch.float32
-
-
 class _FusedAttention(torch.autograd.Function):
     @staticmethod
     def forward(ctx, module, centroids, return_att, names, x, y, *params):
@@ -217,54 +210,35 @@ class _FusedAttention(torch.autograd.Function):
     def backward(ctx, g_out, g_att, g_cen):
         m = ctx.module
         x, y, *params = ctx.saved_tensors
+        # grad mode on: the backward runs with create_graph=True (the generator's path-length penalty, the discriminator's R1
+        # penalty) and must itself be differentiable; each route below serves both orders
+        create_graph = torch.is_grad_enabled()
+        kernels = m.backward_kernels_serve() and x.is_cuda and x.dtype == torch.float32
         if m.kernel_backward and m.duplex:
-            if torch.is_grad_enabled():
-                if not m.kernel_double_backward:
-                    raise RuntimeError("the duplex kernel backward has no derivative of its own (create_graph=True): run the layer "
-                                       "through composite_forward for higher-order gradients, as Discriminator does in the R1 pass")
-                if ctx.dropout or ctx.centroids is not None or not _duplex_kernel_backward_ok(m, x):
-                    raise NotImplementedError("kernel_double_backward serves single-head duplex layers with kmeans_iters == 1, "
-                                              "norm layer / none, computed centroids, no attention dropout, float32 CUDA tensors")
-                return (None, None, None, None, *_duplex_kernel_backward_graph(m, ctx.names, x, y, params, g_out,
-                                                                               g_cen if ctx.cen_grad else None))
-            if not _duplex_kernel_backward_ok(m, x):
+            if create_graph and not m.kernel_double_backward:
+                raise RuntimeError("the duplex kernel backward has no derivative of its own (create_graph=True): run the layer "
+                                   "through composite_forward for higher-order gradients, as Discriminator does in the R1 pass")
+            if create_graph and (ctx.dropout or ctx.centroids is not None or not kernels):
+                raise NotImplementedError("kernel_double_backward serves single-head duplex layers with kmeans_iters == 1, "
+                                          "norm layer / none, computed centroids, no attention dropout, float32 CUDA tensors")
+            if not kernels:
                 raise NotImplementedError("kernel_backward serves single-head duplex layers with kmeans_iters == 1, norm layer / none, "
                                           "float32 CUDA tensors")
-            return (None, None, None, None, *_duplex_kernel_backward(m, ctx.names, x, y, params, g_out, ctx.dropout, ctx.centroids,
-                                                                     g_cen if ctx.cen_grad else None))
-        # grad mode on: the backward runs with create_graph=True (the generator's path-length penalty) and must itself be
-        # differentiable; the first-order calls below are the same with it off
-        graph = torch.is_grad_enabled()
-        if _kernel_backward_ok(m, x):
-            if graph:
-                return (None, None, None, None, *_simplex_kernel_backward_graph(m, ctx.names, x, y, params, g_out, ctx.dropout))
-            return (None, None, None, None, *_kernel_backward(m, ctx.names, x, y, params, g_out, ctx.dropout))
-        if ctx.dropout and _duplex_kernel_backward_ok(m, x):
-            if graph:
-                if ctx.centroids is not None:
-                    raise NotImplementedError("a duplex layer with attention dropout and given centroids has no second derivative "
-                                              "on the kernels")
-                return (None, None, None, None, *_duplex_kernel_backward_graph(m, ctx.names, x, y, params, g_out, dropout=ctx.dropout))
-            return (None, None, None, None, *_duplex_kernel_backward(m, ctx.names, x, y, params, g_out, ctx.dropout, ctx.centroids))
-        if ctx.dropout:
+            route = _duplex_kernel_backward
+        elif kernels and not m.duplex:
+            route = _simplex_kernel_backward
+        elif kernels and ctx.dropout:
+            if create_graph and ctx.centroids is not None:
+                raise NotImplementedError("a duplex layer with attention dropout and given centroids has no second derivative "
+                                          "on the kernels")
+            route = _duplex_kernel_backward
+        elif ctx.dropout:
             raise NotImplementedError("attention dropout needs the backward kernels: single-head layers with norm layer / none, "
                                       "simplex or duplex with kmeans_iters == 1")
-        if graph:                          # composite route, differentiable again: autograd on the saved tensors themselves
-            xs, ys, ps = _alias(x), _alias(y), [_alias(p) for p in params]
-            out, _ = composite_forward(xs, ys, dict(zip(ctx.names, ps)), integration=m.integration, norm=m.norm,
-                                       duplex=m.duplex, use_pos=m.use_pos, centroids=ctx.centroids, kmeans_iters=m.kmeans_iters,
-                                       img2ltnt=m.img2ltnt, num_heads=m.num_heads)
-            grads = torch.autograd.grad(out, [xs, ys, *ps], g_out, allow_unused=True, create_graph=True)
-            return (None, None, None, None, *grads)
-        with torch.enable_grad():
-            xs = x.detach().requires_grad_(True)
-            ys = y.detach().requires_grad_(True)
-            ps = [p.detach().requires_grad_(True) for p in params]
-            out, _ = composite_forward(xs, ys, dict(zip(ctx.names, ps)), integration=m.integration, norm=m.norm,
-                                       duplex=m.duplex, use_pos=m.use_pos, centroids=ctx.centroids, kmeans_iters=m.kmeans_iters,
-                                       img2ltnt=m.img2ltnt, num_heads=m.num_heads)
-            grads = torch.autograd.grad(out, [xs, ys, *ps], g_out, allow_unused=True)
-        return (None, None, None, None, *grads)
+        else:
+            route = _composite_backward
+        return (None, None, None, None, *route(m, ctx.names, x, y, params, g_out, ctx.dropout, ctx.centroids,
+                                               g_cen if ctx.cen_grad else None))
 
 
 @contextlib.contextmanager
@@ -280,17 +254,38 @@ def _fp32_matmul():
         torch.backends.cuda.matmul.allow_tf32 = prev
 
 
+def _alias(t):
+    """A differentiable alias of t: autograd.grad with respect to it does not follow the other paths that reach t."""
+    return t.view_as(t) if t.requires_grad else t.detach().requires_grad_(True)
+
+
+def _leaf(t, create_graph):
+    """What a backward route differentiates its recomputation with respect to: under create_graph an alias of the saved tensor, so
+    the gradients it returns stay connected to the graph; otherwise a detached leaf, so that no graph outlives the call."""
+    return _alias(t) if create_graph else t.detach().requires_grad_(True)
+
+
+def _sum_grads(a, b):
+    return [u if v is None else (v if u is None else u + v) for u, v in zip(a, b)]
+
+
+# The three routes share one signature, (module, parameter names, x, y, parameters, dOut, dropout post-op, given centroids,
+# cotangent of the centroids output); a route ignores what its layers cannot have.
+
 @_fp32_matmul()
-def _kernel_backward(m, names, x, y, params, g_out, dropout=None):
-    """d(loss)/d(x, y, params) of a simplex layer through gf_attn_simplex_bwd (see the module docstring)."""
+def _simplex_kernel_backward(m, names, x, y, params, g_out, dropout=None, centroids=None, g_cen=None):
+    """d(loss)/d(x, y, params) of a simplex layer through gf_attn_simplex_bwd_ex (see the module docstring): the tables (with cb
+    under dropout) from leaves of y and the parameters, the per-token work of ``_stage_t_backward`` (``_StageTBackward`` under
+    create_graph), and autograd back through stages W and I."""
+    create_graph = torch.is_grad_enabled()
     B, H, W, C = x.shape
     with torch.enable_grad():
-        ys = y.detach().requires_grad_(True)
-        ps = [p.detach().requires_grad_(True) for p in params]
-        tables = folded_tables(ys, dict(zip(names, ps)), H=H, W=W, C=C, integration=m.integration, use_pos=m.use_pos)
-    dX, outs, grads = _stage_t_backward(m, x, y.shape[1], y.shape[2], g_out, tables, dropout)
-    gy, *gp = torch.autograd.grad(outs, [ys, *ps], grads, allow_unused=True)
-    return (dX, gy, *gp)
+        ys, ps = _leaf(y, create_graph), [_leaf(p, create_graph) for p in params]
+        Kp, Vt, Rt, Ct, cb = folded_tables(ys, dict(zip(names, ps)), H=H, W=W, C=C, integration=m.integration, use_pos=m.use_pos)
+    stage_t = _StageTBackward.apply if create_graph else _stage_t_backward
+    dX, *grads = stage_t(m, y.shape[1], y.shape[2], dropout, x.contiguous(), g_out, Kp, Vt, Rt, Ct, cb if dropout else None)
+    outs = [Kp, Vt, Rt, Ct] + ([cb] if dropout else [])
+    return (dX, *torch.autograd.grad(outs, [ys, *ps], grads, allow_unused=True, create_graph=create_graph))
 
 
 @_fp32_matmul()
@@ -303,106 +298,58 @@ def _duplex_kernel_backward(m, names, x, y, params, g_out, dropout=None, centroi
          cotangent of the centroids output) Cen is one more (output, cotangent) pair of that autograd call;
       4. r = dXbar . Xbar, then gf_attn_centroid_bwd adds the pass-A part into dX and gives dS of the pass-A logits;
       5. dM = dS^T X, dRt2 / dCt2 = sums of dS, and autograd over the pass-A tables.
+    y and the parameters enter the stage-T tables and the pass-A tables through separate leaves, so that the gradient of the
+    stage-T tables stops at Xbar, while under create_graph Xbar stays connected to X and the pass-A tables.  There the per-token
+    work of steps 1, 3 and 4 runs in ``_CentroidStats``, ``_StageTBackward`` and ``_CentroidBackward``, whose backward are the
+    double-backward kernels; saved for the second pass: X, dOut and the per-image tables.  In first order it runs in their forward
+    bodies, and gf_attn_centroid_bwd adds into stage T's dX in place.
     With ``centroids`` given, pass A did not run in the forward: steps 1, 4 and 5 are skipped and the centroids get no gradient."""
-    B, H, W, C = x.shape
-    k, D = y.shape[1], y.shape[2]
-    xc = x.detach().contiguous()
-    with torch.enable_grad():
-        ys = y.detach().requires_grad_(True)
-        ps = [p.detach().requires_grad_(True) for p in params]
-        pdict = dict(zip(names, ps))
-        if centroids is None:
-            cen_tabs = centroid_tables(ys, pdict, H, W, C, m.use_pos)
-            xbar, lse = _centroid_stats(m, xc, k, D, *(t.detach() for t in cen_tabs))
-            xbar.requires_grad_(True)
-            cen = xbar @ _e(pdict["wv2"]) + pdict["bv2"]
-        else:
-            cen = centroids.detach()
-        tables = folded_tables(ys, pdict, H=H, W=W, C=C, integration=m.integration, use_pos=m.use_pos, centroids=cen, img2ltnt=m.img2ltnt)
-    dX, outs, grads = _stage_t_backward(m, x, k, D, g_out, tables, dropout)
-    if g_cen is not None:
-        outs, grads = outs + [cen], grads + [g_cen.contiguous()]
-    leaves = [ys, *ps] + ([xbar] if centroids is None else [])
-    g1 = list(torch.autograd.grad(outs, leaves, grads, allow_unused=True))
-    if centroids is None:
-        dxbar = g1.pop().contiguous()
-        r = (dxbar * xbar.detach()).sum(dim=2).contiguous()                # [B, k]
-        dS = _centroid_bwd(m, xc, k, D, *(t.detach() for t in cen_tabs), lse, dxbar, r, dX)
-        KP = dS.shape[2]
-        dM = torch.bmm(dS.transpose(1, 2), xc.reshape(B, H * W, C))     # [B, KP, C]
-        dS4 = dS.reshape(B, H, W, KP)
-        Mt, Rt2, Ct2 = cen_tabs
-        g2 = torch.autograd.grad([Mt, Rt2, Ct2], [ys, *ps], [dM, dS4.sum(dim=2), dS4.sum(dim=1)], allow_unused=True)
-        g1 = [a if b is None else (b if a is None else a + b) for a, b in zip(g1, g2)]
-        i = 1 + names.index("bk2")     # constant over the tokens, bk2 cancels in pass A's softmax: its gradient is exactly 0
-        g1[i] = torch.zeros_like(params[i - 1])
-    return (dX, *g1)
-
-
-def _alias(t):
-    """A differentiable alias of t: autograd.grad with respect to it does not follow the other paths that reach t."""
-    return t.view_as(t) if t.requires_grad else t.detach().requires_grad_(True)
-
-
-def _sum_grads(a, b):
-    return [u if v is None else (v if u is None else u + v) for u, v in zip(a, b)]
-
-
-@_fp32_matmul()
-def _simplex_kernel_backward_graph(m, names, x, y, params, g_out, dropout=None):
-    """``_kernel_backward`` as a graph that can be differentiated once more, for a backward run with create_graph=True (the
-    generator's path-length penalty): the tables (with cb under dropout) are built from the graph-connected y and parameters, the
-    per-token work is ``_StageTBackward`` (backward: gf_attn_simplex_bwd_vjp_ex, the same dropout mask), and autograd takes the
-    table gradients back through stages W and I with create_graph=True."""
-    B, H, W, C = x.shape
-    ys, ps = _alias(y), [_alias(p) for p in params]
-    Kp, Vt, Rt, Ct, cb = folded_tables(ys, dict(zip(names, ps)), H=H, W=W, C=C, integration=m.integration, use_pos=m.use_pos)
-    dX, *grads = _StageTBackward.apply(m, y.shape[1], y.shape[2], dropout or None, x.contiguous(), g_out, Kp, Vt, Rt, Ct,
-                                       cb if dropout else None)
-    outs = [Kp, Vt, Rt, Ct] + ([cb] if dropout else [])
-    g = torch.autograd.grad(outs, [ys, *ps], grads, allow_unused=True, create_graph=True)
-    return (dX, *g)
-
-
-@_fp32_matmul()
-def _duplex_kernel_backward_graph(m, names, x, y, params, g_out, g_cen=None, dropout=None):
-    """``_duplex_kernel_backward`` (computed centroids) as a graph that can be differentiated once more, for a backward run with
-    create_graph=True (the discriminator's R1 penalty, the generator's path-length penalty).  The tables are built from the
-    graph-connected y and parameters; the per-token work runs in three once-differentiable Functions whose backward are the
-    double-backward kernels:
-      _CentroidStats    X, pass-A tables -> Xbar, lse           (backward: gf_attn_centroid_bwd with r - lse cotangent)
-      _StageTBackward   X, dOut, tables (+ cb) -> dX, dKp, dVt, dRt, dCt (+ dcb) (backward: gf_attn_simplex_bwd_vjp_ex; with
-                        ``dropout``, the mask of the forward, which only stage T has)
-      _CentroidBackward X, pass-A tables, lse, dXbar, r, dX -> dX + pass A, dM, dRt2, dCt2 (backward: gf_attn_centroid_bwd_vjp)
-    y and the parameters enter the stage-T tables and the pass-A tables through separate aliases, so that the gradient of the
-    stage-T tables stops at Xbar, as in the first-order route, while Xbar stays connected to X and the pass-A tables.  Saved for
-    the second pass: X, dOut and the per-image tables."""
+    create_graph = torch.is_grad_enabled()
+    if create_graph:
+        stats, stage_t, pass_a_backward = _CentroidStats.apply, _StageTBackward.apply, _CentroidBackward.apply
+    else:
+        stats, stage_t, pass_a_backward = _centroid_stats, _stage_t_backward, _centroid_backward
     B, H, W, C = x.shape
     k, D = y.shape[1], y.shape[2]
     xc = x.contiguous()
-    y1, y2 = _alias(y), _alias(y)
-    p1, p2 = [_alias(p) for p in params], [_alias(p) for p in params]
+    y1, y2 = _leaf(y, create_graph), _leaf(y, create_graph)
+    p1, p2 = [_leaf(p, create_graph) for p in params], [_leaf(p, create_graph) for p in params]
     d1, d2 = dict(zip(names, p1)), dict(zip(names, p2))
-    cen_tabs = centroid_tables(y2, d2, H, W, C, m.use_pos)
-    xbar, lse = _CentroidStats.apply(m, k, D, xc, *cen_tabs)
-    if not xbar.requires_grad:
-        xbar.requires_grad_(True)
-    cen = xbar @ _e(d1["wv2"]) + d1["bv2"]
-    Kp, Vt, Rt, Ct, cb = folded_tables(y1, d1, H=H, W=W, C=C, integration=m.integration, use_pos=m.use_pos, centroids=cen,
-                                       img2ltnt=m.img2ltnt)
-    dX, *grads = _StageTBackward.apply(m, k, D, dropout or None, xc, g_out, Kp, Vt, Rt, Ct, cb if dropout else None)
+    if centroids is None:
+        with torch.enable_grad():
+            cen_tabs = centroid_tables(y2, d2, H, W, C, m.use_pos)
+        xbar, lse = stats(m, k, D, xc, *cen_tabs)
+        xbar.requires_grad_(True)                  # first order: a leaf of its own; under create_graph already connected
+    with torch.enable_grad():
+        cen = centroids.detach() if centroids is not None else xbar @ _e(d1["wv2"]) + d1["bv2"]
+        Kp, Vt, Rt, Ct, cb = folded_tables(y1, d1, H=H, W=W, C=C, integration=m.integration, use_pos=m.use_pos, centroids=cen,
+                                           img2ltnt=m.img2ltnt)
+    dX, *grads = stage_t(m, k, D, dropout, xc, g_out, Kp, Vt, Rt, Ct, cb if dropout else None)
     outs = [Kp, Vt, Rt, Ct] + ([cb] if dropout else [])
     if g_cen is not None:
-        outs, grads = outs + [cen], grads + [g_cen]
-    g1 = list(torch.autograd.grad(outs, [y1, *p1, xbar], grads, allow_unused=True, create_graph=True))
-    dxbar = g1.pop()
-    r = (dxbar * xbar).sum(dim=2)
-    dX, *g_tabs = _CentroidBackward.apply(m, k, D, xc, *cen_tabs, lse, dxbar, r, dX)
-    g2 = torch.autograd.grad(list(cen_tabs), [y2, *p2], g_tabs, allow_unused=True, create_graph=True)
-    g = _sum_grads(g1, g2)
-    i = 1 + names.index("bk2")         # constant over the tokens, bk2 cancels in pass A's softmax: its gradient is exactly 0
-    g[i] = torch.zeros_like(params[i - 1])
+        outs, grads = outs + [cen], grads + [g_cen.contiguous()]
+    leaves = [y1, *p1] + ([xbar] if centroids is None else [])
+    g = list(torch.autograd.grad(outs, leaves, grads, allow_unused=True, create_graph=create_graph))
+    if centroids is None:
+        dxbar = g.pop()
+        r = (dxbar * xbar).sum(dim=2)              # [B, k]
+        dX, *g_tabs = pass_a_backward(m, k, D, xc, *cen_tabs, lse, dxbar, r, dX)
+        g = _sum_grads(g, torch.autograd.grad(list(cen_tabs), [y2, *p2], g_tabs, allow_unused=True, create_graph=create_graph))
+        i = 1 + names.index("bk2")     # constant over the tokens, bk2 cancels in pass A's softmax: its gradient is exactly 0
+        g[i] = torch.zeros_like(params[i - 1])
     return (dX, *g)
+
+
+def _composite_backward(m, names, x, y, params, g_out, dropout=None, centroids=None, g_cen=None):
+    """Autograd through ``composite_forward`` recomputed from leaves of the saved tensors (the layers of this route have no
+    attention dropout and no centroid cotangent)."""
+    create_graph = torch.is_grad_enabled()
+    with torch.enable_grad():
+        xs, ys, ps = _leaf(x, create_graph), _leaf(y, create_graph), [_leaf(p, create_graph) for p in params]
+        out, _ = composite_forward(xs, ys, dict(zip(names, ps)), integration=m.integration, norm=m.norm, duplex=m.duplex,
+                                   use_pos=m.use_pos, centroids=centroids, kmeans_iters=m.kmeans_iters, img2ltnt=m.img2ltnt,
+                                   num_heads=m.num_heads)
+    return torch.autograd.grad(out, [xs, ys, *ps], g_out, allow_unused=True, create_graph=create_graph)
 
 
 def _differentiable_twice(backward):
@@ -425,26 +372,23 @@ def _zeros_if_none(g, like):
 class _StageTBackward(torch.autograd.Function):
     """The stage-T backward with its token reductions, (X, dOut, Kp, Vt, Rt, Ct) -> (dX, dKp, dVt, dRt, dCt); with attention
     dropout (the forward's mask, regenerated) cb is one more table and dcb = sum_tokens (1 - sum q) dCtl one more output.
-    Forward: gf_attn_simplex_bwd_ex and the reductions.  Backward: gf_attn_simplex_bwd_vjp_ex (without dropout its att_dp = 0 form,
+    Forward: ``_stage_t_backward``.  Backward: gf_attn_simplex_bwd_vjp_ex (without dropout its att_dp = 0 form,
     gf_attn_simplex_bwd_vjp) and the reductions of its per-token cotangents, Kp: Sg^T X + dS^T U, Vt: Ctlg^T P + dCtl^T dPg,
     Rt / Ct: sums of Sg, cb: (1 - sum P) Ctlg - (sum dPg) dCtl."""
 
     @staticmethod
     def forward(ctx, m, k, D, dropout, x, g_out, Kp, Vt, Rt, Ct, cb):
         gc = g_out.contiguous()
-        dX, _, grads = _stage_t_backward(m, x, k, D, gc, (Kp, Vt, Rt, Ct, cb), dropout)
         ctx.m, ctx.k, ctx.D, ctx.dropout = m, k, D, dropout or {}
         ctx.save_for_backward(x, gc, Kp, Vt, Rt, Ct, cb)
-        return (dX, *grads)
+        return _stage_t_backward(m, k, D, dropout, x, gc, Kp, Vt, Rt, Ct, cb)
 
     @staticmethod
     @_differentiable_twice
     @_fp32_matmul()
     def backward(ctx, gdX, gKp, gVt, gRt, gCt, *gcb):
-        import ctypes
-        from . import _lib
         x, go, Kp, Vt, Rt, Ct, cb = ctx.saved_tensors
-        m, dpo = ctx.m, ctx.dropout
+        dpo = ctx.dropout
         B, H, W, C = x.shape
         n, KP, Cout = H * W, Kp.shape[1], Vt.shape[1]
         U = _zeros_if_none(gdX, x)
@@ -452,18 +396,12 @@ class _StageTBackward(torch.autograd.Function):
         Xg, dOg = torch.empty_like(x), torch.empty_like(x)
         Sg, dPg, dS, P = (torch.empty((B, n, KP), dtype=torch.float32, device=x.device) for _ in range(4))
         Ctlg, dCtl = (torch.empty((B, n, Cout), dtype=torch.float32, device=x.device) for _ in range(2))
-        desc = _lib.make_desc(B, H, W, C, ctx.k, ctx.D, heads=1, norm=m.norm, integration=m.integration,
-                              pos_dim=m.pos_dim if m.use_pos else 0, duplex=False, flags=0)
-        ptrs = [t.data_ptr() for t in (x, go, Kp, Vt, Rt, Ct, U, *cots, Xg, dOg, Sg, dPg, Ctlg, dS, P, dCtl)]
-        stream = ctypes.c_void_p(torch.cuda.current_stream(x.device).cuda_stream)
-        with torch.cuda.device(x.device):
-            if dpo:                              # the mask of the forward, regenerated from the same device state
-                cbg = _zeros_if_none(gcb[0], cb)
-                _lib.check(_lib.load().gf_attn_simplex_bwd_vjp_ex(
-                    ctypes.byref(desc), *ptrs, ctypes.c_float(dpo["att_dp"]), int(dpo.get("dp_salt", 0)), dpo["dp_state"].data_ptr(),
-                    cb.data_ptr(), cbg.data_ptr(), stream), "gf_attn_simplex_bwd_vjp_ex")
-            else:                                # the same kernel: the dropout-free entry is _ex at att_dp = 0
-                _lib.check(_lib.load().gf_attn_simplex_bwd_vjp(ctypes.byref(desc), *ptrs, stream), "gf_attn_simplex_bwd_vjp")
+        if dpo:                                  # the mask of the forward, regenerated from the same device state
+            name, dp_args = "gf_attn_simplex_bwd_vjp_ex", (*_dropout_args(dpo), cb, _zeros_if_none(gcb[0], cb))
+        else:                                    # the same kernel: the dropout-free entry is _ex at att_dp = 0
+            name, dp_args = "gf_attn_simplex_bwd_vjp", ()
+        _launch(name, _desc(ctx.m, x, ctx.k, ctx.D, duplex=0), x, go, Kp, Vt, Rt, Ct, U, *cots, Xg, dOg, Sg, dPg, Ctlg, dS, P, dCtl,
+                *dp_args)
         X2, U2 = x.reshape(B, n, C), U.reshape(B, n, C)
         gKp_ = torch.bmm(Sg.transpose(1, 2), X2) + torch.bmm(dS.transpose(1, 2), U2)
         gVt_ = torch.bmm(Ctlg.transpose(1, 2), P) + torch.bmm(dCtl.transpose(1, 2), dPg)
@@ -475,12 +413,12 @@ class _StageTBackward(torch.autograd.Function):
 
 
 class _CentroidStats(torch.autograd.Function):
-    """Pass A's statistics, (X, M, Rt2, Ct2) -> (Xbar, lse) (gf_attn_centroid_stats).  Backward: with cotangents dXbar and lseg,
-    d lse_j / d s[t,j] = A[t,j], so it is gf_attn_centroid_bwd with r = dXbar . Xbar - lseg and dX starting from zero."""
+    """Pass A's statistics, (X, M, Rt2, Ct2) -> (Xbar, lse) (``_centroid_stats``).  Backward: with cotangents dXbar and lseg,
+    d lse_j / d s[t,j] = A[t,j], so it is ``_centroid_backward`` with r = dXbar . Xbar - lseg and dX starting from zero."""
 
     @staticmethod
     def forward(ctx, m, k, D, x, Mt, Rt2, Ct2):
-        xbar, lse = _centroid_stats(m, x, k, D, Mt, Rt2, Ct2)
+        xbar, lse = _centroid_stats(m, k, D, x, Mt, Rt2, Ct2)
         ctx.m, ctx.k, ctx.D = m, k, D
         ctx.save_for_backward(x, Mt, Rt2, Ct2, xbar, lse)
         return xbar, lse
@@ -490,39 +428,29 @@ class _CentroidStats(torch.autograd.Function):
     @_fp32_matmul()
     def backward(ctx, gxbar, glse):
         x, Mt, Rt2, Ct2, xbar, lse = ctx.saved_tensors
-        B, H, W, C = x.shape
         gxbar = _zeros_if_none(gxbar, xbar)
         r = (gxbar * xbar).sum(dim=2)
         if glse is not None:
             r = r - glse[:, :ctx.k]
-        dX = torch.zeros_like(x)
-        dS = _centroid_bwd(ctx.m, x, ctx.k, ctx.D, Mt, Rt2, Ct2, lse, gxbar, r.contiguous(), dX)
-        dS4 = dS.reshape(B, H, W, dS.shape[2])
-        return None, None, None, dX, torch.bmm(dS.transpose(1, 2), x.reshape(B, H * W, C)), dS4.sum(dim=2), dS4.sum(dim=1)
+        return None, None, None, *_centroid_backward(ctx.m, ctx.k, ctx.D, x, Mt, Rt2, Ct2, lse, gxbar, r, torch.zeros_like(x))
 
 
 class _CentroidBackward(torch.autograd.Function):
     """The pass-A backward with its token reductions, (X, M, Rt2, Ct2, lse, dXbar, r, dX_in) -> (dX_out, dM, dRt2, dCt2).
-    Forward: gf_attn_centroid_bwd into a copy of dX_in (never into a tensor autograd tracks) and the reductions.  Backward:
+    Forward: ``_centroid_backward`` into a copy of dX_in (never into a tensor autograd tracks).  Backward:
     gf_attn_centroid_bwd_vjp and the reductions dXbar: A^T U + Gg^T X, M: Sg^T X + dS^T U, r: -sum_t Gg, lse: -sum_t Sg."""
 
     @staticmethod
     def forward(ctx, m, k, D, x, Mt, Rt2, Ct2, lse, dxbar, r, dX_in):
-        B, H, W, C = x.shape
         dxbar, r = dxbar.contiguous(), r.contiguous()
-        dX = dX_in.contiguous().clone()
-        dS = _centroid_bwd(m, x, k, D, Mt, Rt2, Ct2, lse, dxbar, r, dX)
         ctx.m, ctx.k, ctx.D = m, k, D
         ctx.save_for_backward(x, Mt, Rt2, Ct2, lse, dxbar, r)
-        dS4 = dS.reshape(B, H, W, dS.shape[2])
-        return dX, torch.bmm(dS.transpose(1, 2), x.reshape(B, H * W, C)), dS4.sum(dim=2), dS4.sum(dim=1)
+        return _centroid_backward(m, k, D, x, Mt, Rt2, Ct2, lse, dxbar, r, dX_in.contiguous().clone())
 
     @staticmethod
     @_differentiable_twice
     @_fp32_matmul()
     def backward(ctx, gdX, gM, gRt2, gCt2):
-        import ctypes
-        from . import _lib
         x, Mt, Rt2, Ct2, lse, dxbar, r = ctx.saved_tensors
         B, H, W, C = x.shape
         n, KP, k = H * W, Mt.shape[1], ctx.k
@@ -530,11 +458,8 @@ class _CentroidBackward(torch.autograd.Function):
         cots = [_zeros_if_none(g, t) for g, t in ((gM, Mt), (gRt2, Rt2), (gCt2, Ct2))]
         Xg = torch.empty_like(x)
         Sg, Gg, A, dS = (torch.empty((B, n, KP), dtype=torch.float32, device=x.device) for _ in range(4))
-        desc = _duplex_desc(ctx.m, x, k, ctx.D)
-        with torch.cuda.device(x.device):
-            _lib.check(_lib.load().gf_attn_centroid_bwd_vjp(
-                ctypes.byref(desc), *(t.data_ptr() for t in (x, Mt, Rt2, Ct2, lse, dxbar, r, U, *cots, Xg, Sg, Gg, A, dS)),
-                ctypes.c_void_p(torch.cuda.current_stream(x.device).cuda_stream)), "gf_attn_centroid_bwd_vjp")
+        _launch("gf_attn_centroid_bwd_vjp", _desc(ctx.m, x, k, ctx.D, duplex=1), x, Mt, Rt2, Ct2, lse, dxbar, r, U, *cots, Xg, Sg, Gg,
+                A, dS)
         X2, U2 = x.reshape(B, n, C), U.reshape(B, n, C)
         gM_ = torch.bmm(Sg.transpose(1, 2), X2) + torch.bmm(dS.transpose(1, 2), U2)
         gxbar = (torch.bmm(A.transpose(1, 2), U2) + torch.bmm(Gg.transpose(1, 2), X2))[:, :k]
@@ -542,79 +467,73 @@ class _CentroidBackward(torch.autograd.Function):
         return (None, None, None, Xg, gM_, Sg4.sum(dim=2), Sg4.sum(dim=1), -Sg.sum(dim=1), gxbar, -Gg.sum(dim=1)[:, :k], U)
 
 
-def _duplex_desc(m, x, k, D):
-    from . import _lib
+def _desc(m, x, k, D, duplex):
+    """The descriptor of a backward entry for layer m on x [B,H,W,C]: one head, no flags; duplex = 0 for stage T (a duplex
+    layer's too, its keys are folded from the centroids), 1 for pass A."""
     B, H, W, C = x.shape
-    return _lib.make_desc(B, H, W, C, k, D, heads=1, norm=m.norm, integration=m.integration,
-                          pos_dim=m.pos_dim if m.use_pos else 0, duplex=1, flags=0)
+    return _lib.make_desc(B, H, W, C, k, D, heads=1, norm=m.norm, integration=m.integration, pos_dim=m.pos_dim if m.use_pos else 0,
+                          duplex=duplex, flags=0)
 
 
-def _centroid_stats(m, xc, k, D, Mt, Rt2, Ct2):
+def _launch(name, desc, *args):
+    """The library entry ``name`` on (desc, *args, the current stream) of the device of args[0], the X every backward entry
+    takes first.  Tensors go by data pointer, None as NULL."""
+    dev = args[0].device
+    ptrs = [a.data_ptr() if isinstance(a, torch.Tensor) else a for a in args]
+    with torch.cuda.device(dev):
+        _lib.check(getattr(_lib.load(), name)(ctypes.byref(desc), *ptrs, ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)),
+                   name)
+
+
+def _dropout_args(dropout):
+    """(att_dp, dp_salt, dp_state) of the forward's dropout post-op, with which a backward entry regenerates its mask: att_dp = 0
+    and a NULL state without dropout."""
+    dpo = dropout or {}
+    return ctypes.c_float(dpo.get("att_dp", 0.0)), int(dpo.get("dp_salt", 0)), dpo.get("dp_state")
+
+
+def _centroid_stats(m, k, D, x, Mt, Rt2, Ct2):
     """gf_attn_centroid_stats: pass A recomputed in fp32 -> (Xbar [B,k,C], lse [B,KP])."""
-    import ctypes
-    from . import _lib
-    B, _, _, C = xc.shape
-    desc = _duplex_desc(m, xc, k, D)
-    xbar = torch.empty((B, k, C), dtype=torch.float32, device=xc.device)
-    lse = torch.empty((B, Mt.shape[1]), dtype=torch.float32, device=xc.device)
-    part = torch.empty(_lib.workspace_bytes(desc), dtype=torch.uint8, device=xc.device)       # split-n partials
-    with torch.cuda.device(xc.device):
-        _lib.check(_lib.load().gf_attn_centroid_stats(ctypes.byref(desc), xc.data_ptr(), Mt.data_ptr(), Rt2.data_ptr(), Ct2.data_ptr(),
-                                                      xbar.data_ptr(), lse.data_ptr(), part.data_ptr(),
-                                                      ctypes.c_void_p(torch.cuda.current_stream(xc.device).cuda_stream)),
-                   "gf_attn_centroid_stats")
+    B, _, _, C = x.shape
+    desc = _desc(m, x, k, D, duplex=1)
+    xbar = torch.empty((B, k, C), dtype=torch.float32, device=x.device)
+    lse = torch.empty((B, Mt.shape[1]), dtype=torch.float32, device=x.device)
+    part = torch.empty(_lib.workspace_bytes(desc), dtype=torch.uint8, device=x.device)       # split-n partials
+    _launch("gf_attn_centroid_stats", desc, x, Mt, Rt2, Ct2, xbar, lse, part)
     return xbar, lse
 
 
-def _centroid_bwd(m, xc, k, D, Mt, Rt2, Ct2, lse, dxbar, r, dX):
-    """gf_attn_centroid_bwd: adds the pass-A part of the activation gradient into dX; returns dS [B,n,KP] of the pass-A logits."""
-    import ctypes
-    from . import _lib
-    B, H, W, C = xc.shape
-    desc = _duplex_desc(m, xc, k, D)
-    dS = torch.empty((B, H * W, Mt.shape[1]), dtype=torch.float32, device=xc.device)
-    with torch.cuda.device(xc.device):
-        _lib.check(_lib.load().gf_attn_centroid_bwd(ctypes.byref(desc), xc.data_ptr(), Mt.data_ptr(), Rt2.data_ptr(), Ct2.data_ptr(),
-                                                    lse.data_ptr(), dxbar.data_ptr(), r.data_ptr(), dX.data_ptr(), dS.data_ptr(),
-                                                    ctypes.c_void_p(torch.cuda.current_stream(xc.device).cuda_stream)),
-                   "gf_attn_centroid_bwd")
-    return dS
+def _centroid_backward(m, k, D, x, Mt, Rt2, Ct2, lse, dxbar, r, dX):
+    """gf_attn_centroid_bwd, which adds the pass-A part of the activation gradient into dX in place and gives dS [B,n,KP] of the
+    pass-A logits, and the reductions of dS over the tokens: (dX, dM = dS^T X, dRt2, dCt2)."""
+    B, H, W, C = x.shape
+    KP = Mt.shape[1]
+    dS = torch.empty((B, H * W, KP), dtype=torch.float32, device=x.device)
+    _launch("gf_attn_centroid_bwd", _desc(m, x, k, D, duplex=1), x, Mt, Rt2, Ct2, lse, dxbar.contiguous(), r.contiguous(), dX, dS)
+    dS4 = dS.reshape(B, H, W, KP)
+    return dX, torch.bmm(dS.transpose(1, 2), x.reshape(B, H * W, C)), dS4.sum(dim=2), dS4.sum(dim=1)
 
 
-def _stage_t_backward(m, x, k, D, g_out, tables, dropout):
-    """gf_attn_simplex_bwd_ex and the reductions over the tokens: returns dX and the (tables, gradients) pairs autograd takes
-    back through stages W and I."""
-    import ctypes
-    from . import _lib
+def _stage_t_backward(m, k, D, dropout, x, g_out, Kp, Vt, Rt, Ct, cb):
+    """gf_attn_simplex_bwd_ex and the reductions over the tokens: (dX, dKp, dVt, dRt, dCt), and dcb under dropout, the gradients
+    autograd takes back through stages W and I.  cb: the unscaled control-signal constants, None without dropout."""
     B, H, W, C = x.shape
     n = H * W
-    Kp, Vt, Rt, Ct, cb = tables
     KP, Cout = Kp.shape[1], Vt.shape[1]
     xc, gc = x.detach().contiguous(), g_out.detach().contiguous()
     dX = torch.empty_like(xc)
     dS = torch.empty((B, n, KP), dtype=torch.float32, device=x.device)
     P = torch.empty_like(dS)
     dCtl = torch.empty((B, n, Cout), dtype=torch.float32, device=x.device)
-    desc = _lib.make_desc(B, H, W, C, k, D, heads=1, norm=m.norm, integration=m.integration,
-                          pos_dim=m.pos_dim if m.use_pos else 0, duplex=False, flags=0)
-    with torch.cuda.device(x.device):
-        dpo = dropout or {}
-        _lib.check(_lib.load().gf_attn_simplex_bwd_ex(ctypes.byref(desc), xc.data_ptr(), gc.data_ptr(), Kp.data_ptr(), Vt.data_ptr(),
-                                                      Rt.data_ptr(), Ct.data_ptr(), dX.data_ptr(), dS.data_ptr(), P.data_ptr(),
-                                                      dCtl.data_ptr(), ctypes.c_float(dpo.get("att_dp", 0.0)), int(dpo.get("dp_salt", 0)),
-                                                      dpo["dp_state"].data_ptr() if dpo else None, cb.detach().data_ptr() if dpo else None,
-                                                      ctypes.c_void_p(torch.cuda.current_stream(x.device).cuda_stream)),
-                   "gf_attn_simplex_bwd_ex")
+    _launch("gf_attn_simplex_bwd_ex", _desc(m, x, k, D, duplex=0), xc, gc, Kp, Vt, Rt, Ct, dX, dS, P, dCtl, *_dropout_args(dropout), cb)
     # reductions over the tokens: plain batched GEMMs / sums
     dKp = torch.bmm(dS.transpose(1, 2), xc.reshape(B, n, C))             # [B, KP, C]
     dVt = torch.bmm(dCtl.transpose(1, 2), P)                             # [B, Cout, KP]
     dS4 = dS.reshape(B, H, W, KP)
-    dRt, dCt = dS4.sum(dim=2), dS4.sum(dim=1)
-    outs, grads = [Kp, Vt, Rt, Ct], [dKp, dVt, dRt, dCt]
-    if dpo:                                      # ctl = sum_j q_j (Vt_j - cb) + cb: the constants' own gradient
-        outs.append(cb)
+    grads = [dKp, dVt, dS4.sum(dim=2), dS4.sum(dim=1)]
+    if dropout:                                  # ctl = sum_j q_j (Vt_j - cb) + cb: the constants' own gradient
         grads.append((dCtl * (1.0 - P.sum(dim=2, keepdim=True))).sum(dim=(0, 1)))
-    return dX, outs, grads
+    return (dX, *grads)
 
 
 def bipartite_attention_autograd(module, x, y, centroids, return_att):

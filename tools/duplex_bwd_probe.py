@@ -76,9 +76,9 @@ def main():
             return torch.autograd.grad(out, [x, y, *params], g, allow_unused=True)
 
         def kernel():
-            with torch.no_grad():
+            with torch.no_grad():                  # grad mode off: the first-order backward, as autograd runs it
                 attn(x, y)
-            return ag._duplex_kernel_backward(attn, names, x, y, params, g)
+                return ag._duplex_kernel_backward(attn, names, x, y, params, g)
 
         def kernel_dp():
             out, _, _ = attn_dp(x, y)
