@@ -8,8 +8,8 @@
 * ops.augment's first and second derivatives against fp64 autograd of the definition.
 * Determinism and CUDA-graph replay, bit for bit; a captured sampler draws new parameters on every replay.
 * Training with Discriminator(transformer=True), with and without labels: step_graphed against the eager step from the same state
-  and the same RNG state, at lr = 0 (the p trajectory and the D loss bit for bit, R1 to 1e-3), and the R1 penalty and its
-  gradient through the augmentation against fp64 autograd of the oracle discriminator.
+  and the same RNG state, at lr = 0 (the p trajectory, the D and G losses and the last step's gradients bit for bit, R1 to 1e-3),
+  and the R1 penalty and its gradient through the augmentation against fp64 autograd of the oracle discriminator.
 """
 import copy
 import math
@@ -21,6 +21,7 @@ import torch
 from tests import conditional_ref as cref
 from tests.guards import Guarded, assert_exact
 from tests.test_gpu_ops_exact import F64, _call, _stream, ints
+from tests.test_gpu_step_determinism import assert_same_grads
 
 pytestmark = pytest.mark.gpu
 
@@ -193,9 +194,9 @@ def test_augmented_step_graphed_matches_eager(gf, cuda_dev, c_dim):
     """step_graphed with "bc" augmentation and ADA against the eager step.  After the graphed trainer's first call (warm-up, capture,
     replay) its weights, Adam states and ADA state go to an eager trainer; then both take three steps (the second with R1), each
     from the same CUDA RNG state, so both draw the same augmentation parameters.  lr = 0 keeps the weights of both trainers equal.
-    p moves every step (interval 1); its trajectory and the D phase's loss (reals and fakes, both augmented) must be the same bits,
-    and R1 must agree to 1e-3.  The G phase's loss is printed, not held: it has differed by up to 1.1 % between the two (DESIGN
-    4.11, an open finding).  cuDNN is pinned to its deterministic algorithms, as in the "bgc" and "bgcfn" versions of this test:
+    p moves every step (interval 1); its trajectory, the D phase's loss (reals and fakes, both augmented) and the G phase's loss
+    must be the same bits, and R1 must agree to 1e-3; after the last step every G and D gradient must be the same bits too.  cuDNN
+    is pinned to its deterministic algorithms, as in the "bgc" and "bgcfn" versions of this test:
     with its default algorithms the graph and the eager step may run different convolutions, and the D loss of the R1 step has
     differed in its last bit (6.027669906616211 against 6.0276689529418945 on an H100)."""
     prev = torch.backends.cudnn.deterministic, torch.backends.cudnn.benchmark
@@ -233,9 +234,11 @@ def _graphed_against_eager(gf, cuda_dev, c_dim):
         assert sg.augment_p == se.augment_p, i
         assert (sg.r1 > 0) == (se.r1 > 0) == (i % 2 == 1)
         assert sg.loss_d == se.loss_d, i
+        assert sg.loss_g == se.loss_g, i
         assert abs(se.r1 - sg.r1) <= 1e-3 * max(1.0, abs(se.r1)), i
         ps.append(se.augment_p)
     assert len(set(ps)) > 1 or ps[0] in (0.0, 1.0)
+    assert_same_grads(tg, te, "graphed against eager, last step")
 
 
 def test_r1_through_the_augmentation_against_fp64(gf, cuda_dev):

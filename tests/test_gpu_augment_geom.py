@@ -6,7 +6,8 @@
   images outside the parameter domain (NaN for that image, its neighbours untouched); batches that wrap the grid.
 * The adjoint identity in fp64 of the fp32 results; ops.augment(..., frac=...)'s first and second derivatives against fp64 autograd.
 * Determinism and CUDA-graph replay, bit for bit; a captured sampler draws new maps on every replay and p = 0 replays the identity.
-* R1 through "bgc" against fp64 autograd of the oracle discriminator; step_graphed with "bgc" and ADA against the eager step.
+* R1 through "bgc" against fp64 autograd of the oracle discriminator; step_graphed with "bgc" and ADA against the eager step (the
+  losses and the last step's gradients bit for bit).
 """
 import copy
 from importlib import import_module
@@ -17,6 +18,7 @@ import torch
 from tests import conditional_ref as cref
 from tests.guards import Guarded, assert_exact
 from tests.test_gpu_augment import _batch, _gan
+from tests.test_gpu_step_determinism import assert_same_grads
 from tests.test_gpu_ops_exact import F64, _call, _stream
 
 pytestmark = pytest.mark.gpu
@@ -289,7 +291,8 @@ def test_r1_through_bgc_against_fp64(gf, cuda_dev):
 
 
 def test_bgc_step_graphed_matches_eager(gf, cuda_dev):
-    """As test_augmented_step_graphed_matches_eager, with "bgc": the p trajectory and the D loss bit for bit, R1 to 1e-3.  cuDNN is
+    """As test_augmented_step_graphed_matches_eager, with "bgc": the p trajectory, the D and G losses and the last step's gradients
+    bit for bit, R1 to 1e-3.  cuDNN is
     pinned to its deterministic algorithms, whose choice does not depend on timing: with autotuned algorithms the D loss of an R1 step
     has differed in its last bits between the two (DESIGN 4.12)."""
     prev = torch.backends.cudnn.deterministic, torch.backends.cudnn.benchmark
@@ -325,4 +328,6 @@ def _graphed_against_eager(gf, cuda_dev):
         assert sg.augment_p == se.augment_p, i
         assert (sg.r1 > 0) == (se.r1 > 0) == (i % 2 == 1)
         assert sg.loss_d == se.loss_d, i
+        assert sg.loss_g == se.loss_g, i
         assert abs(se.r1 - sg.r1) <= 1e-3 * max(1.0, abs(se.r1)), i
+    assert_same_grads(tg, te, "graphed against eager, last step")
