@@ -69,12 +69,13 @@ def generator_forward(sd, z, c, *, resolution: int, components_num: int, latent_
 
 
 def discriminator_forward(sd, img, c: Optional[torch.Tensor], *, mbstd_group: int = 4, integration: str = "mul",
-                          norm: Optional[str] = "layer", use_pos: bool = True) -> torch.Tensor:
-    """Logits [B] of the discriminator whose fc1 [c_dim, C] is projected onto c [B, c_dim] (None: the unconditional head).
+                          norm: Optional[str] = "layer", use_pos: bool = True, dtype=torch.float64) -> torch.Tensor:
+    """Logits [B] of the discriminator whose fc1 [c_dim, C] is projected onto c [B, c_dim] (None: the unconditional head), computed
+    in ``dtype`` (oracle.discriminator_forward's: fp64 unless a test restates it in fp32).
 
     The projection is linear in fc1's rows: logit_b = sum_j c_bj (fc1_j . h_b + b_j).  So this runs oracle.discriminator_forward
     once per class, with fc1 cut to that class's row, and sums the per-class logits weighted by c: the whole trunk is the oracle's."""
-    kw = dict(mbstd_group=mbstd_group, integration=integration, norm=norm, use_pos=use_pos)
+    kw = dict(mbstd_group=mbstd_group, integration=integration, norm=norm, use_pos=use_pos, dtype=dtype)
     if c is None:
         return od.discriminator_forward(sd, img, **kw)
     logits = []

@@ -5,11 +5,11 @@
   algorithms.  The losses, R1, p and every parameter gradient of G and D must be the same bits on both.  ``zero_grad(set_to_none)``
   runs at the start of each phase, so after a step D holds the D phase's gradients and G the G phase's.  The configurations:
   plain D without augmentation (the control), ``Discriminator(transformer=True)`` with no augmentation, "bc", "bgc" and "bgcfn",
-  "bc" with labels and "bc" with ``r1_kernels``.
-* The G phase against fp64: one eager step with the augmentation samplers recorded, with "bc" and "bgc"; the G loss and the
-  gradients of a spread of G parameters are rebuilt in fp64 on the CPU from the state dicts (tests/conditional_ref.py's generator and discriminator,
-  ops.augment_ref with the G phase's draws).  The gradients flow back through D's duplex kernel backward (dX), the augmentation's
-  adjoint and G's training path.
+  "bc" with labels, "bc" with ``r1_kernels`` and "bc" with img2img in both networks.
+* The G phase against fp64: one eager step with the augmentation samplers recorded (tests/step_phase_ref.py), with "bc", "bgc",
+  "bgcfn" and "bc" with labels; the G loss and the gradients of a spread of G parameters are rebuilt in fp64 on the CPU from the
+  state dicts (tests/conditional_ref.py's generator and discriminator, ops.augment_ref and ops.augment_filter_ref with the G phase's
+  draws).  The gradients flow back through D's duplex kernel backward (dX), the augmentation's adjoints and G's training path.
 """
 import contextlib
 import copy
@@ -19,13 +19,13 @@ import pytest
 import torch
 
 from tests import conditional_ref as cref
+from tests import step_phase_ref as step_ref
 
 pytestmark = pytest.mark.gpu
 
 TRAIN = "gansformer-reproducibility-challenge_b200.training"
-OPS = "gansformer-reproducibility-challenge_b200.ops"
 
-# (Discriminator options, TrainConfig.augment, c_dim)
+# (Discriminator options, TrainConfig.augment, c_dim); img2img, when a case has it, goes to both networks
 RERUN_CASES = {
     "plain-d": (dict(transformer=False), "", 0),
     "attention-d": (dict(transformer=True), "", 0),
@@ -34,6 +34,7 @@ RERUN_CASES = {
     "bgcfn": (dict(transformer=True), "bgcfn", 0),
     "bc-labels": (dict(transformer=True), "bc", 5),
     "bc-r1-kernels": (dict(transformer=True, r1_kernels=True), "bc", 0),
+    "img2img-bc": (dict(transformer=True, img2img=16), "bc", 0),
 }
 
 # The G phase against fp64: relative errors (2-norm of the difference over the 2-norm of the fp64 value).  Measured on an H100 80GB
@@ -41,6 +42,18 @@ RERUN_CASES = {
 # to 3.4e-4) and 3.8e-5 ("bgc").  Frozen at about 1.6x the worst.
 TOL_LOSS_G = 5e-6
 TOL_GRAD = 6e-4
+# (TrainConfig.augment, c_dim, CUDA seed of the step, bound on the loss, bound on the gradients).  Seed 7's draws put D where fp32
+# itself keeps few digits under "bgcfn" (an fp32 restatement of the definition 2.8e-3 off fp64 on the gradients) and with labels
+# (7.5e-2).  Those two cases take a seed whose draws the restatement resolves, found by a sweep of seeds 1-12 on the H100 (DESIGN
+# section 4.11), with bounds frozen at about 2x the larger of the kernels' and the restatement's error there: "bgcfn" at seed 5,
+# kernels 1.7e-6 (loss) and 3.7e-5 (gradients), restatement 6.6e-7 and 1.3e-5; labels at seed 8, kernels 5.9e-7 and 7.6e-5,
+# restatement 2.8e-8 and 1.4e-4.
+G_PHASE_CASES = {
+    "bc": ("bc", 0, 7, TOL_LOSS_G, TOL_GRAD),
+    "bgc": ("bgc", 0, 7, TOL_LOSS_G, TOL_GRAD),
+    "bgcfn": ("bgcfn", 0, 5, 3.4e-6, 7.5e-5),
+    "bc-labels": ("bc", 5, 8, 1.2e-6, 3e-4),
+}
 # The untrained generator's images (std 3.2, up to 16 in magnitude) put the attention discriminator where fp32 keeps no digit of
 # the G phase: an all-fp32 restatement of the reference is 5e-2 off fp64 on the loss and 8x off on the gradients (condition number
 # of the loss in the image about 1e5).  Scaling the tRGB weights by 0.3 brings the images to std 0.66, where that restatement agrees
@@ -62,11 +75,12 @@ def _deterministic_cudnn():
 
 
 def _gan(gf, dev, dkw, c_dim):
-    """The 64x64 pair of tests/test_gpu_augment.py (exact_fp32), with the discriminator's options dkw."""
+    """The 64x64 pair of tests/test_gpu_augment.py (exact_fp32), with the discriminator's options dkw (an img2img there is given to
+    the generator too)."""
     tr = import_module(TRAIN)
     torch.manual_seed(0)
     G = gf.Generator(resolution=64, components_num=8, latent_dim=32, fmap_base=2048, fmap_max=128, mapping_layers=4, exact_fp32=True,
-                     c_dim=c_dim).to(dev)
+                     c_dim=c_dim, img2img=dkw.get("img2img", 0)).to(dev)
     D = tr.Discriminator(64, fmap_base=2048, fmap_max=128, components_num=8, latent_dim=32, exact_fp32=True, c_dim=c_dim,
                          **dkw).to(dev)
     return tr, G, D
@@ -143,43 +157,54 @@ def test_step_reruns_bit_for_bit(gf, cuda_dev, case):
             assert_same_grads(ta, tb, f"{case} step {i}")
 
 
-@pytest.mark.parametrize("augment", ["bc", "bgc"])
-def test_g_phase_against_fp64(gf, cuda_dev, augment, monkeypatch):
+def g_phase_errors(gf, dev, augment, c_dim, seed, monkeypatch):
     """One eager step with Discriminator(transformer=True) at lr = 0, so that D after its update is still D0, and the generator's
-    tRGB weights scaled by TORGB_SCALE.  The samplers record their draws; the G phase's are the last.  The G loss and the gradients
-    of G_GRADS against fp64 autograd of the reference."""
-    ops = import_module(OPS)
-    tr, G, D = _gan(gf, cuda_dev, dict(transformer=True), 0)
+    tRGB weights scaled by TORGB_SCALE, from CUDA seed ``seed``.  The samplers record their draws (tests/step_phase_ref.StepRecorder);
+    the G phase's are the last.  Returns the relative errors of the G loss and of the gradients of G_GRADS against fp64 autograd
+    of the reference (labels gen_c on both networks), and those of the same definition restated in fp32 on the same draws."""
+    tr, G, D = _gan(gf, dev, dict(transformer=True), c_dim)
     with torch.no_grad():
         for t in G.synthesis.torgbs:
             t.weight.mul_(TORGB_SCALE)
-    draws = {"sample_augment": [], "sample_augment_frac": []}
-    for name, seen in draws.items():
-        fn = getattr(tr, name)
-        monkeypatch.setattr(tr, name, lambda *a, _fn=fn, _seen=seen, **k: _seen.append(_fn(*a, **k)) or _seen[-1])
+    filtered = bool(set(tr.parse_augment(augment)) & set(tr.FILTER_OPS))
+    rec = step_ref.StepRecorder(tr, monkeypatch, filtered)
     trainer = tr.Trainer(G, D, tr.TrainConfig(lr=0.0, noise_mode="const", r1_gamma=0.0, augment=augment, augment_p=0.8))
-    z, reals, _, _ = _batch(cuda_dev)
+    z, reals, gen_c, real_c = _batch(dev, c_dim=c_dim)
     sd_g, sd_d = cref.cast(G.state_dict()), cref.cast(D.state_dict())
-    torch.cuda.manual_seed(7)
+    torch.cuda.manual_seed(seed)
     with _deterministic_cudnn():
-        st = trainer.step(z, reals)
-    assert len(draws["sample_augment"]) == 3                          # the D phase's reals and fakes, the G phase's fakes
-    geom, color = (t.cpu() for t in draws["sample_augment"][-1])
-    frac = draws["sample_augment_frac"][-1]
-    frac = None if frac is None else frac.cpu()
-    assert (frac is not None) == (augment == "bgc")
-    for n in G_GRADS:
-        sd_g[n].requires_grad_(True)
-    img = cref.generator_forward(sd_g, z.double().cpu(), None, resolution=64, components_num=8, latent_dim=32, mapping_layers=4)
-    loss64 = torch.nn.functional.softplus(-cref.discriminator_forward(sd_d, ops.augment_ref(img, geom, color.double(), frac), None)).mean()
-    grads64 = torch.autograd.grad(loss64, [sd_g[n] for n in G_GRADS])
+        st = trainer.step(z, reals, gen_c, real_c)
+    draw = rec.draws(0, 1)["fakes_g"]                                 # after the D phase's reals and fakes
+    assert (draw[2] is not None) == (augment != "bc") and (draw[3] is not None) == filtered
+    res = {}
+    for dt in (torch.float64, torch.float32):                          # fp64, and the same definition restated in fp32
+        sd = cref.cast(sd_g, dt)
+        for n in G_GRADS:
+            sd[n].requires_grad_(True)
+        c = None if gen_c is None else gen_c.to("cpu", dt)
+        img = cref.generator_forward(sd, z.to("cpu", dt), c, resolution=64, components_num=8, latent_dim=32, mapping_layers=4)
+        logits = cref.discriminator_forward(cref.cast(sd_d, dt), step_ref.augment64(img, draw), c, dtype=dt)
+        loss = torch.nn.functional.softplus(-logits).mean()
+        res[dt] = (loss.item(), torch.autograd.grad(loss, [sd[n] for n in G_GRADS]))
+    loss64, grads64 = res[torch.float64]
     params = dict(G.named_parameters())
-    e_loss = abs(st.loss_g - loss64.item()) / abs(loss64.item())
-    errs = {}
-    for n, want in zip(G_GRADS, grads64):
+    e_loss, r_loss = (abs(v - loss64) / abs(loss64) for v in (st.loss_g, res[torch.float32][0]))
+    errs, restated = {}, {}
+    for n, want, w32 in zip(G_GRADS, grads64, res[torch.float32][1]):
         assert want.norm() > 0, n
-        errs[n] = ((params[n].grad.double().cpu() - want).norm() / want.norm()).item()
-    print(f"[G phase {augment}] loss_g {st.loss_g:.8f} vs {loss64.item():.8f}: rel {e_loss:.2e}; gradients "
-          + " ".join(f"{n}={e:.2e}" for n, e in errs.items()))
-    assert e_loss < TOL_LOSS_G, e_loss
-    assert max(errs.values()) < TOL_GRAD, errs
+        errs[n], restated[n] = step_ref.rel(params[n].grad, want), step_ref.rel(w32, want)
+    print(f"[G phase {augment} c_dim={c_dim} seed={seed}] loss_g {st.loss_g:.8f} vs {loss64:.8f}: rel {e_loss:.2e} (fp32 "
+          f"restatement {r_loss:.2e}); gradients " + " ".join(f"{n}={e:.2e}" for n, e in errs.items())
+          + f"; max {max(errs.values()):.2e} (fp32 restatement {max(restated.values()):.2e})")
+    return e_loss, r_loss, errs, restated
+
+
+@pytest.mark.parametrize("case", list(G_PHASE_CASES))
+def test_g_phase_against_fp64(gf, cuda_dev, case, monkeypatch):
+    """The G loss and the gradients of G_GRADS against fp64 under frozen bounds, on draws that fp32 itself resolves: the fp32
+    restatement on the same draws must stay within the case's bounds too, so that the bounds measure the step and not the draw."""
+    augment, c_dim, seed, tol_loss, tol_grad = G_PHASE_CASES[case]
+    e_loss, r_loss, errs, restated = g_phase_errors(gf, cuda_dev, augment, c_dim, seed, monkeypatch)
+    assert r_loss < tol_loss and max(restated.values()) < tol_grad, (r_loss, restated)
+    assert e_loss < tol_loss, e_loss
+    assert max(errs.values()) < tol_grad, errs
