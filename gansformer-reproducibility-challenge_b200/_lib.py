@@ -36,7 +36,7 @@ EXPORTS = ("gf_attn_abi_version", "gf_last_error", "gf_attn_last_path", "gf_attn
 # include/gf_ops.h
 OPS_EXPORTS = ("gf_chan_scale_nhwc", "gf_blur_up_nhwc", "gf_upsample2x_nchw", "gf_bias_act_nhwc", "gf_demod_coef", "gf_torgb_nhwc", "gf_fir4_nhwc", "gf_blur_up_phases_nhwc", "gf_torgb_scale_nhwc", "gf_mapping_fwd", "gf_conv3x3_pack_weights", "gf_conv3x3_nhwc_tf32", "gf_demod_coef_batch", "gf_upconv3x3_blur_nhwc_tf32", "gf_mapping_fwd_cond", "gf_augment_nchw", "gf_augment_adjoint_nchw",
                "gf_augment_resample_nchw", "gf_augment_resample_adjoint_nchw", "gf_augment_filter_nchw", "gf_augment_filter_adjoint_nchw",
-               "gf_self_attn_fwd", "gf_self_attn_bwd")
+               "gf_self_attn_fwd", "gf_self_attn_bwd", "gf_self_attn_bwd_vjp")
 
 
 class GfAttnDesc(ctypes.Structure):
@@ -129,6 +129,7 @@ def load() -> ctypes.CDLL:
     lib.gf_augment_filter_adjoint_nchw.argtypes = [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]
     lib.gf_self_attn_fwd.argtypes = [c_void_p] * 5 + [c_int] * 4 + [ctypes.c_float, c_void_p]
     lib.gf_self_attn_bwd.argtypes = [c_void_p] * 13 + [c_int] * 4 + [ctypes.c_float, c_void_p]
+    lib.gf_self_attn_bwd_vjp.argtypes = [c_void_p] * 22 + [c_int] * 4 + [ctypes.c_float, c_void_p]
     for name in OPS_EXPORTS:
         getattr(lib, name).restype = c_int
     for name in EXPORTS:

@@ -16,6 +16,7 @@
 //             streams the query tiles (Q, dO, Q^T, dO^T, lse, Delta); dQ kernel, grid (n / 64, h, B): one warpgroup per 64-query
 //             tile streams the key tiles (K, V, K^T).  Each output is accumulated by one CTA in a fixed order: no atomics, the same
 //             bits on every call.
+//   double backward (gf_self_attn_bwd_vjp)  a row pass, a query-tile and a key-tile kernel, laid out as the backward (see below).
 // Operands are truncated to TF32 by the tensor core (P and dS are rounded to nearest first); accumulation is fp32.
 #include <limits.h>
 #include <math.h>
@@ -470,6 +471,472 @@ self_attn_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
 }
 
 // ------------------------------------------------------------------------------------------------------------------------------
+// double backward: the vector-Jacobian product of the backward (Q, K, V, dO) -> (dQ, dK, dV) with cotangents A of dQ, Bk of dK
+// and Cv of dV.  P is recomputed from lse as above, Delta is the backward's; with s = scale:
+//   dS = P o (dP - Delta),   GdS = s [A | Q] [K | Bk]^T,   r = rowsum(P o GdS),   u = rowsum(P o GdS o dP),   PC = P Cv
+//   GdP = P o (GdS - r),   GP = GdS o (dP - Delta) - r o dP + dO Cv^T,   t = u - 2 Delta r + dO . PC (= rowsum(P o GP)),
+//   GS = P o (GP - t);     gQ = s (dS Bk + GS K),   gK = s (dS^T A + GS^T Q),   gV = GdP^T dO,   gdO = GdP V + PC
+//   rows kernel, grid (n / 64, h, B): one warpgroup per 64-query tile streams K, V, Bk, Cv^T over every key and writes r, t and
+//               PC (into gdO);
+//   q kernel,    grid (n / 64, h, B): one warpgroup per 64-query tile streams K, V, Bk, Cv, K^T, Bk^T, V^T: gQ, and gdO += GdP V;
+//   kv kernel,   grid (n / 64, h, B): one warpgroup per 64-key tile streams Q, dO, A, Q^T, A^T, dO^T and lse, Delta, r, t of
+//               each query tile: gK, gV.
+// The q and kv kernels hold seven and six streamed tiles per stage: at d = 64 their ring has one slot (the shared memory of a
+// second is not there), at d = 32 two.
+// ------------------------------------------------------------------------------------------------------------------------------
+// one pair of staged elements (row, col), (row, col + 1), col even, rounded to TF32
+__device__ __forceinline__ void stage_pair(uint8_t* dst, int row, int col, float v0, float v1) {
+  *reinterpret_cast<float2*>(dst + (col >> 5) * CHUNK + sw_off(row, col & 31)) = make_float2(round_tf32_rn(v0), round_tf32_rn(v1));
+}
+
+// out[row0 .., col0 ..] += a [64 x D] accumulator (the element's previous value added last)
+template <int D>
+__device__ __forceinline__ void add_tile(float* out, const float* acc, size_t row0, int col0, int C, int w, int g, int t) {
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    float* row = out + (row0 + 16 * w + g + 8 * i) * (size_t)C + col0 + 2 * t;
+#pragma unroll
+    for (int jb = 0; jb < D / 8; ++jb) {
+      float2* p = reinterpret_cast<float2*>(row + 8 * jb);
+      const float2 o = *p;
+      *p = make_float2(acc[4 * jb + 2 * i] + o.x, acc[4 * jb + 2 * i + 1] + o.y);
+    }
+  }
+}
+
+constexpr int VJP_ROW_ST = 2;
+
+template <int D>
+struct VjpRowCfg {
+  static constexpr int TILE = T * D * 4;
+  static constexpr int OFF_Q = 0, OFF_DO = TILE, OFF_A = 2 * TILE;   // this CTA's query tile of Q, dO and A
+  static constexpr int OFF_P = 3 * TILE;                            // staged P
+  static constexpr int OFF_RING = OFF_P + PT_BYTES;                 // VJP_ROW_ST x (K, V, Bk [64 keys x D], Cv^T [D x 64 keys])
+  static constexpr int STAGE = 4 * TILE;
+  static constexpr int OFF_BARS = OFF_RING + VJP_ROW_ST * STAGE;
+  static constexpr int SMEM = OFF_BARS + (int)sizeof(Bars) + 1024;
+};
+
+template <int D>
+__global__ void __launch_bounds__(BWD_THREADS, 1)
+self_attn_vjp_rows_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
+                          const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmdO,
+                          const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmBk,
+                          const __grid_constant__ CUtensorMap tmCvt, const float* __restrict__ lse, const float* __restrict__ delta,
+                          float* __restrict__ rr, float* __restrict__ tt, float* __restrict__ gdO, int n, int C, float sl2, float scale) {
+  using CF = VjpRowCfg<D>;
+  constexpr int ST = VJP_ROW_ST;
+  extern __shared__ __align__(1024) uint8_t smem_raw[];
+  uint8_t* smem = align1024(smem_raw);
+  const uint32_t s_base = smem_u32(smem);
+  Bars* bars = reinterpret_cast<Bars*>(smem + CF::OFF_BARS);
+  const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;
+  const int qt = blockIdx.x, j = blockIdx.y, b = blockIdx.z, h = C / D, ntiles = n / T;
+  if (threadIdx.x == 128) {
+    prefetch_tmap(&tmQ); prefetch_tmap(&tmK); prefetch_tmap(&tmV); prefetch_tmap(&tmdO); prefetch_tmap(&tmA); prefetch_tmap(&tmBk);
+    prefetch_tmap(&tmCvt);
+    for (int i = 0; i < ST; ++i) { mbar_init(smem_u32(&bars->full[i]), 1); mbar_init(smem_u32(&bars->empty[i]), 1); }
+    mbar_init(smem_u32(&bars->once), 1);
+    fence_barrier_init();
+  }
+  __syncthreads();
+
+  if (warp == 4) {
+    if (lane == 0) {
+      const uint32_t qb = smem_u32(&bars->once);
+      mbar_expect_tx(qb, (uint32_t)(3 * CF::TILE));
+#pragma unroll
+      for (int c = 0; c < D / 32; ++c) {
+        tma_load_2d(s_base + CF::OFF_Q + c * CHUNK, &tmQ, qb, j * D + c * 32, b * n + qt * T);
+        tma_load_2d(s_base + CF::OFF_DO + c * CHUNK, &tmdO, qb, j * D + c * 32, b * n + qt * T);
+        tma_load_2d(s_base + CF::OFF_A + c * CHUNK, &tmA, qb, j * D + c * 32, b * n + qt * T);
+      }
+      for (int kt = 0; kt < ntiles; ++kt) {
+        const int st = kt % ST;
+        mbar_wait(smem_u32(&bars->empty[st]), ((kt / ST) & 1) ^ 1);
+        const uint32_t fb = smem_u32(&bars->full[st]), dst = s_base + CF::OFF_RING + st * CF::STAGE;
+        mbar_expect_tx(fb, (uint32_t)CF::STAGE);
+#pragma unroll
+        for (int c = 0; c < D / 32; ++c) {
+          tma_load_2d(dst + c * CHUNK, &tmK, fb, j * D + c * 32, b * n + kt * T);
+          tma_load_2d(dst + CF::TILE + c * CHUNK, &tmV, fb, j * D + c * 32, b * n + kt * T);
+          tma_load_2d(dst + 2 * CF::TILE + c * CHUNK, &tmBk, fb, j * D + c * 32, b * n + kt * T);
+        }
+#pragma unroll
+        for (int c = 0; c < 2; ++c) tma_load_2d(dst + 3 * CF::TILE + c * D * 128, &tmCvt, fb, kt * T + c * 32, b * C + j * D);
+      }
+    }
+    return;
+  }
+
+  const int w = warp, g = lane >> 2, t = lane & 3;
+  const uint32_t sQ = s_base + CF::OFF_Q, sdO = s_base + CF::OFF_DO, sA = s_base + CF::OFF_A, sP = s_base + CF::OFF_P;
+  float L[2], Dl[2], rs[2] = {0.f, 0.f}, us[2] = {0.f, 0.f};
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    const size_t r = ((size_t)b * h + j) * n + qt * T + 16 * w + g + 8 * i;
+    L[i] = __ldg(lse + r);
+    Dl[i] = __ldg(delta + r);
+  }
+  float pc[D / 2];
+#pragma unroll
+  for (int i = 0; i < D / 2; ++i) pc[i] = 0.f;
+  mbar_wait(smem_u32(&bars->once), 0);
+  for (int kt = 0; kt < ntiles; ++kt) {
+    const int st = kt % ST;
+    mbar_wait(smem_u32(&bars->full[st]), (kt / ST) & 1);
+    const uint32_t sK = s_base + CF::OFF_RING + st * CF::STAGE, sV = sK + CF::TILE, sBk = sK + 2 * CF::TILE, sCvt = sK + 3 * CF::TILE;
+    float s[32], dp[32], gs[32];
+    wgmma_fence();
+    gemm<64, D>(s, sQ, sK, false);                          // S = Q K^T
+    gemm<64, D>(dp, sdO, sV, false);                        // dP = dO V^T
+    gemm<64, D>(gs, sA, sK, false);                         // GdS / s = A K^T + Q Bk^T
+    gemm<64, D>(gs, sQ, sBk, true);
+    wgmma_commit();
+    wgmma_wait<0>();
+    fence_regs<32>(s); fence_regs<32>(dp); fence_regs<32>(gs);
+#pragma unroll
+    for (int jb = 0; jb < 8; ++jb)
+#pragma unroll
+      for (int i = 0; i < 2; ++i)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int x = 4 * jb + 2 * i + e;
+          const float p = exp2f(__fmul_rn(s[x], sl2) - L[i]);
+          const float pg = p * (gs[x] * scale);
+          rs[i] += pg;
+          us[i] += pg * dp[x];
+          s[x] = p;
+        }
+    stage_tile(smem + CF::OFF_P, s, w, g, t);
+    fence_proxy_async();
+    named_bar_sync(1, 128);
+    wgmma_fence();
+    gemm<D, 64>(pc, sP, sCvt, true);                        // PC += P Cv
+    wgmma_commit();
+    wgmma_wait<0>();
+    fence_regs<D / 2>(pc);
+    named_bar_sync(1, 128);
+    if (w == 0 && lane == 0) mbar_arrive(smem_u32(&bars->empty[st]));
+  }
+  const uint8_t* pdO = smem + CF::OFF_DO;
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    const int row = 16 * w + g + 8 * i;
+    float dot = 0.f;                                        // dO . PC over this thread's columns, in column order
+#pragma unroll
+    for (int jb = 0; jb < D / 8; ++jb)
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const int col = 8 * jb + 2 * t + e;
+        dot = fmaf(*reinterpret_cast<const float*>(pdO + (col >> 5) * CHUNK + sw_off(row, col & 31)), pc[4 * jb + 2 * i + e], dot);
+      }
+    float R = rs[i], U = us[i];
+    R += __shfl_xor_sync(0xffffffffu, R, 1); R += __shfl_xor_sync(0xffffffffu, R, 2);
+    U += __shfl_xor_sync(0xffffffffu, U, 1); U += __shfl_xor_sync(0xffffffffu, U, 2);
+    dot += __shfl_xor_sync(0xffffffffu, dot, 1); dot += __shfl_xor_sync(0xffffffffu, dot, 2);
+    if (t == 0) {
+      const size_t r = ((size_t)b * h + j) * n + qt * T + row;
+      rr[r] = R;
+      tt[r] = (U - 2.f * Dl[i] * R) + dot;
+    }
+  }
+  store_tile<D>(gdO, pc, (size_t)b * n + qt * T, j * D, C, w, g, t, 1.f, 1.f);
+}
+
+template <int D>
+struct VjpQCfg {
+  static constexpr int ST = D == 32 ? 2 : 1;
+  static constexpr int TILE = T * D * 4;
+  static constexpr int OFF_Q = 0, OFF_DO = TILE, OFF_A = 2 * TILE;   // this CTA's query tile of Q, dO and A
+  static constexpr int OFF_DS = 3 * TILE, OFF_GS = OFF_DS + PT_BYTES, OFF_GDP = OFF_GS + PT_BYTES;   // staged dS, GS, GdP
+  static constexpr int OFF_RING = OFF_GDP + PT_BYTES;     // ST x (K, V, Bk, Cv [64 keys x D], K^T, Bk^T, V^T [D x 64 keys])
+  static constexpr int STAGE = 7 * TILE;
+  static constexpr int OFF_BARS = OFF_RING + ST * STAGE;
+  static constexpr int SMEM = OFF_BARS + (int)sizeof(Bars) + 1024;
+};
+
+template <int D>
+__global__ void __launch_bounds__(BWD_THREADS, 1)
+self_attn_vjp_q_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
+                       const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmdO,
+                       const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmBk,
+                       const __grid_constant__ CUtensorMap tmCv, const __grid_constant__ CUtensorMap tmKt,
+                       const __grid_constant__ CUtensorMap tmBkt, const __grid_constant__ CUtensorMap tmVt, const float* __restrict__ lse,
+                       const float* __restrict__ delta, const float* __restrict__ rr, const float* __restrict__ tt, float* __restrict__ gQ,
+                       float* __restrict__ gdO, int n, int C, float sl2, float scale) {
+  using CF = VjpQCfg<D>;
+  constexpr int ST = CF::ST;
+  extern __shared__ __align__(1024) uint8_t smem_raw[];
+  uint8_t* smem = align1024(smem_raw);
+  const uint32_t s_base = smem_u32(smem);
+  Bars* bars = reinterpret_cast<Bars*>(smem + CF::OFF_BARS);
+  const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;
+  const int qt = blockIdx.x, j = blockIdx.y, b = blockIdx.z, h = C / D, ntiles = n / T;
+  if (threadIdx.x == 128) {
+    prefetch_tmap(&tmQ); prefetch_tmap(&tmK); prefetch_tmap(&tmV); prefetch_tmap(&tmdO); prefetch_tmap(&tmA); prefetch_tmap(&tmBk);
+    prefetch_tmap(&tmCv); prefetch_tmap(&tmKt); prefetch_tmap(&tmBkt); prefetch_tmap(&tmVt);
+    for (int i = 0; i < ST; ++i) { mbar_init(smem_u32(&bars->full[i]), 1); mbar_init(smem_u32(&bars->empty[i]), 1); }
+    mbar_init(smem_u32(&bars->once), 1);
+    fence_barrier_init();
+  }
+  __syncthreads();
+
+  if (warp == 4) {
+    if (lane == 0) {
+      const uint32_t qb = smem_u32(&bars->once);
+      mbar_expect_tx(qb, (uint32_t)(3 * CF::TILE));
+#pragma unroll
+      for (int c = 0; c < D / 32; ++c) {
+        tma_load_2d(s_base + CF::OFF_Q + c * CHUNK, &tmQ, qb, j * D + c * 32, b * n + qt * T);
+        tma_load_2d(s_base + CF::OFF_DO + c * CHUNK, &tmdO, qb, j * D + c * 32, b * n + qt * T);
+        tma_load_2d(s_base + CF::OFF_A + c * CHUNK, &tmA, qb, j * D + c * 32, b * n + qt * T);
+      }
+      for (int kt = 0; kt < ntiles; ++kt) {
+        const int st = kt % ST;
+        mbar_wait(smem_u32(&bars->empty[st]), ((kt / ST) & 1) ^ 1);
+        const uint32_t fb = smem_u32(&bars->full[st]), dst = s_base + CF::OFF_RING + st * CF::STAGE;
+        mbar_expect_tx(fb, (uint32_t)CF::STAGE);
+#pragma unroll
+        for (int c = 0; c < D / 32; ++c) {
+          tma_load_2d(dst + c * CHUNK, &tmK, fb, j * D + c * 32, b * n + kt * T);
+          tma_load_2d(dst + CF::TILE + c * CHUNK, &tmV, fb, j * D + c * 32, b * n + kt * T);
+          tma_load_2d(dst + 2 * CF::TILE + c * CHUNK, &tmBk, fb, j * D + c * 32, b * n + kt * T);
+          tma_load_2d(dst + 3 * CF::TILE + c * CHUNK, &tmCv, fb, j * D + c * 32, b * n + kt * T);
+        }
+#pragma unroll
+        for (int c = 0; c < 2; ++c) {
+          tma_load_2d(dst + 4 * CF::TILE + c * D * 128, &tmKt, fb, kt * T + c * 32, b * C + j * D);
+          tma_load_2d(dst + 5 * CF::TILE + c * D * 128, &tmBkt, fb, kt * T + c * 32, b * C + j * D);
+          tma_load_2d(dst + 6 * CF::TILE + c * D * 128, &tmVt, fb, kt * T + c * 32, b * C + j * D);
+        }
+      }
+    }
+    return;
+  }
+
+  const int w = warp, g = lane >> 2, t = lane & 3;
+  const uint32_t sQ = s_base + CF::OFF_Q, sdO = s_base + CF::OFF_DO, sA = s_base + CF::OFF_A;
+  const uint32_t sdS = s_base + CF::OFF_DS, sGS = s_base + CF::OFF_GS, sGdP = s_base + CF::OFF_GDP;
+  float L[2], Dl[2], R[2], Tr[2];
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    const size_t r = ((size_t)b * h + j) * n + qt * T + 16 * w + g + 8 * i;
+    L[i] = __ldg(lse + r);
+    Dl[i] = __ldg(delta + r);
+    R[i] = __ldg(rr + r);
+    Tr[i] = __ldg(tt + r);
+  }
+  float gq[D / 2], gdo[D / 2];
+#pragma unroll
+  for (int i = 0; i < D / 2; ++i) { gq[i] = 0.f; gdo[i] = 0.f; }
+  mbar_wait(smem_u32(&bars->once), 0);
+  for (int kt = 0; kt < ntiles; ++kt) {
+    const int st = kt % ST;
+    mbar_wait(smem_u32(&bars->full[st]), (kt / ST) & 1);
+    const uint32_t sK = s_base + CF::OFF_RING + st * CF::STAGE, sV = sK + CF::TILE, sBk = sK + 2 * CF::TILE, sCv = sK + 3 * CF::TILE;
+    const uint32_t sKt = sK + 4 * CF::TILE, sBkt = sK + 5 * CF::TILE, sVt = sK + 6 * CF::TILE;
+    float s[32], dp[32], gp[32];
+    wgmma_fence();
+    gemm<64, D>(s, sQ, sK, false);                          // S = Q K^T
+    gemm<64, D>(dp, sdO, sV, false);                        // dP = dO V^T
+    gemm<64, D>(gp, sA, sK, false);                         // GdS / s = A K^T + Q Bk^T
+    gemm<64, D>(gp, sQ, sBk, true);
+    wgmma_commit();
+    wgmma_wait<0>();
+    fence_regs<32>(s); fence_regs<32>(dp); fence_regs<32>(gp);
+#pragma unroll
+    for (int jb = 0; jb < 8; ++jb)
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        float gdp[2];
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int x = 4 * jb + 2 * i + e;
+          const float p = exp2f(__fmul_rn(s[x], sl2) - L[i]);
+          const float dpm = dp[x] - Dl[i], gds = gp[x] * scale;
+          gdp[e] = p * (gds - R[i]);                                     // GdP
+          gp[x] = gds * dpm - R[i] * dp[x];                              // GP, before dO Cv^T
+          dp[x] = p * dpm;                                               // dS
+          s[x] = p;
+        }
+        stage_pair(smem + CF::OFF_GDP, 16 * w + g + 8 * i, 8 * jb + 2 * t, gdp[0], gdp[1]);
+      }
+    stage_tile(smem + CF::OFF_DS, dp, w, g, t);
+    wgmma_fence();
+    gemm<64, D>(gp, sdO, sCv, true);                        // GP += dO Cv^T
+    wgmma_commit();
+    wgmma_wait<0>();
+    fence_regs<32>(gp);
+#pragma unroll
+    for (int x = 0; x < 32; ++x) gp[x] = s[x] * (gp[x] - Tr[(x >> 1) & 1]);   // GS
+    stage_tile(smem + CF::OFF_GS, gp, w, g, t);
+    fence_proxy_async();
+    named_bar_sync(1, 128);
+    wgmma_fence();
+    gemm<D, 64>(gq, sdS, sBkt, true);                       // gQ / s += dS Bk + GS K
+    gemm<D, 64>(gq, sGS, sKt, true);
+    gemm<D, 64>(gdo, sGdP, sVt, true);                      // gdO += GdP V
+    wgmma_commit();
+    wgmma_wait<0>();
+    fence_regs<D / 2>(gq); fence_regs<D / 2>(gdo);
+    named_bar_sync(1, 128);
+    if (w == 0 && lane == 0) mbar_arrive(smem_u32(&bars->empty[st]));
+  }
+  store_tile<D>(gQ, gq, (size_t)b * n + qt * T, j * D, C, w, g, t, scale, scale);
+  add_tile<D>(gdO, gdo, (size_t)b * n + qt * T, j * D, C, w, g, t);
+}
+
+template <int D>
+struct VjpKvCfg {
+  static constexpr int ST = D == 32 ? 2 : 1;
+  static constexpr int TILE = T * D * 4;
+  static constexpr int OFF_K = 0, OFF_V = TILE, OFF_BK = 2 * TILE, OFF_CV = 3 * TILE;   // this CTA's key tile of K, V, Bk, Cv
+  static constexpr int OFF_DST = 4 * TILE, OFF_GST = OFF_DST + PT_BYTES, OFF_GDPT = OFF_GST + PT_BYTES;   // staged dS^T, GS^T, GdP^T
+  static constexpr int OFF_RING = OFF_GDPT + PT_BYTES;    // ST x (Q, dO, A [64 q x D], Q^T, A^T, dO^T [D x 64 q], lse, Delta, r, t [64])
+  static constexpr int STAGE_TX = 6 * TILE + 4 * T * 4;
+  static constexpr int STAGE = 6 * TILE + 1024;
+  static constexpr int OFF_BARS = OFF_RING + ST * STAGE;
+  static constexpr int SMEM = OFF_BARS + (int)sizeof(Bars) + 1024;
+};
+
+template <int D>
+__global__ void __launch_bounds__(BWD_THREADS, 1)
+self_attn_vjp_kv_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
+                        const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmdO,
+                        const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmBk,
+                        const __grid_constant__ CUtensorMap tmCv, const __grid_constant__ CUtensorMap tmQt,
+                        const __grid_constant__ CUtensorMap tmAt, const __grid_constant__ CUtensorMap tmdOt, const float* __restrict__ lse,
+                        const float* __restrict__ delta, const float* __restrict__ rr, const float* __restrict__ tt, float* __restrict__ gK,
+                        float* __restrict__ gV, int n, int C, float sl2, float scale) {
+  using CF = VjpKvCfg<D>;
+  constexpr int ST = CF::ST;
+  extern __shared__ __align__(1024) uint8_t smem_raw[];
+  uint8_t* smem = align1024(smem_raw);
+  const uint32_t s_base = smem_u32(smem);
+  Bars* bars = reinterpret_cast<Bars*>(smem + CF::OFF_BARS);
+  const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;
+  const int kt = blockIdx.x, j = blockIdx.y, b = blockIdx.z, h = C / D, ntiles = n / T;
+  if (threadIdx.x == 128) {
+    prefetch_tmap(&tmQ); prefetch_tmap(&tmK); prefetch_tmap(&tmV); prefetch_tmap(&tmdO); prefetch_tmap(&tmA); prefetch_tmap(&tmBk);
+    prefetch_tmap(&tmCv); prefetch_tmap(&tmQt); prefetch_tmap(&tmAt); prefetch_tmap(&tmdOt);
+    for (int i = 0; i < ST; ++i) { mbar_init(smem_u32(&bars->full[i]), 1); mbar_init(smem_u32(&bars->empty[i]), 1); }
+    mbar_init(smem_u32(&bars->once), 1);
+    fence_barrier_init();
+  }
+  __syncthreads();
+  const size_t bj = ((size_t)b * h + j) * n;
+
+  if (warp == 4) {
+    if (lane == 0) {
+      const uint32_t kb = smem_u32(&bars->once);
+      mbar_expect_tx(kb, (uint32_t)(4 * CF::TILE));
+#pragma unroll
+      for (int c = 0; c < D / 32; ++c) {
+        tma_load_2d(s_base + CF::OFF_K + c * CHUNK, &tmK, kb, j * D + c * 32, b * n + kt * T);
+        tma_load_2d(s_base + CF::OFF_V + c * CHUNK, &tmV, kb, j * D + c * 32, b * n + kt * T);
+        tma_load_2d(s_base + CF::OFF_BK + c * CHUNK, &tmBk, kb, j * D + c * 32, b * n + kt * T);
+        tma_load_2d(s_base + CF::OFF_CV + c * CHUNK, &tmCv, kb, j * D + c * 32, b * n + kt * T);
+      }
+      for (int qt = 0; qt < ntiles; ++qt) {
+        const int st = qt % ST;
+        mbar_wait(smem_u32(&bars->empty[st]), ((qt / ST) & 1) ^ 1);
+        const uint32_t fb = smem_u32(&bars->full[st]), dst = s_base + CF::OFF_RING + st * CF::STAGE;
+        mbar_expect_tx(fb, (uint32_t)CF::STAGE_TX);
+#pragma unroll
+        for (int c = 0; c < D / 32; ++c) {
+          tma_load_2d(dst + c * CHUNK, &tmQ, fb, j * D + c * 32, b * n + qt * T);
+          tma_load_2d(dst + CF::TILE + c * CHUNK, &tmdO, fb, j * D + c * 32, b * n + qt * T);
+          tma_load_2d(dst + 2 * CF::TILE + c * CHUNK, &tmA, fb, j * D + c * 32, b * n + qt * T);
+        }
+#pragma unroll
+        for (int c = 0; c < 2; ++c) {
+          tma_load_2d(dst + 3 * CF::TILE + c * D * 128, &tmQt, fb, qt * T + c * 32, b * C + j * D);
+          tma_load_2d(dst + 4 * CF::TILE + c * D * 128, &tmAt, fb, qt * T + c * 32, b * C + j * D);
+          tma_load_2d(dst + 5 * CF::TILE + c * D * 128, &tmdOt, fb, qt * T + c * 32, b * C + j * D);
+        }
+        bulk_load_1d(dst + 6 * CF::TILE, lse + bj + qt * T, T * 4, fb);
+        bulk_load_1d(dst + 6 * CF::TILE + T * 4, delta + bj + qt * T, T * 4, fb);
+        bulk_load_1d(dst + 6 * CF::TILE + 2 * T * 4, rr + bj + qt * T, T * 4, fb);
+        bulk_load_1d(dst + 6 * CF::TILE + 3 * T * 4, tt + bj + qt * T, T * 4, fb);
+      }
+    }
+    return;
+  }
+
+  const int w = warp, g = lane >> 2, t = lane & 3;
+  const uint32_t sK = s_base + CF::OFF_K, sV = s_base + CF::OFF_V, sBk = s_base + CF::OFF_BK, sCv = s_base + CF::OFF_CV;
+  const uint32_t sdSt = s_base + CF::OFF_DST, sGSt = s_base + CF::OFF_GST, sGdPt = s_base + CF::OFF_GDPT;
+  float gk[D / 2], gv[D / 2];
+#pragma unroll
+  for (int i = 0; i < D / 2; ++i) { gk[i] = 0.f; gv[i] = 0.f; }
+  mbar_wait(smem_u32(&bars->once), 0);
+  for (int qt = 0; qt < ntiles; ++qt) {
+    const int st = qt % ST;
+    mbar_wait(smem_u32(&bars->full[st]), (qt / ST) & 1);
+    const uint32_t sQ = s_base + CF::OFF_RING + st * CF::STAGE, sdO = sQ + CF::TILE, sA = sQ + 2 * CF::TILE;
+    const uint32_t sQt = sQ + 3 * CF::TILE, sAt = sQ + 4 * CF::TILE, sdOt = sQ + 5 * CF::TILE;
+    const float* lse_s = reinterpret_cast<const float*>(smem + CF::OFF_RING + st * CF::STAGE + 6 * CF::TILE);
+    const float *delta_s = lse_s + T, *r_s = lse_s + 2 * T, *t_s = lse_s + 3 * T;
+    float s[32], dp[32], gp[32];
+    wgmma_fence();
+    gemm<64, D>(s, sK, sQ, false);                          // S^T [key, query] = K Q^T
+    gemm<64, D>(dp, sV, sdO, false);                        // dP^T = V dO^T
+    gemm<64, D>(gp, sK, sA, false);                         // GdS^T / s = K A^T + Bk Q^T
+    gemm<64, D>(gp, sBk, sQ, true);
+    wgmma_commit();
+    wgmma_wait<0>();
+    fence_regs<32>(s); fence_regs<32>(dp); fence_regs<32>(gp);
+#pragma unroll
+    for (int jb = 0; jb < 8; ++jb)
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        float gdp[2];
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int x = 4 * jb + 2 * i + e, q = 8 * jb + 2 * t + e;
+          const float Dl = delta_s[q], R = r_s[q];
+          const float p = exp2f(__fmul_rn(s[x], sl2) - lse_s[q]);
+          const float dpm = dp[x] - Dl, gds = gp[x] * scale;
+          gdp[e] = p * (gds - R);                                        // GdP^T
+          gp[x] = gds * dpm - R * dp[x];                                 // GP^T, before (dO Cv^T)^T
+          dp[x] = p * dpm;                                               // dS^T
+          s[x] = p;
+        }
+        stage_pair(smem + CF::OFF_GDPT, 16 * w + g + 8 * i, 8 * jb + 2 * t, gdp[0], gdp[1]);
+      }
+    stage_tile(smem + CF::OFF_DST, dp, w, g, t);
+    wgmma_fence();
+    gemm<64, D>(gp, sCv, sdO, true);                        // GP^T += Cv dO^T
+    wgmma_commit();
+    wgmma_wait<0>();
+    fence_regs<32>(gp);
+#pragma unroll
+    for (int jb = 0; jb < 8; ++jb)
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const float Tq = t_s[8 * jb + 2 * t + e];
+#pragma unroll
+        for (int i = 0; i < 2; ++i) gp[4 * jb + 2 * i + e] = s[4 * jb + 2 * i + e] * (gp[4 * jb + 2 * i + e] - Tq);   // GS^T
+      }
+    stage_tile(smem + CF::OFF_GST, gp, w, g, t);
+    fence_proxy_async();
+    named_bar_sync(1, 128);
+    wgmma_fence();
+    gemm<D, 64>(gk, sdSt, sAt, true);                       // gK / s += dS^T A + GS^T Q
+    gemm<D, 64>(gk, sGSt, sQt, true);
+    gemm<D, 64>(gv, sGdPt, sdOt, true);                     // gV += GdP^T dO
+    wgmma_commit();
+    wgmma_wait<0>();
+    fence_regs<D / 2>(gk); fence_regs<D / 2>(gv);
+    named_bar_sync(1, 128);
+    if (w == 0 && lane == 0) mbar_arrive(smem_u32(&bars->empty[st]));
+  }
+  store_tile<D>(gK, gk, (size_t)b * n + kt * T, j * D, C, w, g, t, scale, scale);
+  store_tile<D>(gV, gv, (size_t)b * n + kt * T, j * D, C, w, g, t, 1.f, 1.f);
+}
+
+// ------------------------------------------------------------------------------------------------------------------------------
 // host side
 // ------------------------------------------------------------------------------------------------------------------------------
 static int check_args(const char* name, const void* const* ptrs, const char* const* names, int np, int B, int n, int C, int d, float scale) {
@@ -534,6 +1001,37 @@ static int launch_bwd(const float* q, const float* qt, const float* k, const flo
   return GF_OK;
 }
 
+template <int D>
+static int launch_bwd_vjp(const float* q, const float* qt, const float* k, const float* kt, const float* v, const float* vt, const float* dO,
+                          const float* dOt, const float* lse, const float* delta, const float* a, const float* at, const float* bk,
+                          const float* bkt, const float* cv, const float* cvt, float* row_r, float* row_t, float* gq, float* gk, float* gv,
+                          float* gdo, int B, int n, int C, float scale, cudaStream_t st) {
+  CUtensorMap mq, mk, mv, mdo, ma, mbk, mcv, mqt, mkt, mvt, mdot, mat, mbkt, mcvt;
+  int rc;
+  if ((rc = map_nat(&mq, q, B, n, C)) || (rc = map_nat(&mk, k, B, n, C)) || (rc = map_nat(&mv, v, B, n, C)) ||
+      (rc = map_nat(&mdo, dO, B, n, C)) || (rc = map_nat(&ma, a, B, n, C)) || (rc = map_nat(&mbk, bk, B, n, C)) ||
+      (rc = map_nat(&mcv, cv, B, n, C)) || (rc = map_tr(&mqt, qt, B, n, C, D)) || (rc = map_tr(&mkt, kt, B, n, C, D)) ||
+      (rc = map_tr(&mvt, vt, B, n, C, D)) || (rc = map_tr(&mdot, dOt, B, n, C, D)) || (rc = map_tr(&mat, at, B, n, C, D)) ||
+      (rc = map_tr(&mbkt, bkt, B, n, C, D)) || (rc = map_tr(&mcvt, cvt, B, n, C, D)))
+    return rc;
+  const dim3 grid(n / T, C / D, B);
+  const float sl2 = scale * LOG2E;
+  constexpr int smem_r = VjpRowCfg<D>::SMEM, smem_q = VjpQCfg<D>::SMEM, smem_kv = VjpKvCfg<D>::SMEM;
+  GF_CUDA_OK(cudaFuncSetAttribute(self_attn_vjp_rows_kernel<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_r));
+  self_attn_vjp_rows_kernel<D><<<grid, BWD_THREADS, smem_r, st>>>(mq, mk, mv, mdo, ma, mbk, mcvt, lse, delta, row_r, row_t, gdo, n, C,
+                                                                  sl2, scale);
+  GF_LAUNCH_OK();
+  GF_CUDA_OK(cudaFuncSetAttribute(self_attn_vjp_q_kernel<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_q));
+  self_attn_vjp_q_kernel<D><<<grid, BWD_THREADS, smem_q, st>>>(mq, mk, mv, mdo, ma, mbk, mcv, mkt, mbkt, mvt, lse, delta, row_r, row_t,
+                                                               gq, gdo, n, C, sl2, scale);
+  GF_LAUNCH_OK();
+  GF_CUDA_OK(cudaFuncSetAttribute(self_attn_vjp_kv_kernel<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_kv));
+  self_attn_vjp_kv_kernel<D><<<grid, BWD_THREADS, smem_kv, st>>>(mq, mk, mv, mdo, ma, mbk, mcv, mqt, mat, mdot, lse, delta, row_r, row_t,
+                                                                 gk, gv, n, C, sl2, scale);
+  GF_LAUNCH_OK();
+  return GF_OK;
+}
+
 }  // namespace sa
 }  // namespace gf
 
@@ -560,6 +1058,22 @@ int gf_self_attn_bwd(const float* q, const float* qt, const float* k, const floa
   if (rc != GF_OK) return rc;
   return d == 32 ? launch_bwd<32>(q, qt, k, kt, v, o, lse, dO, dOt, delta, dq, dk, dv, B, n, C, scale, (cudaStream_t)stream)
                  : launch_bwd<64>(q, qt, k, kt, v, o, lse, dO, dOt, delta, dq, dk, dv, B, n, C, scale, (cudaStream_t)stream);
+}
+
+int gf_self_attn_bwd_vjp(const float* q, const float* qt, const float* k, const float* kt, const float* v, const float* vt, const float* dO,
+                         const float* dOt, const float* lse, const float* delta, const float* a, const float* at, const float* bk,
+                         const float* bkt, const float* cv, const float* cvt, float* row_r, float* row_t, float* gq, float* gk, float* gv,
+                         float* gdo, int B, int n, int C, int d, float scale, void* stream) {
+  using namespace gf::sa;
+  const void* ptrs[] = {q, qt, k, kt, v, vt, dO, dOt, lse, delta, a, at, bk, bkt, cv, cvt, row_r, row_t, gq, gk, gv, gdo};
+  const char* names[] = {"q", "qt", "k", "kt", "v", "vt", "dO", "dOt", "lse", "delta", "a", "at", "bk", "bkt", "cv", "cvt", "row_r", "row_t",
+                         "gq", "gk", "gv", "gdo"};
+  const int rc = check_args("gf_self_attn_bwd_vjp", ptrs, names, 22, B, n, C, d, scale);
+  if (rc != GF_OK) return rc;
+  return d == 32 ? launch_bwd_vjp<32>(q, qt, k, kt, v, vt, dO, dOt, lse, delta, a, at, bk, bkt, cv, cvt, row_r, row_t, gq, gk, gv, gdo, B,
+                                      n, C, scale, (cudaStream_t)stream)
+                 : launch_bwd_vjp<64>(q, qt, k, kt, v, vt, dO, dOt, lse, delta, a, at, bk, bkt, cv, cvt, row_r, row_t, gq, gk, gv, gdo, B,
+                                      n, C, scale, (cudaStream_t)stream);
 }
 
 }  // extern "C"

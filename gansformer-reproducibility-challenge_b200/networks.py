@@ -535,14 +535,19 @@ class Generator(nn.Module):
     ``img2img = r`` (SURVEY A.4 item 18): image self-attention (``ImageSelfAttention``, with the generator's integration, norm and
     use_pos) on the output of block r, after its last synthesis layer and before its tRGB; r is a block resolution in 8 .. resolution.
     The layer has no latent input: num_ws, style mixing and the latent routing are unchanged.  0 (the default) builds exactly the
-    network without it."""
+    network without it.
+
+    ``pl_kernels=True`` runs the img2img layer's part of the path-length penalty on the double-backward kernel
+    (``ImageSelfAttention.kernel_double_backward``) instead of the torch composite, which holds n x n tensors.  It changes only that
+    layer: the bipartite attention layers run their path-length pass on kernels already.  The gradients then differ from the
+    default route by TF32 round-off."""
 
     def __init__(self, resolution: int = 256, components_num: int = 16, latent_size: int = 512, latent_dim: Optional[int] = None,
                  transformer: bool = True, g_start_res: int = 8, g_end_res: Optional[int] = None, kmeans: bool = False,
                  kmeans_iters: int = 1, iterative: bool = False, integration: str = "mul", norm: Optional[str] = "layer",
                  use_pos: bool = True, pos_dim: Optional[int] = None, num_heads: int = 1, mapping_layers: int = 8,
                  fmap_base: int = 16384, fmap_max: int = 512, exact_fp32: bool = False, ltnt2ltnt: bool = False, g_img2ltnt: bool = False,
-                 att_dp: float = 0.0, c_dim: int = 0, img2img: int = 0):
+                 att_dp: float = 0.0, c_dim: int = 0, img2img: int = 0, pl_kernels: bool = False):
         super().__init__()
         # SURVEY A.4 item 1: D = latent_size // components_num unless given
         self.latent_dim = latent_dim if latent_dim is not None else max(latent_size // max(components_num, 1), 1)
@@ -556,6 +561,8 @@ class Generator(nn.Module):
         self.synthesis = SynthesisNetwork(resolution, self.latent_dim, components_num, fmap_base=fmap_base, fmap_max=fmap_max,
                                           g_start_res=g_start_res, g_end_res=g_end_res, transformer=transformer,
                                           attn_kwargs=attn_kwargs, img2img=img2img)
+        if self.synthesis.img2img is not None:
+            self.synthesis.img2img.kernel_double_backward = bool(pl_kernels)
 
     def forward(self, z: torch.Tensor, c=None, truncation_psi: float = 1.0, noise_mode: str = "const", return_att: bool = False,
                 return_features: bool = False):

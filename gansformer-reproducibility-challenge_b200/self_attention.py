@@ -10,7 +10,10 @@ The n x n part runs on the fused kernels of csrc/gf_self_attn.cu (``gf_self_attn
 tensor in memory, deterministic backward) through one autograd Function.  The four projections and ``integrate`` are ordinary GEMM and
 elementwise work: TF32 matmuls here, true fp32 with ``exact_fp32=True``, which also runs the n x n part as the torch composite.
 A backward run with grad mode on (the generator's path-length phase, the discriminator's R1 pass) recomputes the n x n part through
-the composite with create_graph=True, as ``autograd._FusedAttention`` does.  No attention dropout, no attention map, no CPU path.
+the composite with create_graph=True, which materialises P and the n x n tensors of its own backward graph.  A layer whose
+``kernel_double_backward`` is set runs that backward on the kernels instead (``_SelfAttentionBackward``: gf_self_attn_bwd, and the
+double-backward kernel gf_self_attn_bwd_vjp as its derivative), so that every tensor it keeps is [B,n,C] or [B,h,n].  No attention
+dropout, no attention map, no CPU path.
 """
 from __future__ import annotations
 
@@ -23,7 +26,7 @@ import torch
 from torch import nn
 
 from . import _lib
-from .autograd import _alias, _e, _fp32_matmul, grid_pos_table, integrate
+from .autograd import _alias, _differentiable_twice, _e, _fp32_matmul, _zeros_if_none, grid_pos_table, integrate
 
 
 def heads_of(C: int):
@@ -75,6 +78,11 @@ def attention_fwd_native(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, head
 
 def attention_bwd_native(q, k, v, o, lse, do, heads: int):
     """gf_self_attn_bwd: -> (dq, dk, dv) [B,n,C]."""
+    return _attention_bwd(q, k, v, o, lse, do, heads)[:3]
+
+
+def _attention_bwd(q, k, v, o, lse, do, heads: int):
+    """gf_self_attn_bwd: -> (dq, dk, dv, delta), delta [B,h,n] = rowsum(dO o O), which the double backward takes."""
     B, n, C = q.shape
     d = C // heads
     qt, kt, dot = (t.transpose(1, 2).contiguous() for t in (q, k, do))
@@ -85,17 +93,35 @@ def attention_bwd_native(q, k, v, o, lse, do, heads: int):
                                                 lse.data_ptr(), do.data_ptr(), dot.data_ptr(), delta.data_ptr(), dq.data_ptr(),
                                                 dk.data_ptr(), dv.data_ptr(), B, n, C, d, 1.0 / math.sqrt(d), _stream(q)),
                    "gf_self_attn_bwd")
-    return dq, dk, dv
+    return dq, dk, dv, delta
+
+
+def attention_bwd_vjp_native(q, k, v, do, lse, delta, a, bk, cv, heads: int):
+    """gf_self_attn_bwd_vjp: the cotangents a, bk, cv of (dq, dk, dv) -> (gq, gk, gv, gdo) [B,n,C], the gradients of
+    <a, dq> + <bk, dk> + <cv, dv> with respect to q, k, v and dO."""
+    B, n, C = q.shape
+    d = C // heads
+    qt, kt, vt, dot, at, bkt, cvt = (t.transpose(1, 2).contiguous() for t in (q, k, v, do, a, bk, cv))
+    row_r, row_t = torch.empty_like(lse), torch.empty_like(lse)
+    gq, gk, gv, gdo = (torch.empty_like(q) for _ in range(4))
+    with torch.cuda.device(q.device):
+        _lib.check(_lib.load().gf_self_attn_bwd_vjp(q.data_ptr(), qt.data_ptr(), k.data_ptr(), kt.data_ptr(), v.data_ptr(), vt.data_ptr(),
+                                                    do.data_ptr(), dot.data_ptr(), lse.data_ptr(), delta.data_ptr(), a.data_ptr(),
+                                                    at.data_ptr(), bk.data_ptr(), bkt.data_ptr(), cv.data_ptr(), cvt.data_ptr(),
+                                                    row_r.data_ptr(), row_t.data_ptr(), gq.data_ptr(), gk.data_ptr(), gv.data_ptr(),
+                                                    gdo.data_ptr(), B, n, C, d, 1.0 / math.sqrt(d), _stream(q)), "gf_self_attn_bwd_vjp")
+    return gq, gk, gv, gdo
 
 
 class _SelfAttention(torch.autograd.Function):
-    """The n x n part on the kernels: forward gf_self_attn_fwd, first-order backward gf_self_attn_bwd; a backward under grad mode
-    recomputes through ``attention_composite`` with create_graph=True (no double-backward kernel)."""
+    """The n x n part on the kernels: forward gf_self_attn_fwd, first-order backward gf_self_attn_bwd.  A backward under grad mode
+    runs ``_SelfAttentionBackward`` when ``double_kernels`` is set, and otherwise recomputes through ``attention_composite`` with
+    create_graph=True."""
 
     @staticmethod
-    def forward(ctx, q, k, v, heads):
+    def forward(ctx, q, k, v, heads, double_kernels=False):
         o, lse = attention_fwd_native(q, k, v, heads)
-        ctx.heads = heads
+        ctx.heads, ctx.double_kernels = heads, double_kernels
         ctx.save_for_backward(q, k, v, o, lse)
         return o
 
@@ -103,15 +129,45 @@ class _SelfAttention(torch.autograd.Function):
     def backward(ctx, g):
         q, k, v, o, lse = ctx.saved_tensors
         if torch.is_grad_enabled():
+            if ctx.double_kernels:
+                return (*_SelfAttentionBackward.apply(q, k, v, o.detach(), lse, g.contiguous(), ctx.heads), None, None)
             qs, ks, vs = _alias(q), _alias(k), _alias(v)
             out = attention_composite(qs, ks, vs, ctx.heads)
-            return (*torch.autograd.grad(out, [qs, ks, vs], g, create_graph=True), None)
-        return (*attention_bwd_native(q, k, v, o, lse, g.contiguous(), ctx.heads), None)
+            return (*torch.autograd.grad(out, [qs, ks, vs], g, create_graph=True), None, None)
+        return (*attention_bwd_native(q, k, v, o, lse, g.contiguous(), ctx.heads), None, None)
+
+
+class _SelfAttentionBackward(torch.autograd.Function):
+    """The first-order backward as a differentiable function of (q, k, v, dO): forward gf_self_attn_bwd, backward the
+    double-backward kernel gf_self_attn_bwd_vjp.  o and lse are recomputation aids, not inputs of the function: Delta =
+    rowsum(dO o O) carries the whole dependence on O.  Saved for the second pass: q, k, v, dO, lse and Delta.  A third derivative
+    raises."""
+
+    @staticmethod
+    def forward(ctx, q, k, v, o, lse, do, heads):
+        dq, dk, dv, delta = _attention_bwd(q, k, v, o, lse, do, heads)
+        ctx.heads = heads
+        ctx.save_for_backward(q, k, v, do, lse, delta)
+        return dq, dk, dv
+
+    @staticmethod
+    @_differentiable_twice
+    def backward(ctx, ga, gb, gc):
+        q, k, v, do, lse, delta = ctx.saved_tensors
+        a, bk, cv = (_zeros_if_none(g_, t) for g_, t in ((ga, q), (gb, k), (gc, v)))
+        gq, gk, gv, gdo = attention_bwd_vjp_native(q, k, v, do, lse, delta, a, bk, cv, ctx.heads)
+        return gq, gk, gv, None, None, gdo, None
 
 
 class ImageSelfAttention(nn.Module):
     """One img2img layer: x [B,H,W,C] channels-last fp32 CUDA -> [B,H,W,C].  Parameters follow ``BipartiteAttention``'s names
-    (wq bq wk bk wv bv wo bo, wpq wpk with use_pos), [fan_in, fan_out], weights N(0, 1), biases zero."""
+    (wq bq wk bk wv bv wo bo, wpq wpk with use_pos), [fan_in, fan_out], weights N(0, 1), biases zero.
+
+    ``kernel_double_backward`` (the meaning of ``BipartiteAttention.kernel_double_backward``): a backward run with create_graph=True
+    (R1, path length) stays on the kernels, differentiated by gf_self_attn_bwd_vjp, instead of recomputing through the composite.
+    Its second-order gradients then differ from the composite route by TF32 round-off.  Off by default; ignored with exact_fp32."""
+
+    kernel_double_backward = False
 
     def __init__(self, C: int, pos_dim: int, integration: str = "mul", norm: Optional[str] = "layer", use_pos: bool = True,
                  exact_fp32: bool = False):
@@ -150,6 +206,6 @@ class ImageSelfAttention(nn.Module):
             if self.exact_fp32:
                 A = attention_composite(Q, K, V, self.heads)
             else:
-                A = _SelfAttention.apply(Q.contiguous(), K.contiguous(), V.contiguous(), self.heads)
+                A = _SelfAttention.apply(Q.contiguous(), K.contiguous(), V.contiguous(), self.heads, bool(self.kernel_double_backward))
             ctl = A @ _e(self.wo) + self.bo
         return integrate(X, ctl, self.integration, self.norm).reshape(B, H, W, C)

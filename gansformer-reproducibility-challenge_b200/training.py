@@ -165,7 +165,8 @@ class Discriminator(nn.Module):
 
     ``img2img = r`` (SURVEY A.4 item 18): image self-attention (``ImageSelfAttention``, with the discriminator's integration, norm and
     use_pos, positional width latent_dim) on the activation entering the block of input resolution r, in 8 .. resolution.  Its R1
-    pass differentiates the layer's backward through the torch composite."""
+    pass differentiates the layer's backward through the torch composite, which holds n x n tensors; with ``r1_kernels=True`` it
+    runs on the double-backward kernel instead (``ImageSelfAttention.kernel_double_backward``), which holds none."""
 
     def __init__(self, resolution: int = 256, fmap_base: int = 16384, fmap_max: int = 512, mbstd_group: int = 4,
                  transformer: bool = False, components_num: int = 16, latent_dim: int = 32, d_start_res: int = 8,
@@ -196,6 +197,7 @@ class Discriminator(nn.Module):
         if img2img:
             self.img2img = ImageSelfAttention(nf(img2img, fmap_base, fmap_max), latent_dim, integration=integration, norm=norm,
                                               use_pos=use_pos, exact_fp32=exact_fp32)
+            self.img2img.kernel_double_backward = bool(r1_kernels)
 
     def forward(self, img, c: Optional[torch.Tensor] = None):
         if self.c_dim > 0:

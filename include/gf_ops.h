@@ -195,6 +195,18 @@ int gf_self_attn_bwd(const float* q, const float* qt, const float* k, const floa
                      const float* dO, const float* dOt, float* delta, float* dq, float* dk, float* dv, int B, int n, int C, int d,
                      float scale, void* stream);
 
+/* The double backward: the vector-Jacobian product of gf_self_attn_bwd as a function (q, k, v, dO) -> (dq, dk, dv), with cotangents
+ * a of dq, bk of dk and cv of dv, all [B, n, C].  lse and delta are those of the forward and of gf_self_attn_bwd (delta carries the
+ * whole dependence on O).  Writes gq, gk, gv, gdo [B, n, C]; row_r and row_t [B, h, n] are scratch it fills with the row statistics
+ * r = rowsum(P o GdS) and t = rowsum(P o GP).  The products that contract over tokens take the per-head transposed copies qt, kt, vt,
+ * dOt, at, bkt, cvt [B, C, n].  No n x n tensor is stored; three kernels, each output element accumulated by one thread in a fixed
+ * order (no atomics), so the same bits on every call.  Enqueue only, CUDA-graph capturable; the argument rules and errors of
+ * gf_self_attn_bwd. */
+int gf_self_attn_bwd_vjp(const float* q, const float* qt, const float* k, const float* kt, const float* v, const float* vt, const float* dO,
+                         const float* dOt, const float* lse, const float* delta, const float* a, const float* at, const float* bk,
+                         const float* bkt, const float* cv, const float* cvt, float* row_r, float* row_t, float* gq, float* gk, float* gv,
+                         float* gdo, int B, int n, int C, int d, float scale, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

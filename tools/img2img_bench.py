@@ -5,7 +5,13 @@
    (S = Q K^T and P V), backward 10 B n^2 C (the five n x n products of FlashAttention-2's backward: S, dP, dV, dK, dQ; the kernels
    compute S and dP twice, once per output kernel, which is not counted) -- with the share of the H100 SXM data sheet's 495 TFLOP/s
    dense TF32.
-2. The 256^2 generator (BASELINE configs[1] shape: K = 16, batch 32) forward + backward of mean(img^2), with and without img2img=32,
+   gf_self_attn_bwd_vjp (the double backward) likewise, with 24 B n^2 C FLOPs: the twelve n x n products of its algebra (S, dP,
+   GdS over 2d, dO Cv^T, P Cv, dS Bk + GS K over 2 x 64 keys, dS^T A + GS^T Q likewise, GdP^T dO, GdP V); the kernels compute S,
+   dP, GdS and dO Cv^T again in each output kernel, which is not counted.
+2. One R1 gradient through the discriminator's img2img layer (ImageSelfAttention with C = 512, batch 32): time and peak
+   memory (torch.cuda.max_memory_allocated above the inputs) on the composite route and on the double-backward kernel, at 32^2,
+   where the composite fits; then the kernel route alone at 64^2, where one n x n fp32 tensor of the composite is 17.2 GB.
+3. The 256^2 generator (BASELINE configs[1] shape: K = 16, batch 32) forward + backward of mean(img^2), with and without img2img=32,
    alternated in the same run, min and median over repeats.
 The card name and power limit are read in the same run.
 """
@@ -58,12 +64,42 @@ def kernels(res, C, B=32, iters=20):
     bwd = lambda: _lib.check(lib.gf_self_attn_bwd(q.data_ptr(), qt.data_ptr(), k.data_ptr(), kt.data_ptr(), v.data_ptr(), o.data_ptr(),
                                                   lse.data_ptr(), do.data_ptr(), dot.data_ptr(), delta.data_ptr(), dq.data_ptr(),
                                                   dk.data_ptr(), dv.data_ptr(), B, n, C, d, scale, st), "gf_self_attn_bwd")
+    a, bk, cv = (torch.randn(B, n, C, device=dev, generator=g) for _ in range(3))
+    at, bkt, cvt = (t.transpose(1, 2).contiguous() for t in (a, bk, cv))
+    row_r, row_t = torch.empty_like(lse), torch.empty_like(lse)
+    gq, gk, gv, gdo = (torch.empty_like(q) for _ in range(4))
+    vjp = lambda: _lib.check(lib.gf_self_attn_bwd_vjp(q.data_ptr(), qt.data_ptr(), k.data_ptr(), kt.data_ptr(), v.data_ptr(), vt.data_ptr(),
+                                                      do.data_ptr(), dot.data_ptr(), lse.data_ptr(), delta.data_ptr(), a.data_ptr(),
+                                                      at.data_ptr(), bk.data_ptr(), bkt.data_ptr(), cv.data_ptr(), cvt.data_ptr(),
+                                                      row_r.data_ptr(), row_t.data_ptr(), gq.data_ptr(), gk.data_ptr(), gv.data_ptr(),
+                                                      gdo.data_ptr(), B, n, C, d, scale, st), "gf_self_attn_bwd_vjp")
     out = {}
-    for name, fn, flops in (("fwd", fwd, 4.0 * B * n * n * C), ("bwd", bwd, 10.0 * B * n * n * C)):
+    for name, fn, flops in (("fwd", fwd, 4.0 * B * n * n * C), ("bwd", bwd, 10.0 * B * n * n * C), ("bwd_vjp", vjp, 24.0 * B * n * n * C)):
         ms = timed(fn, iters)
         tf = flops / ms / 1e9
         out[name] = {"ms": round(ms, 3), "TFLOP_s": round(tf, 1), "share_of_495": round(tf / TF32_PEAK, 3)}
     return out
+
+
+def r1_layer(res, kernel, C=512, B=32, iters=3):
+    """One R1 gradient through ImageSelfAttention(C) on x [B, res, res, C]: ms per gradient and the peak memory above the inputs."""
+    torch.manual_seed(0)
+    m = gf.ImageSelfAttention(C, 32).to(dev)
+    m.kernel_double_backward = kernel
+    x = torch.randn(B, res, res, C, device=dev)
+
+    def r1():
+        xs = x.detach().requires_grad_(True)
+        (gx,) = torch.autograd.grad(m(xs).sum(), xs, create_graph=True)
+        torch.autograd.grad(gx.square().sum(), [xs, *m.parameters()])
+
+    r1()
+    torch.cuda.synchronize()
+    torch.cuda.reset_peak_memory_stats(dev)
+    base = torch.cuda.memory_allocated(dev)
+    ms = timed(r1, iters, warmup=1)
+    peak = torch.cuda.max_memory_allocated(dev) - base
+    return {"ms": round(ms, 2), "peak_GiB": round(peak / 2 ** 30, 2)}
 
 
 def generator_steps(repeats=5, iters=3, B=32):
@@ -90,6 +126,8 @@ def main():
     res = {"card": card(), "kernels": {}}
     for r, C in ((32, 512), (64, 256)):
         res["kernels"][f"{r}^2 C={C} h={C // 64} B=32"] = kernels(r, C)
+    res["r1_d_layer_C512_B32"] = {"32^2 composite": r1_layer(32, False), "32^2 kernels": r1_layer(32, True),
+                                  "64^2 kernels": r1_layer(64, True)}
     res["generator_256_fwd_bwd_B32"] = generator_steps()
     print(json.dumps(res))
 
