@@ -676,6 +676,38 @@ class Trainer:
             stats.augment_p = float(self.augment_p)
         return stats
 
+    def _snapshot(self, device) -> tuple:
+        """Clones of everything ``_step_tensors`` writes: the parameters and buffers of G, D and G_ema, both Adams' states, pl_mean,
+        the ADA tensors, the attention-dropout state and the RNG state of ``device``.  For ``_restore``."""
+        live = [t for m in (self.G, self.D, self.G_ema) for t in (*m.parameters(), *m.buffers())]
+        live += [t for t in (self.pl_mean, self.augment_p, self.ada_stats, self.ada_steps) if t is not None]
+        cuda = torch.device(device).type == "cuda"
+        if cuda:
+            from .attention import dropout_state
+            live.append(dropout_state(device))
+        adam = [{p: {k: v.clone() for k, v in s.items()} for p, s in opt.state.items()} for opt in (self.opt_g, self.opt_d)]
+        rng = torch.cuda.get_rng_state(device) if cuda else torch.get_rng_state()
+        return [(t, t.detach().clone()) for t in live], adam, rng
+
+    def _restore(self, snap: tuple, device) -> None:
+        """Copies a ``_snapshot`` back in place (captured graphs keep pointers: no tensor is replaced).  An Adam state created since
+        the snapshot is zeroed, which is how a fresh Adam starts, and kept, so that a capture finds it instead of creating it."""
+        live, adam, rng = snap
+        with torch.no_grad():
+            for t, saved in live:
+                t.copy_(saved)
+            for opt, states in zip((self.opt_g, self.opt_d), adam):
+                for p, s in opt.state.items():
+                    for k, v in s.items():
+                        if p in states:
+                            v.copy_(states[p][k])
+                        else:
+                            v.zero_()
+        if torch.device(device).type == "cuda":
+            torch.cuda.set_rng_state(rng, device)
+        else:
+            torch.set_rng_state(rng)
+
     def step(self, z: torch.Tensor, reals: torch.Tensor, gen_c: Optional[torch.Tensor] = None,
              real_c: Optional[torch.Tensor] = None) -> StepStats:
         """gen_c [B, c_dim]: the labels of the fakes (one per z); real_c: those of the reals.  Required iff c_dim > 0."""
@@ -692,8 +724,9 @@ class Trainer:
                      real_c: Optional[torch.Tensor] = None) -> StepStats:
         """The same step replayed from a CUDA graph (one graph per combination of the lazy R1 term and the lazy path-length
         phase that occurs, at most three with the default intervals): the eager step is bound by the host launching ~5000 small
-        kernels.  Shapes are fixed by the first call; the first calls warm up eagerly.  The labels, like z and reals, go through
-        static buffers."""
+        kernels.  Shapes are fixed by the first call.  Before it captures, the first call runs the step eagerly once per graph
+        (cuDNN autotuning, workspaces), then puts back everything those runs wrote (``_snapshot``, ``_restore``), so that it takes
+        one step like every later call.  The labels, like z and reals, go through static buffers."""
         from . import attention as _att, networks as _nets
         cfg = self.cfg
         gen_c, real_c = self._labels(z, reals, gen_c, real_c)
@@ -714,7 +747,7 @@ class Trainer:
             if gen_c is not None:
                 st["gen_c"], st["real_c"] = gen_c.clone(), real_c.clone()
             lab = dict(gen_c=st["gen_c"], real_c=st["real_c"])
-            ada = [t.clone() for t in (self.augment_p, self.ada_stats, self.ada_steps) if t is not None]
+            snap = self._snapshot(z.device)
             side = torch.cuda.Stream(device=z.device)                 # warm-up off the capture stream: cuDNN autotune, workspaces
             side.wait_stream(torch.cuda.current_stream(z.device))
             with torch.cuda.stream(side):
@@ -723,8 +756,8 @@ class Trainer:
                 if cfg.pl_weight > 0:
                     self._step_tensors(st["z"], st["reals"], False, do_pl=True, **lab)
             torch.cuda.current_stream(z.device).wait_stream(side)
-            for t, saved in zip([t for t in (self.augment_p, self.ada_stats, self.ada_steps) if t is not None], ada):
-                t.copy_(saved)                                        # the warm-up steps do not count towards the ADA schedule
+            self._restore(snap, z.device)                             # the warm-up steps leave no trace: the first call is one step
+            del snap
             torch.cuda.synchronize(z.device)
         st["z"].copy_(z); st["reals"].copy_(reals)
         if gen_c is not None:

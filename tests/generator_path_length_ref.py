@@ -39,7 +39,8 @@ def synthesis_forward(sd: Dict[str, torch.Tensor], ws: torch.Tensor, *, resoluti
                       integration="mul", norm="layer", duplex=False, use_pos=True, num_heads=1, g_start_res: int = 8,
                       g_end_res: Optional[int] = None, noise_mode: str = "const", img2ltnt: bool = False,
                       att_mults: Optional[List[Optional[torch.Tensor]]] = None,
-                      lrelu_pos: Optional[List[Optional[torch.Tensor]]] = None, img2img: int = 0) -> torch.Tensor:
+                      lrelu_pos: Optional[List[Optional[torch.Tensor]]] = None, img2img: int = 0,
+                      layer_pos: Optional[List[torch.Tensor]] = None) -> torch.Tensor:
     """G_synthesis of ``generator_forward`` from the dlatents ws [B, k+1, D], differentiable (``sd`` and ``ws`` used as given), for
     the path-length penalty's gradients.  att_mults: per attention layer (in order), the attention-dropout multipliers [B, H*W, k]
     (oracle/philox.py) or None -- the training-mode forward of a generator with att_dp > 0.  One k-means iteration, no carried
@@ -47,7 +48,8 @@ def synthesis_forward(sd: Dict[str, torch.Tensor], ws: torch.Tensor, *, resoluti
     True, 0.2 elsewhere) instead of the sign of the fp64 pre-activation: the branch another evaluation took, so that both compare
     derivatives of the same piece of a function that is not differentiable at its kinks.  img2img = r: the image self-attention layer
     (``oracle.self_attention.self_attention_layer``) on the output of block r, before its tRGB, as in
-    ``tests.img2img_ref.generator_forward``.  -> img [B, 3, R, R]."""
+    ``tests.img2img_ref.generator_forward``.  layer_pos: the same choice for every synthesis layer (in order), attention or not; it
+    takes precedence over lrelu_pos.  -> img [B, 3, R, R]."""
     k = components_num
     g_end_res = resolution if g_end_res is None else g_end_res
     B = ws.shape[0]
@@ -76,6 +78,8 @@ def synthesis_forward(sd: Dict[str, torch.Tensor], ws: torch.Tensor, *, resoluti
             elif noise_mode != "none":
                 raise ValueError("the oracle supports noise_mode 'const' or 'none' (random noise is not reproducible)")
             x = x + sd[pre + ".bias"][None, :, None, None]
+            if layer_pos is not None:
+                pos = layer_pos[li - 1]
             x = (F.leaky_relu(x, 0.2) if pos is None else torch.where(pos, x, 0.2 * x)) * SQRT2
         if res == img2img:
             x = self_attention_layer(x, _img2img_weights(sd, "synthesis.img2img."), integration=integration, norm=norm,
